@@ -30,14 +30,10 @@ extern "C" {
 const char* b200orb_last_error(void);   /* thread-local message of the last failing call */
 int b200orb_device_count(void);         /* number of CUDA devices visible (0 if none / no driver) */
 const char* b200orb_version(void);
-/* Bit mask of the round-2 kernel formulations in force (default 3; environment B200ORB_EXPERIMENTAL overrides it, 0 = the
- * first formulations, kept for A/B): bit 0 k_orient_desc2, bit 1 second FAST tile staging.  Results never depend on it. */
-int b200orb_experimental(void);
-/* Launch-shape tuning of the extractor (process-wide; results never depend on it): FAST cells per CTA (1, 2, 4, 8) and the
- * quad-tree's register budget (2, 3 or 4 CTAs per SM); exp_mask as above.  Negative arguments keep the current value.
- * Environment at load: B200ORB_EXPERIMENTAL, B200ORB_FAST_WPC, B200ORB_QT_MINB. */
+/* Read-only report of the extractor kernels this build runs (fixed at compile time; NULL pointers are skipped):
+ * exp_mask = 3 (the orientation + descriptor formulation, bit 0, and the four-row FAST tile staging, bit 1),
+ * fast_wpc = FAST cells per CTA (8), qt_minblocks = the quad-tree's register budget in CTAs per SM (4). */
 int b200orb_get_tuning(int* exp_mask, int* fast_wpc, int* qt_minblocks);
-int b200orb_set_tuning(int exp_mask, int fast_wpc, int qt_minblocks);
 
 /* ------------------------------------------------------------------------------------------------
  * ORB extractor  --  ORB_SLAM2::ORBextractor (include/ORBextractor.h:41-118, src/ORBextractor.cc)

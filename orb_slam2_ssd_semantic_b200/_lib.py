@@ -22,7 +22,7 @@ _lib = None
 
 # every symbol include/b200orb.h declares that is implemented so far (tests check the .so exports them)
 EXPORTS = [
-    "b200orb_last_error", "b200orb_device_count", "b200orb_version", "b200orb_experimental", "b200orb_get_tuning", "b200orb_set_tuning",
+    "b200orb_last_error", "b200orb_device_count", "b200orb_version", "b200orb_get_tuning",
     "orbx_create", "orbx_destroy", "orbx_max_keypoints", "orbx_extract", "orbx_extract_batch",
     "orbx_extract_batch_device", "orbx_device_results", "orbx_sync", "orbx_stream", "orbx_level_dims",
     "orbx_get_level", "orbx_scale_tables", "orbx_candidates_per_level", "orbx_launch_count",
@@ -59,9 +59,7 @@ def lib() -> C.CDLL:
     L.b200orb_last_error.restype = C.c_char_p
     L.b200orb_version.restype = C.c_char_p
     L.b200orb_device_count.restype = i
-    L.b200orb_experimental.restype = i
     L.b200orb_get_tuning.argtypes = [C.POINTER(i), C.POINTER(i), C.POINTER(i)]
-    L.b200orb_set_tuning.argtypes = [i, i, i]
     L.orbx_create.argtypes = [C.POINTER(OrbxParams), i, C.POINTER(vp)]
     L.orbx_destroy.argtypes = [vp]
     L.orbx_destroy.restype = None

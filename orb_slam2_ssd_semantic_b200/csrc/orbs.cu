@@ -290,9 +290,7 @@ static int orbs_after_select(void* ctx, int f0, int F) {
   B200_CUDA(cudaEventRecord(h->sel_ev, ex->stream));
   B200_CUDA(cudaStreamWaitEvent(h->gather_stream, h->sel_ev, 0));
   const long long items = (long long)F * h->cap;
-  int ctas = DEPTH_PF_CTAS;
-  if (const char* e = getenv("B200ORB_PF_CTAS")) ctas = std::max(1, atoi(e));   // tuning knob (see k_depth_prefetch)
-  const int pf_grid = (int)std::min<long long>(ctas, (items + DEPTH_PF_THREADS - 1) / DEPTH_PF_THREADS);
+  const int pf_grid = (int)std::min<long long>(DEPTH_PF_CTAS, (items + DEPTH_PF_THREADS - 1) / DEPTH_PF_THREADS);
   k_depth_prefetch<<<pf_grid, DEPTH_PF_THREADS, 0, h->gather_stream>>>(ex->ltab, ex->d_sel, ex->d_selcnt, ex->sel_per_frame, h->cap,
                                                                        h->sparse_d16, h->rows, h->cols, f0, F, h->d_kpd16);
   ++h->launches;

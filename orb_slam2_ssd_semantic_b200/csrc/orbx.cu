@@ -39,34 +39,13 @@ static const signed char kPatternHost[1024] = {
 #include "../../include/orb_pattern_31.inc"
 };
 
-// Kernel selection.  `exp_mask` switches the formulations added in round 2 (bit 0 = k_orient_desc2, bit 1 = second tile
-// staging of k_fast_cells; the first ones stay available for A/B); `fast_wpc` (FAST cells
-// = warps per CTA: 1, 2, 4, 8) and `qt_minb` (quad-tree register budget for 2, 3 or 4 CTAs per SM) only change launch
-// shapes.  Defaults below; the environment (B200ORB_EXPERIMENTAL, B200ORB_FAST_WPC, B200ORB_QT_MINB) overrides them at
-// load, b200orb_set_tuning() at run time (tools/tune_extractor.py); b200orb_experimental() / b200orb_get_tuning() report.
-// Defaults, measured on an H100 SXM (80 GB HBM3, 400 W power limit): every setting is byte-identical to (0, 8, 2)
-// (tools/tune_extractor.py 96 2000); per 96-frame batch k_orient_desc2 takes the orientation stage from 0.228 to 0.209 ms,
-// the second tile staging FAST from 0.441 to 0.438 ms, and the FAST CTA size moves the stage by under 1 % (the suite's 8
-// stays).  The quad-tree alone is fastest at 2 CTAs per SM (0.34 ms; 0.42 / 0.47 ms capped for 3 / 4, which spill on
-// sm_90a), but in bench.py, with two batches and the mapper in flight, 2 CTAs per SM gave 46.7 k `value` / 38.4-40.2 k
-// `e2e` frames/s against 44.5-44.6 k / 41.4-41.8 k for 4 (3: 45.0-45.1 k / 40.9-41.3 k): 4 stays, the one setting that
-// slows neither number.  B200ORB_EXPERIMENTAL=0 B200ORB_QT_MINB=2 restores round 1's kernels.
-constexpr int kExperimentalDefault = 3, kFastWpcDefault = 8, kQtMinbDefault = 4;
-constexpr int EXP_ORIENT2 = 1, EXP_FAST_STAGE2 = 2;
-struct Tuning { int exp_mask, fast_wpc, qt_minb; };
-static inline bool valid_wpc(int v) { return v == 1 || v == 2 || v == 4 || v == 8; }
-static inline bool valid_minb(int v) { return v >= 2 && v <= 4; }
-static Tuning& tuning() {
-  static Tuning t = [] {
-    Tuning d{kExperimentalDefault, kFastWpcDefault, kQtMinbDefault};
-    if (const char* e = getenv("B200ORB_EXPERIMENTAL")) d.exp_mask = atoi(e);
-    if (const char* e = getenv("B200ORB_FAST_WPC")) { const int v = atoi(e); if (valid_wpc(v)) d.fast_wpc = v; }
-    if (const char* e = getenv("B200ORB_QT_MINB")) { const int v = atoi(e); if (valid_minb(v)) d.qt_minb = v; }
-    return d;
-  }();
-  return t;
-}
-static inline int experimental_mask() { return tuning().exp_mask; }
+// One formulation per stage, each chosen on an H100 SXM (80 GB HBM3, 400 W power limit) with 96-frame batches of 2000
+// features, all giving identical bytes: k_orient_desc's formulation takes the orientation stage from 0.228 to 0.209 ms
+// per batch against one warp per keypoint; staging up to four FAST tile rows per warp step and clearing the score map
+// with 128-bit stores takes FAST from 0.441 to 0.438 ms against two rows and 32-bit stores; FAST CTAs of 1, 2 or 4
+// cells instead of FAST_WARPS = 8 move that stage by under 1 %.  The quad-tree's register budget is explained at
+// k_quadtree.  What the host still selects follows from the input: the FAST tile pitch from the cell size, and k_resize
+// instead of k_resize_g for scale factors above 2.
 
 static inline int cv_round_f(float v) { return (int)lrintf(v); }
 static inline int cv_round_d(double v) { return (int)lrint(v); }
@@ -112,10 +91,8 @@ int orbx::init(const OrbxParams& p, int dev) {
     ++v0;
   }
   B200_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  for (v = 1; v <= HALF_PATCH_SIZE; ++v)   // k_orient_desc2 tests the circular mask as v <= vmax(|u|)
+  for (v = 1; v <= HALF_PATCH_SIZE; ++v)   // k_orient_desc tests the circular mask as v <= vmax(|u|)
     if (otab.umax[v] > otab.umax[v - 1]) { set_error("umax table is not non-increasing"); return B200ORB_EINVAL; }
-  B200_CUDA(cudaMalloc(&d_pattern, 1024));
-  B200_CUDA(cudaMemcpyAsync(d_pattern, kPatternHost, 1024, cudaMemcpyHostToDevice, stream));
   float patf[1024];
   for (int i = 0; i < 1024; ++i) patf[i] = (float)kPatternHost[i];
   B200_CUDA(cudaMalloc(&d_patf, sizeof(patf)));
@@ -140,7 +117,6 @@ void orbx::free_geometry() {
 orbx::~orbx() {
   DeviceGuard g(device);
   free_geometry();
-  if (d_pattern) cudaFree(d_pattern);
   if (d_patf) cudaFree(d_patf);
   if (stream) cudaStreamDestroy(stream);
 }
@@ -273,10 +249,8 @@ int orbx::ensure_geometry(int r, int c, int F) {
     fast_rows_max = rhm;
     fast_smem = (size_t)FAST_WARPS * (2 * rhm * fast_tp + 2 * FAST_QLEN + 2 * fast_clist_cap);
     if (fast_smem > 48 * 1024) {
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_BIG, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_SMALL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_BIG, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_SMALL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
+      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
+      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_SMALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
     }
   }
   slots_per_frame = align_up(slots, 4);
@@ -285,30 +259,7 @@ int orbx::ensure_geometry(int r, int c, int F) {
   qt_cap = align_up(qcap, 8);
   qt_smem = qt_smem_bytes(qt_cap);
   if (qt_smem > 100 * 1024) { set_error("nfeatures too large for the quad-tree kernel's shared memory"); return B200ORB_EINVAL; }
-  {
-    // Levels are launched in three groups with decreasing shared-memory budgets (level 0-1: 200 KB, 2-4: 112 KB,
-    // 5+: 56 KB) so that small levels keep several CTAs per SM; a (frame, level) whose candidates exceed its group's
-    // budget uses the global scratch instead (same code path, generic pointers).
-    // Staging the candidates in shared memory cuts a CTA's latency but costs CTA-level concurrency (1 CTA/SM for the
-    // big levels, split launches for the small ones).  All levels run in ONE launch on the L2-resident scratch
-    // (budget 0); the staging path stays available behind the budgets.
-    const int bounds[4] = {0, nl, nl, nl};
-    const size_t budget[3] = {0, 0, 0};
-    size_t mx = 0;
-    for (int g = 0; g < 3; ++g) {
-      qt_group_lb[g] = bounds[g]; qt_group_le[g] = bounds[g + 1];
-      int worst = 0;
-      for (int l = bounds[g]; l < bounds[g + 1]; ++l) worst = std::max(worst, ltab.slot_begin[l + 1] - ltab.slot_begin[l]);
-      size_t room = budget[g] > qt_smem ? budget[g] - qt_smem : 0;
-      int kcap = (int)std::min<size_t>((size_t)worst, room / 8) & ~3;
-      qt_group_kcap[g] = std::max(kcap, 0);
-      qt_group_smem[g] = qt_smem + (size_t)qt_group_kcap[g] * 8;
-      mx = std::max(mx, qt_group_smem[g]);
-    }
-    B200_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mx));
-    B200_CUDA(cudaFuncSetAttribute(k_quadtree_o3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mx));
-    B200_CUDA(cudaFuncSetAttribute(k_quadtree_o4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mx));
-  }
+  B200_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qt_smem));
 
   rows = r; cols = c; maxF = keepF;
   const size_t Fz = (size_t)maxF;
@@ -362,11 +313,23 @@ int orbx::ensure_geometry(int r, int c, int F) {
   return B200ORB_OK;
 }
 
-// Enqueue the whole extractor for F frames whose level 0 is (d_l0, pitch0, fstride0) on `stream`.
 // Enqueue the whole extractor for frames [f0, f0+F) of the batch; d_l0 = level 0 of frame f0.  Ranges of one batch may be
 // enqueued one after another (the host path uploads and extracts in chunks so that PCIe and the SMs overlap).
 int orbx::run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0) {
   const int nl = prm.nlevels;
+  B200_CHECK(prof_begin(F));
+  // The kernels read level rows as aligned 32-bit words.  A level 0 that is not 4-byte aligned (pointer, pitch or frame
+  // stride) is copied into the internal plane first.  The ranges of one batch all take the same branch: their pointers
+  // differ by multiples of fstride0.
+  if ((((uintptr_t)d_l0) | (uintptr_t)pitch0 | fstride0) & 3) {
+    uint8_t* staged = d_raw + (size_t)f0 * frame_bytes;
+    for (int f = 0; f < F; ++f)
+      B200_CUDA(cudaMemcpy2DAsync(staged + (size_t)f * frame_bytes, lpitch[0], d_l0 + (size_t)f * fstride0, pitch0, lw[0],
+                                  lh[0], cudaMemcpyDeviceToDevice, stream));
+    d_l0 = staged;
+    pitch0 = lpitch[0];
+    fstride0 = frame_bytes;
+  }
   // frame-range views: every per-frame array is addressed as base + frame * stride inside the kernels
   PyrView rawv = this->rawv, blurv = this->blurv;
   for (int l = 1; l < nl; ++l) rawv.p[l] += (size_t)f0 * rawv.fstride[l];
@@ -387,13 +350,11 @@ int orbx::run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0) {
   OrbxKeyPoint* d_kps = this->d_kps + (size_t)f0 * cap;
   uint8_t* d_desc = this->d_desc + (size_t)f0 * cap * 32;
   int* d_n = this->d_n + f0;
-  B200_CHECK(prof_begin(F));
   // K1 pyramid
   for (int l = 1; l < nl; ++l) {
     dim3 blk(32, 8), grd((lw[l] + 127) / 128, (lh[l] + 7) / 8, F);
-    // k_resize_g needs aligned source rows and 4 outputs within an 8-byte source window (scale factor <= 2)
-    const bool src_aligned = prm.scale_factor <= 2.0f && (((uintptr_t)rawv.p[l - 1]) & 3) == 0 && (rawv.pitch[l - 1] & 3) == 0 && (rawv.fstride[l - 1] & 3) == 0;
-    if (src_aligned && resize_group_ok)
+    // k_resize_g needs the 4 outputs of a thread within an 8-byte source window (scale factor <= 2)
+    if (resize_group_ok)
       k_resize_g<<<grd, blk, 0, stream>>>(rawv.p[l - 1], rawv.pitch[l - 1], rawv.fstride[l - 1], lh[l - 1], rawv.p[l],
                                          rawv.pitch[l], rawv.fstride[l], lw[l], lh[l], d_xg + xg_off[l], d_yt + yt_off[l]);
     else
@@ -404,69 +365,27 @@ int orbx::run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0) {
   }
   B200_CHECK(prof_mark(ST_RESIZE + 1));
   // K2 FAST cells
-  int fast_aligned = 1;   // every level's rows 4-byte aligned? (internal planes always are; level 0 may alias a caller buffer)
-  for (int l = 0; l < nl; ++l)
-    if ((((uintptr_t)rawv.p[l]) & 3) || (rawv.pitch[l] & 3) || (rawv.fstride[l] & 3)) fast_aligned = 0;
-  if (fast_aligned && (experimental_mask() & EXP_FAST_STAGE2)) fast_aligned |= 2;   // second tile staging of k_fast_cells
-  {
-    // cells (= warps) per CTA: smaller CTAs (same kernel: a warp never synchronises with its neighbours) shorten the
-    // tail a CTA spends waiting for its slowest cell
-    const int wpc = tuning().fast_wpc;
-    const dim3 grd((ncells + wpc - 1) / wpc, F);
-    const size_t fast_smem_l = fast_smem / FAST_WARPS * wpc;
-    // B200ORB_FAST_SWEEP=1 selects the one-pixel-per-lane sweep (development A/B switch; default: the word sweep)
-    static const bool sweep4 = [] { const char* e = getenv("B200ORB_FAST_SWEEP"); return !(e && e[0] == '1'); }();
-#define B200_FAST_LAUNCH(TPV, S4)                                                                                          \
-  k_fast_cells<TPV, S4><<<grd, wpc * 32, fast_smem_l, stream>>>(rawv, d_cells, ncells, slots_per_frame, prm.ini_th_fast,   \
-                                                                  prm.min_th_fast, d_cand, d_cellcnt, fast_aligned,        \
-                                                                  fast_rows_max, fast_clist_cap)
-    if (fast_tp == FAST_TP_SMALL) { if (sweep4) B200_FAST_LAUNCH(FAST_TP_SMALL, true); else B200_FAST_LAUNCH(FAST_TP_SMALL, false); }
-    else { if (sweep4) B200_FAST_LAUNCH(FAST_TP_BIG, true); else B200_FAST_LAUNCH(FAST_TP_BIG, false); }
-#undef B200_FAST_LAUNCH
-  }
+  auto* fast_kernel = fast_tp == FAST_TP_SMALL ? k_fast_cells<FAST_TP_SMALL> : k_fast_cells<FAST_TP_BIG>;
+  fast_kernel<<<dim3((ncells + FAST_WARPS - 1) / FAST_WARPS, F), FAST_THREADS, fast_smem, stream>>>(
+      rawv, d_cells, ncells, slots_per_frame, prm.ini_th_fast, prm.min_th_fast, d_cand, d_cellcnt, fast_rows_max,
+      fast_clist_cap);
   ++launches;
   B200_CHECK(prof_mark(ST_FAST + 1));
-  // K3 quad-tree: levels are launched in two groups so that each group's per-candidate arrays fit shared memory
-  QtScratchView qs{d_qkp, d_qnode};
-  for (int g = 0; g < 3; ++g) {
-    const int lb = qt_group_lb[g], le = qt_group_le[g];
-    if (le <= lb) continue;
-    auto* qt_kernel = tuning().qt_minb == 4 ? k_quadtree_o4 : tuning().qt_minb == 3 ? k_quadtree_o3 : k_quadtree;
-    qt_kernel<<<dim3(le - lb, F), QT_THREADS, qt_group_smem[g], stream>>>(ltab, d_cells, d_cand, d_cellcnt, ncells,
-                                                                          slots_per_frame, qs, qt_cap, d_sel, d_selcnt,
-                                                                          d_candcnt, sel_per_frame, lb, qt_group_kcap[g]);
-    ++launches;
-  }
+  // K3 quad-tree: one CTA per (level, frame)
+  k_quadtree<<<dim3(nl, F), QT_THREADS, qt_smem, stream>>>(ltab, d_cells, d_cand, d_cellcnt, ncells, slots_per_frame,
+                                                           QtScratchView{d_qkp, d_qnode}, qt_cap, d_sel, d_selcnt,
+                                                           d_candcnt, sel_per_frame);
+  ++launches;
   B200_CHECK(prof_mark(ST_QUADTREE + 1));
   if (after_select) B200_CHECK(after_select(after_select_ctx, f0, F));
-  // K4 blur: one launch over every (level, 128x35 tile, frame) when all planes are 4-byte aligned
-  {
-    bool aligned = true;
-    for (int l = 0; l < nl; ++l)
-      if ((((uintptr_t)rawv.p[l]) & 3) || (rawv.pitch[l] & 3) || (rawv.fstride[l] & 3)) aligned = false;
-    if (aligned) {
-      k_blur7_strip<<<dim3(n_blur_tiles, F), 32, 0, stream>>>(rawv, blurv, d_blur_tiles);
-      k_blur7_edges<<<dim3((n_blur_edges + 63) / 64, F), 64, 0, stream>>>(rawv, blurv, d_blur_edges, n_blur_edges);
-      launches += 2;
-    } else {
-      for (int l = 0; l < nl; ++l) {
-        dim3 grd((lw[l] + BL_TW - 1) / BL_TW, (lh[l] + BL_TH - 1) / BL_TH, F);
-        k_blur7<<<grd, 256, 0, stream>>>(rawv.p[l], rawv.pitch[l], rawv.fstride[l], blurv.p[l], blurv.pitch[l],
-                                         blurv.fstride[l], lw[l], lh[l]);
-        ++launches;
-      }
-    }
-  }
+  // K4 blur: one launch over every (level, 128x35 tile, frame), one over the border column groups
+  k_blur7_strip<<<dim3(n_blur_tiles, F), 32, 0, stream>>>(rawv, blurv, d_blur_tiles);
+  k_blur7_edges<<<dim3((n_blur_edges + 63) / 64, F), 64, 0, stream>>>(rawv, blurv, d_blur_edges, n_blur_edges);
+  launches += 2;
   B200_CHECK(prof_mark(ST_BLUR + 1));
   // K5 orientation + descriptors
-  {
-    if (!(experimental_mask() & EXP_ORIENT2))
-      k_orient_desc<<<dim3((cap + OD_WARPS - 1) / OD_WARPS, F), OD_WARPS * 32, 0, stream>>>(
-          ltab, otab, rawv, blurv, d_pattern, d_sel, d_selcnt, sel_per_frame, d_kps, d_desc, d_n, cap);
-    else
-      k_orient_desc2<<<dim3((cap + OD_WARPS * OD_KPW - 1) / (OD_WARPS * OD_KPW), F), OD_WARPS * 32, 0, stream>>>(
-          ltab, otab, rawv, blurv, d_patf, d_sel, d_selcnt, sel_per_frame, d_kps, d_desc, d_n, cap);
-  }
+  k_orient_desc<<<dim3((cap + OD_WARPS * OD_KPW - 1) / (OD_WARPS * OD_KPW), F), OD_WARPS * 32, 0, stream>>>(
+      ltab, otab, rawv, blurv, d_patf, d_sel, d_selcnt, sel_per_frame, d_kps, d_desc, d_n, cap);
   ++launches;
   B200_CHECK(prof_mark(ST_ORIENT_DESC + 1));
   B200_CUDA(cudaGetLastError());
@@ -516,26 +435,12 @@ int orbx::ensure_tmp(size_t bytes) {
 // =====================================================================================================
 extern "C" {
 
-int b200orb_experimental(void) { return experimental_mask(); }
 int b200orb_get_tuning(int* exp_mask, int* fast_wpc, int* qt_minblocks) {
-  const Tuning& t = tuning();
-  if (exp_mask) *exp_mask = t.exp_mask;
-  if (fast_wpc) *fast_wpc = t.fast_wpc;
-  if (qt_minblocks) *qt_minblocks = t.qt_minb;
+  if (exp_mask) *exp_mask = 3;   // both bits: k_orient_desc's formulation (1) and the four-row FAST tile staging (2)
+  if (fast_wpc) *fast_wpc = FAST_WARPS;
+  if (qt_minblocks) *qt_minblocks = QT_MIN_CTAS;
   return B200ORB_OK;
 }
-int b200orb_set_tuning(int exp_mask, int fast_wpc, int qt_minblocks) {   // negative = keep
-  if ((fast_wpc >= 0 && !valid_wpc(fast_wpc)) || (qt_minblocks >= 0 && !valid_minb(qt_minblocks))) {
-    set_error("bad tuning value");
-    return B200ORB_EINVAL;
-  }
-  Tuning& t = tuning();
-  if (exp_mask >= 0) t.exp_mask = exp_mask;
-  if (fast_wpc >= 0) t.fast_wpc = fast_wpc;
-  if (qt_minblocks >= 0) t.qt_minb = qt_minblocks;
-  return B200ORB_OK;
-}
-
 
 const char* b200orb_last_error(void) { return g_err; }
 const char* b200orb_version(void) { return "b200orb 0.1 (sm_90a)"; }

@@ -26,8 +26,7 @@ struct orbx {
   float sf[b200::MAX_LEVELS], invsf[b200::MAX_LEVELS], sigma2[b200::MAX_LEVELS], invsigma2[b200::MAX_LEVELS];
   int nfeat[b200::MAX_LEVELS];
   b200::OrientTab otab{};
-  signed char* d_pattern = nullptr;
-  float4* d_patf = nullptr;   // the 256 tests as float4 (x0, y0, x1, y1), for k_orient_desc2
+  float4* d_patf = nullptr;   // the 256 tests as float4 (x0, y0, x1, y1), for k_orient_desc
   // geometry-dependent state
   int rows = 0, cols = 0, maxF = 0, lastF = 0;
   int lw[b200::MAX_LEVELS], lh[b200::MAX_LEVELS], lpitch[b200::MAX_LEVELS];
@@ -40,8 +39,6 @@ struct orbx {
   size_t qt_smem = 0;
   int fast_tp = 0, fast_rows_max = 0, fast_clist_cap = 0;
   size_t fast_smem = 0;
-  int qt_group_lb[3] = {0, 0, 0}, qt_group_le[3] = {0, 0, 0}, qt_group_kcap[3] = {0, 0, 0};
-  size_t qt_group_smem[3] = {0, 0, 0};
   uint8_t *d_raw = nullptr, *d_blur = nullptr;
   b200::CellDesc* d_cells = nullptr;
   unsigned* d_cand = nullptr;
@@ -58,7 +55,7 @@ struct orbx {
   int4* d_xg = nullptr;   // per 4-output group: {first source word, 8*byte phase, PRMT selectors, -} + 4 coefficient pairs
   b200::BlurTile* d_blur_tiles = nullptr;
   b200::BlurEdge* d_blur_edges = nullptr;
-  int n_blur_tiles = 0, n_blur_edges = 0, blur_edge_rows = 0;
+  int n_blur_tiles = 0, n_blur_edges = 0;
   void* d_tmp = nullptr;
   size_t tmp_bytes = 0;
   void* h_stage = nullptr;

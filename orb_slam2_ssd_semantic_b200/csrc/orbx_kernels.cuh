@@ -4,7 +4,8 @@
 //   pyramid   level l : F planes of h_l rows x pitch_l bytes (pitch_l = w_l rounded up to 16), no border --
 //             the 19-px REFLECT_101 frame of ComputePyramid (:1125-1142) is never read by anything that
 //             feeds operator()'s outputs (SURVEY App. B.12); orbx_get_level synthesises it on read-back.
-//             Level 0 aliases the caller's device buffer when the batch is already resident.
+//             Level 0 aliases the caller's device buffer when the batch is already resident and its rows are
+//             4-byte aligned; otherwise it is staged into the internal plane, so every plane's rows are aligned.
 //   blurred   same layout, GaussianBlur 7x7 sigma 2 of every level (:1094-1095)
 //   cand      per frame: one fixed segment per FAST cell (worst-case capacity ceil(iw/2)*ceil(ih/2): strict
 //             3x3 NMS forbids 8-adjacent survivors), packed u32 x:12 | y:12 | response:8, row-major in cell
@@ -181,27 +182,26 @@ __device__ __forceinline__ int fast_m_exact(const uint8_t* c) {
   return max(0, max((int)(m0 & 0xffffu), (int)(m0 >> 16)) - 256);
 }
 
-// One WARP per (cell, frame), 8 cells per CTA, no block-level synchronisation.  Per-warp shared memory: the ROI and
-// its score map interleaved row by row (pixel row y at y*2*TP, its score row at y*2*TP + TP, so one base register and
-// compile-time offsets address both), a 64-entry ring of pixels that passed the compass test, and the list of corners.
-//   sweep   lane = column, row by row (a second sweep covers cells wider than 32): compass test; failing pixels get
-//           score 0, passing ones are queued;
+// One WARP per (cell, frame), FAST_WARPS cells per CTA, no block-level synchronisation.  Per-warp shared memory: the ROI
+// and its score map interleaved row by row (pixel row y at y*2*TP, its score row at y*2*TP + TP, so one base register
+// and compile-time offsets address both), a ring of pixels that passed the compass test, and the list of corners.
+//   sweep   a thread owns one aligned tile word (4 pixels) of one row, several rows per warp step: compass test;
+//           passing pixels are queued;
 //   dense   whenever 32 pixels are queued, a full warp evaluates their exact m(p); corners (m > t) go to the corner
 //           list -- the queue is FIFO over a row-major sweep, so the list is row-major as well;
 //   NMS     32 corners at a time: strict 3x3 maximum, order-preserving compaction into the cell's output segment.
-// `aligned` bit 0 (host-checked): level rows are 4-byte aligned, so the ROI is fetched as aligned 32-bit words and kept
-// at the same byte phase (pixel x of the ROI sits at column (x0 & 3) + x).  Bit 1 selects the second tile staging:
-// up to four ROI rows per warp step and 128-bit stores for the score-map clear (fewer instructions for the same work).
-template <int TP, bool SWEEP4>
+// Level rows are 4-byte aligned (the host stages an unaligned level 0), so the ROI is fetched as aligned 32-bit words
+// and kept at the same byte phase (pixel x of the ROI sits at column (x0 & 3) + x).
+template <int TP>
 __global__ void __launch_bounds__(FAST_THREADS, 4) k_fast_cells(PyrView pyr, const CellDesc* __restrict__ cells,
                                                                 int ncells, int slots_per_frame, int ini_th,
                                                                 int min_th, unsigned* __restrict__ cand,
-                                                                int* __restrict__ cellcnt, int aligned, int rows_max,
+                                                                int* __restrict__ cellcnt, int rows_max,
                                                                 int clist_cap) {
   extern __shared__ __align__(16) uint8_t fsm[];
   constexpr int P = 2 * TP;   // row pitch of the interleaved tile
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int cell = blockIdx.x * (blockDim.x >> 5) + w, f = blockIdx.y;   // blockDim.x / 32 cells per CTA (host: <= FAST_WARPS)
+  const int cell = blockIdx.x * FAST_WARPS + w, f = blockIdx.y;
   if (cell >= ncells) return;
   uint8_t* tile = fsm + (size_t)w * (rows_max * P + 2 * FAST_QLEN + 2 * clist_cap);
   unsigned short* queue = reinterpret_cast<unsigned short*>(tile + (size_t)rows_max * P);
@@ -209,60 +209,29 @@ __global__ void __launch_bounds__(FAST_THREADS, 4) k_fast_cells(PyrView pyr, con
   const CellDesc cd = cells[cell];
   const int l = cd.level, rw = cd.rw, rh = cd.rh;
   const int pitch = pyr.pitch[l];
-  const bool stage2 = (aligned & 2) != 0;     // host switch: second formulation of the tile staging (below)
-  aligned &= 1;
-  const int sh = aligned ? (cd.x0 & 3) : 0;   // byte phase of the ROI inside its first word
+  const int sh = cd.x0 & 3;   // byte phase of the ROI inside its first word
   {
     const uint8_t* img = pyr.p[l] + (size_t)f * pyr.fstride[l] + (size_t)cd.y0 * pitch + (cd.x0 - sh);
-    if (aligned) {
-      const int nw = (sh + rw + 3) >> 2;   // words per ROI row (<= (3 + FAST_MAX_ROI + 3) / 4 = 19)
-      if (stage2) {
-        // up to four rows per warp step: lane = r * nw + k (640x480: nw = 10 -> 3 rows, 30 lanes); no integer division
-        const int rpl = (nw <= 8) ? 4 : (nw <= 10) ? 3 : (nw <= 16) ? 2 : 1;
-        const int r0 = (lane >= nw) + (lane >= 2 * nw) + (lane >= 3 * nw), k = lane - r0 * nw;
-        if (r0 < rpl && k < nw) {
-          const unsigned* src = reinterpret_cast<const unsigned*>(img + (size_t)r0 * pitch) + k;
-          unsigned* dst = reinterpret_cast<unsigned*>(tile + r0 * P) + k;
-          const size_t sstep = (size_t)rpl * (pitch >> 2);   // level pitches are multiples of 4 on this path
-          for (int y = r0; y < rh; y += rpl, src += sstep, dst += rpl * (P / 4)) *dst = __ldg(src);
-        }
-      } else if (nw <= 16) {               // two rows per step: lanes 0-15 / 16-31
-        const int k = lane & 15, half = lane >> 4;
-        for (int y = half; y < rh; y += 2)
-          if (k < nw) reinterpret_cast<unsigned*>(tile + y * P)[k] = __ldg(reinterpret_cast<const unsigned*>(img + (size_t)y * pitch) + k);
-      } else {
-        for (int y = 0; y < rh; ++y)
-          for (int k = lane; k < nw; k += 32)
-            reinterpret_cast<unsigned*>(tile + y * P)[k] = __ldg(reinterpret_cast<const unsigned*>(img + (size_t)y * pitch) + k);
-      }
-    } else {
-      for (int y = 0; y < rh; ++y)
-        for (int x = lane; x < rw; x += 32) tile[y * P + x] = __ldg(img + (size_t)y * pitch + x);
+    const int nw = (sh + rw + 3) >> 2;   // words per ROI row (<= (3 + FAST_MAX_ROI + 3) / 4 = 19)
+    // up to four rows per warp step: lane = r * nw + k (640x480: nw = 10 -> 3 rows, 30 lanes); no integer division
+    const int rpl = (nw <= 8) ? 4 : (nw <= 10) ? 3 : (nw <= 16) ? 2 : 1;
+    const int r0 = (lane >= nw) + (lane >= 2 * nw) + (lane >= 3 * nw), k = lane - r0 * nw;
+    if (r0 < rpl && k < nw) {
+      const unsigned* src = reinterpret_cast<const unsigned*>(img + (size_t)r0 * pitch) + k;
+      unsigned* dst = reinterpret_cast<unsigned*>(tile + r0 * P) + k;
+      const size_t sstep = (size_t)rpl * (pitch >> 2);
+      for (int y = r0; y < rh; y += rpl, src += sstep, dst += rpl * (P / 4)) *dst = __ldg(src);
     }
-    if (SWEEP4 && aligned) {
-      // the word sweep only writes the scores of corners: clear every score row once (rows 2 .. rh-3 are read by the NMS)
-      if (stage2) {   // tile, P and TP are multiples of 16 bytes: 128-bit stores
-        constexpr int QPR = TP / 16;
-        for (int i = lane; i < (rh - 4) * QPR; i += 32) {
-          const int y = 2 + i / QPR, k = i - (y - 2) * QPR;
-          reinterpret_cast<uint4*>(tile + y * P + TP)[k] = make_uint4(0u, 0u, 0u, 0u);
-        }
-      } else {
-        constexpr int WPR = TP / 4;
-        for (int i = lane; i < (rh - 4) * WPR; i += 32) {
-          const int y = 2 + i / WPR, k = i - (y - 2) * WPR;
-          reinterpret_cast<unsigned*>(tile + y * P + TP)[k] = 0u;
-        }
-      }
-    } else {
-      // only the one-pixel frame around the detection range is read without being written: clear it
-      for (int i = lane; i < rw; i += 32) { tile[2 * P + TP + sh + i] = 0; tile[(rh - 3) * P + TP + sh + i] = 0; }
-      for (int i = lane; i < rh; i += 32) { tile[i * P + TP + sh + 2] = 0; tile[i * P + TP + sh + rw - 3] = 0; }
+    // the sweep only writes the scores of corners: clear every score row once (rows 2 .. rh-3 are read by the NMS);
+    // tile, P and TP are multiples of 16 bytes: 128-bit stores
+    constexpr int QPR = TP / 16;
+    for (int i = lane; i < (rh - 4) * QPR; i += 32) {
+      const int y = 2 + i / QPR, q = i - (y - 2) * QPR;
+      reinterpret_cast<uint4*>(tile + y * P + TP)[q] = make_uint4(0u, 0u, 0u, 0u);
     }
   }
   __syncwarp();
   unsigned* out = cand + (size_t)f * slots_per_frame + cd.slot_off;
-  const bool wide = rw - 6 > 32;
   const unsigned lt_mask = (1u << lane) - 1u;
   int total = 0;
   // pass 0: everything at ini_th (pixels with m <= ini_th can neither be corners nor outscore one at that threshold);
@@ -284,100 +253,66 @@ __global__ void __launch_bounds__(FAST_THREADS, 4) k_fast_cells(PyrView pyr, con
       if (cr) clist[cn + __popc(cb & lt_mask)] = (unsigned short)o;
       cn += __popc(cb);
     };
-    if (SWEEP4 && aligned) {
-      // Word sweep: a thread owns the 4 pixels of one aligned tile word (columns 4g .. 4g+3) of one row; several rows per
-      // warp step.  The compass test runs on pixel PAIRS in s16x2 lanes, bright and dark polarity in separate registers:
-      //   bright: 256 + r - c,  dark: 256 + c - r   (one IADD3 each per ring pixel and pixel pair, operands spread from the
-      //   byte lanes by one PRMT), q = min(max(v0, v8), max(v4, v12)) per polarity, hit <=> q > 256 + t in either.
-      // Queue positions are the pixels' ranks in ROW-MAJOR order (lanes are ordered (row, word); inside a word by column),
-      // so the corner list the dense phase builds stays row-major.
-      const unsigned kq = (unsigned)(0x7fff - 256 - t) * 0x10001u;
-      const int gA = (sh + 3) >> 2, gB = (sh + rw - 4) >> 2, NW = gB - gA + 1;
-      const int RPI = 32 / NW;                       // rows per warp step (NW <= 19 < 32)
-      const int rs = lane / NW, g = gA + (lane - rs * NW);
-      const int cmin = sh + 3, cmax = sh + rw - 3;   // detection columns [cmin, cmax) in tile coordinates
-      const unsigned* trow = reinterpret_cast<const unsigned*>(tile);
-      for (int y0 = 3; y0 < rh - 3; y0 += RPI) {
-        const int y = y0 + rs;
-        unsigned hits = 0;                           // bit k: pixel 4g+k of row y passed
-        if (rs < RPI && y < rh - 3) {
-          const unsigned* wr = trow + (y * P) / 4;
-          const unsigned wc = wr[g], wl = wr[max(g - 1, 0)], wn = wr[g + 1];
-          const unsigned w0 = wr[g + (3 * P) / 4], w8 = wr[g - (3 * P) / 4];
-          const unsigned w12 = __funnelshift_r(wl, wc, 8);     // bytes x-3 of the four pixels
-          const unsigned w4 = __funnelshift_r(wc, wn, 24);     // bytes x+3
+    // Word sweep: a thread owns the 4 pixels of one aligned tile word (columns 4g .. 4g+3) of one row; several rows per
+    // warp step.  The compass test is necessary for a corner at t: a 9-arc always holds one pixel of each opposite
+    // compass pair, and all its pixels lie on the same side of the centre.  It runs on pixel PAIRS in s16x2 lanes,
+    // bright and dark polarity in separate registers:
+    //   bright: 256 + r - c,  dark: 256 + c - r   (one IADD3 each per ring pixel and pixel pair, operands spread from the
+    //   byte lanes by one PRMT), q = min(max(v0, v8), max(v4, v12)) per polarity, hit <=> q > 256 + t in either.
+    // Queue positions are the pixels' ranks in ROW-MAJOR order (lanes are ordered (row, word); inside a word by column),
+    // so the corner list the dense phase builds stays row-major.
+    const unsigned kq = (unsigned)(0x7fff - 256 - t) * 0x10001u;
+    const int gA = (sh + 3) >> 2, gB = (sh + rw - 4) >> 2, NW = gB - gA + 1;
+    const int RPI = 32 / NW;                       // rows per warp step (NW <= 19 < 32)
+    const int rs = lane / NW, g = gA + (lane - rs * NW);
+    const int cmin = sh + 3, cmax = sh + rw - 3;   // detection columns [cmin, cmax) in tile coordinates
+    const unsigned* trow = reinterpret_cast<const unsigned*>(tile);
+    for (int y0 = 3; y0 < rh - 3; y0 += RPI) {
+      const int y = y0 + rs;
+      unsigned hits = 0;                           // bit k: pixel 4g+k of row y passed
+      if (rs < RPI && y < rh - 3) {
+        const unsigned* wr = trow + (y * P) / 4;
+        const unsigned wc = wr[g], wl = wr[max(g - 1, 0)], wn = wr[g + 1];
+        const unsigned w0 = wr[g + (3 * P) / 4], w8 = wr[g - (3 * P) / 4];
+        const unsigned w12 = __funnelshift_r(wl, wc, 8);     // bytes x-3 of the four pixels
+        const unsigned w4 = __funnelshift_r(wc, wn, 24);     // bytes x+3
 #pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {                     // pixel pairs (0,2) and (1,3)
-            const unsigned sel = h2 ? 0x4341u : 0x4240u;
-            const unsigned C = __byte_perm(wc, 0u, sel), R0 = __byte_perm(w0, 0u, sel), R8 = __byte_perm(w8, 0u, sel);
-            const unsigned R4 = __byte_perm(w4, 0u, sel), R12 = __byte_perm(w12, 0u, sel);
-            const unsigned cb = 0x01000100u - C, cd = 0x01000100u + C;   // halves stay in [1, 511]: no borrow / carry across
-            const unsigned qb = __vmins2(__vmaxs2(R0 + cb, R8 + cb), __vmaxs2(R4 + cb, R12 + cb));
-            const unsigned qd = __vmins2(__vmaxs2(cd - R0, cd - R8), __vmaxs2(cd - R4, cd - R12));
-            const unsigned hb = ((qb + kq) | (qd + kq)) & 0x80008000u;
-            if (hb & 0x8000u) hits |= 1u << h2;
-            if (hb & 0x80000000u) hits |= 4u << h2;
-          }
-          const int c0 = 4 * g;                                // drop the pixels outside the detection columns
-          unsigned cm = 0;
+        for (int h2 = 0; h2 < 2; ++h2) {                     // pixel pairs (0,2) and (1,3)
+          const unsigned sel = h2 ? 0x4341u : 0x4240u;
+          const unsigned C = __byte_perm(wc, 0u, sel), R0 = __byte_perm(w0, 0u, sel), R8 = __byte_perm(w8, 0u, sel);
+          const unsigned R4 = __byte_perm(w4, 0u, sel), R12 = __byte_perm(w12, 0u, sel);
+          const unsigned cb = 0x01000100u - C, cd = 0x01000100u + C;   // halves stay in [1, 511]: no borrow / carry across
+          const unsigned qb = __vmins2(__vmaxs2(R0 + cb, R8 + cb), __vmaxs2(R4 + cb, R12 + cb));
+          const unsigned qd = __vmins2(__vmaxs2(cd - R0, cd - R8), __vmaxs2(cd - R4, cd - R12));
+          const unsigned hb = ((qb + kq) | (qd + kq)) & 0x80008000u;
+          if (hb & 0x8000u) hits |= 1u << h2;
+          if (hb & 0x80000000u) hits |= 4u << h2;
+        }
+        const int c0 = 4 * g;                                // drop the pixels outside the detection columns
+        unsigned cm = 0;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) cm |= ((c0 + k >= cmin) && (c0 + k < cmax)) ? (1u << k) : 0u;
-          hits &= cm;
-        }
-        const unsigned b0 = __ballot_sync(0xffffffffu, hits & 1u), b1 = __ballot_sync(0xffffffffu, hits & 2u);
-        const unsigned b2 = __ballot_sync(0xffffffffu, hits & 4u), b3 = __ballot_sync(0xffffffffu, hits & 8u);
-        if (hits) {
-          int pos = qh + qn + __popc(b0 & lt_mask) + __popc(b1 & lt_mask) + __popc(b2 & lt_mask) + __popc(b3 & lt_mask);
-          const int o = y * P + 4 * g;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (hits & (1u << k)) { queue[pos & (FAST_QLEN - 1)] = (unsigned short)(o + k); ++pos; }
-        }
-        qn += __popc(b0) + __popc(b1) + __popc(b2) + __popc(b3);
-        while (qn >= 32) {
-          __syncwarp();
-          dense(queue[(qh + lane) & (FAST_QLEN - 1)], true);
-          qh += 32;
-          qn -= 32;
-        }
+        for (int k = 0; k < 4; ++k) cm |= ((c0 + k >= cmin) && (c0 + k < cmax)) ? (1u << k) : 0u;
+        hits &= cm;
       }
-      __syncwarp();
-      dense((lane < qn) ? queue[(qh + lane) & (FAST_QLEN - 1)] : 0, lane < qn);
-    } else {
-      // The compass test in packed form: a 9-arc always holds one pixel of each opposite compass pair, and all its
-      // pixels lie on the same side of the centre, so min(max(v0, v8), max(v4, v12)) > 256 + t in either half is
-      // necessary for a corner at t.
-      const unsigned kq = (unsigned)(0x7fff - 256 - t) * 0x10001u;
-      uint8_t* rowp = tile + 3 * P + sh + 3 + lane;
-      const int colmax = rw - 6;   // detection columns
-      for (int y = 3; y < rh - 3; ++y, rowp += P) {
+      const unsigned b0 = __ballot_sync(0xffffffffu, hits & 1u), b1 = __ballot_sync(0xffffffffu, hits & 2u);
+      const unsigned b2 = __ballot_sync(0xffffffffu, hits & 4u), b3 = __ballot_sync(0xffffffffu, hits & 8u);
+      if (hits) {
+        int pos = qh + qn + __popc(b0 & lt_mask) + __popc(b1 & lt_mask) + __popc(b2 & lt_mask) + __popc(b3 & lt_mask);
+        const int o = y * P + 4 * g;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (h == 1 && !wide) break;
-          uint8_t* cc = rowp + 32 * h;
-          bool hit = false;
-          if (lane + 32 * h < colmax) {
-            const int bias = 256 * 65537 - (int)cc[0] * 65535;
-            const unsigned v0 = (unsigned)((int)cc[3 * P] * 65535 + bias), v8 = (unsigned)((int)cc[-3 * P] * 65535 + bias);
-            const unsigned v4 = (unsigned)((int)cc[3] * 65535 + bias), v12 = (unsigned)((int)cc[-3] * 65535 + bias);
-            const unsigned qv = __vmins2(__vmaxs2(v0, v8), __vmaxs2(v4, v12));
-            hit = ((qv + kq) & 0x80008000u) != 0u;   // halves are in [1,511]: no carry between them
-            if (!hit) cc[TP] = 0;
-          }
-          const unsigned bal = __ballot_sync(0xffffffffu, hit);
-          if (hit) queue[(qh + qn + __popc(bal & lt_mask)) & (FAST_QLEN - 1)] = (unsigned short)(cc - tile);
-          qn += __popc(bal);
-          if (qn >= 32) {
-            __syncwarp();
-            dense(queue[(qh + lane) & (FAST_QLEN - 1)], true);
-            qh += 32;
-            qn -= 32;
-          }
-        }
+        for (int k = 0; k < 4; ++k)
+          if (hits & (1u << k)) { queue[pos & (FAST_QLEN - 1)] = (unsigned short)(o + k); ++pos; }
       }
-      __syncwarp();
-      dense((lane < qn) ? queue[(qh + lane) & (FAST_QLEN - 1)] : 0, lane < qn);
+      qn += __popc(b0) + __popc(b1) + __popc(b2) + __popc(b3);
+      while (qn >= 32) {
+        __syncwarp();
+        dense(queue[(qh + lane) & (FAST_QLEN - 1)], true);
+        qh += 32;
+        qn -= 32;
+      }
     }
+    __syncwarp();
+    dense((lane < qn) ? queue[(qh + lane) & (FAST_QLEN - 1)] : 0, lane < qn);
     __syncwarp();
     // NMS (strict 3x3 maximum of the scores; a neighbour that is no corner at t scores 0) over the corner list, 32
     // corners at a time, + order-preserving compaction (one ballot per batch, running offset).
@@ -477,21 +412,24 @@ __device__ int qt_scan_array(int* a, int n, int* ws) {
   return total;
 }
 
-// The body is shared by three entry points that differ only in their register budget (k_quadtree: the compiler's choice,
-// 52 registers on sm_90a -> 2 CTAs per SM; k_quadtree_o3 / _o4: capped for 3 / 4 CTAs per SM, which spills): the kernel
-// is latency-bound (barriers + L2 round trips per round), so resident CTAs are what hides it.
-__device__ __forceinline__ void quadtree_body(const LevelTab& lt, const CellDesc* __restrict__ cells,
-                                              const unsigned* __restrict__ cand,
-                                              const int* __restrict__ cellcnt, int ncells,
-                                              int slots_per_frame, QtScratchView sc, int qt_cap,
-                                              unsigned* __restrict__ sel, int* __restrict__ selcnt,
-                                              int* __restrict__ candcnt, int sel_per_frame,
-                                              int level_begin, int kp_smem_cap) {
+// Register budget: 4 CTAs per SM (the compiler's own choice is 52 registers on sm_90a, i.e. 2 CTAs per SM; the cap
+// spills a little).  The kernel is latency-bound (barriers + L2 round trips per round), so resident CTAs are what hides
+// it.  Measured on an H100 SXM (80 GB HBM3, 400 W power limit), per 96-frame batch of 2000 features alone the stage
+// takes 0.34 ms at 2 CTAs per SM and 0.42 / 0.47 ms capped for 3 / 4.  But in bench.py, with two batches and the mapper
+// in flight, 2 CTAs per SM gave 46.7 k `value` / 38.4-40.2 k `e2e` frames/s against 44.5-44.6 k / 41.4-41.8 k for 4
+// (3: 45.0-45.1 k / 40.9-41.3 k): 4 is the one budget that slows neither number.
+constexpr int QT_MIN_CTAS = 4;
+__global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab lt, const CellDesc* __restrict__ cells,
+                                                            const unsigned* __restrict__ cand,
+                                                            const int* __restrict__ cellcnt, int ncells,
+                                                            int slots_per_frame, QtScratchView sc, int qt_cap,
+                                                            unsigned* __restrict__ sel, int* __restrict__ selcnt,
+                                                            int* __restrict__ candcnt, int sel_per_frame) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int ws[33];
   __shared__ int s_coff[QT_THREADS];
   __shared__ int s_expand, s_rstar;
-  const int l = blockIdx.x + level_begin, f = blockIdx.y, tid = threadIdx.x, nthr = blockDim.x;
+  const int l = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, nthr = blockDim.x;
   const int nlev = lt.nlevels;
   const int N = lt.nfeat[l];
   QtSmem S;
@@ -512,10 +450,9 @@ __device__ __forceinline__ void quadtree_body(const LevelTab& lt, const CellDesc
   const unsigned* fcand = cand + (size_t)f * slots_per_frame;
   const int* fcnt = cellcnt + (size_t)f * ncells;
   // Per-candidate arrays (packed keypoint + node id) stay in the L2-resident global scratch: staging them in shared
-  // memory costs CTA-level concurrency and generic addressing (see the budgets in orbx.cu).
+  // memory costs CTA-level concurrency.
   unsigned* __restrict__ qkp = sc.qkp + (size_t)f * slots_per_frame + lt.slot_begin[l];
   int* __restrict__ qnode = sc.qnode + (size_t)f * slots_per_frame + lt.slot_begin[l];
-  (void)kp_smem_cap;
   // ---- gather this level's per-cell segments into one contiguous, order-preserving list -----------
   const int cb = lt.cell_begin[l], nc = lt.cell_begin[l + 1] - cb;
   int K = 0;
@@ -737,64 +674,9 @@ __device__ __forceinline__ void quadtree_body(const LevelTab& lt, const CellDesc
   if (tid == 0) selcnt[(size_t)f * nlev + l] = n;
 }
 
-#define B200_QT_ARGS LevelTab lt, const CellDesc* __restrict__ cells, const unsigned* __restrict__ cand,             \
-                     const int* __restrict__ cellcnt, int ncells, int slots_per_frame, QtScratchView sc, int qt_cap,   \
-                     unsigned* __restrict__ sel, int* __restrict__ selcnt, int* __restrict__ candcnt, int sel_per_frame, \
-                     int level_begin, int kp_smem_cap
-#define B200_QT_PASS lt, cells, cand, cellcnt, ncells, slots_per_frame, sc, qt_cap, sel, selcnt, candcnt, sel_per_frame, \
-                     level_begin, kp_smem_cap
-__global__ void __launch_bounds__(QT_THREADS) k_quadtree(B200_QT_ARGS) { quadtree_body(B200_QT_PASS); }
-__global__ void __launch_bounds__(QT_THREADS, 3) k_quadtree_o3(B200_QT_ARGS) { quadtree_body(B200_QT_PASS); }
-__global__ void __launch_bounds__(QT_THREADS, 4) k_quadtree_o4(B200_QT_ARGS) { quadtree_body(B200_QT_PASS); }
-#undef B200_QT_ARGS
-#undef B200_QT_PASS
-
-// ---------------------------------------------------------------------------------------------------
-// K4  GaussianBlur 7x7 sigma 2, BORDER_REFLECT_101 (SURVEY App. A.3; call site :1094-1095).
-//     Integer kernel [18,34,48,56,48,34,18]/256 in both passes, (v + 32768) >> 16.
-//     Tile 64x16 outputs per CTA; (64+6)x(16+6) source halo in shared memory; horizontal pass into u16.
-// ---------------------------------------------------------------------------------------------------
-constexpr int BL_TW = 64, BL_TH = 16;
-
-__device__ __forceinline__ int reflect101(int p, int n) {
-  if (n == 1) return 0;
-  while (p < 0 || p >= n) p = (p < 0) ? -p : 2 * (n - 1) - p;
-  return p;
-}
-
-__global__ void __launch_bounds__(256) k_blur7(const uint8_t* __restrict__ src, int spitch, size_t sfs,
-                                               uint8_t* __restrict__ dst, int dpitch, size_t dfs, int w, int h) {
-  __shared__ uint8_t t[(BL_TH + 6)][BL_TW + 8];
-  __shared__ unsigned short hb[(BL_TH + 6)][BL_TW];
-  const uint8_t* s = src + (size_t)blockIdx.z * sfs;
-  uint8_t* d = dst + (size_t)blockIdx.z * dfs;
-  const int x0 = blockIdx.x * BL_TW, y0 = blockIdx.y * BL_TH;
-  for (int i = threadIdx.x; i < (BL_TH + 6) * (BL_TW + 6); i += 256) {
-    const int ty = i / (BL_TW + 6), tx = i - ty * (BL_TW + 6);
-    const int sy = reflect101(y0 + ty - 3, h), sx = reflect101(x0 + tx - 3, w);
-    t[ty][tx] = s[(size_t)sy * spitch + sx];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < (BL_TH + 6) * BL_TW; i += 256) {
-    const int ty = i / BL_TW, tx = i - ty * BL_TW;
-    const uint8_t* r = &t[ty][tx];
-    hb[ty][tx] = (unsigned short)(18 * (r[0] + r[6]) + 34 * (r[1] + r[5]) + 48 * (r[2] + r[4]) + 56 * r[3]);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < BL_TH * BL_TW; i += 256) {
-    const int ty = i / BL_TW, tx = i - ty * BL_TW;
-    const int x = x0 + tx, y = y0 + ty;
-    if (x < w && y < h) {
-      const unsigned v = 18u * (hb[ty][tx] + hb[ty + 6][tx]) + 34u * (hb[ty + 1][tx] + hb[ty + 5][tx]) +
-                         48u * (hb[ty + 2][tx] + hb[ty + 4][tx]) + 56u * hb[ty + 3][tx];
-      d[(size_t)y * dpitch + x] = (uint8_t)((v + 32768u) >> 16);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------
 // K5  orientation (IC_Angle :59-88 on the raw level) + steered BRIEF (computeOrbDescriptor :92-131 on the
-//     blurred level) + final KeyPoint assembly (:846-856, :1104-1110).  One warp per keypoint.
+//     blurred level) + final KeyPoint assembly (:846-856, :1104-1110).  One warp per keypoint at a time.
 // ---------------------------------------------------------------------------------------------------
 struct OrientTab {
   int umax[HALF_PATCH_SIZE + 1];
@@ -822,91 +704,8 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {   // cv::fas
 
 constexpr int OD_WARPS = 8;
 
-__global__ void __launch_bounds__(OD_WARPS * 32) k_orient_desc(LevelTab lt, OrientTab ot, PyrView raw, PyrView blr,
-                                                               const signed char* __restrict__ pattern,
-                                                               const unsigned* __restrict__ sel,
-                                                               const int* __restrict__ selcnt, int sel_per_frame,
-                                                               OrbxKeyPoint* __restrict__ kps,
-                                                               uint8_t* __restrict__ desc, int* __restrict__ nout,
-                                                               int cap) {
-  __shared__ int spat[256];   // 512 points x (int8 x, int8 y) = 1024 B
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) spat[i] = reinterpret_cast<const int*>(pattern)[i];
-  __syncthreads();
-  const int f = blockIdx.y, lane = threadIdx.x & 31;
-  const int j = blockIdx.x * OD_WARPS + (threadIdx.x >> 5);
-  const int* sc = selcnt + (size_t)f * lt.nlevels;
-  int l = -1, idx = 0, acc = 0;
-  for (int q = 0; q < lt.nlevels; ++q) {
-    const int c = sc[q];
-    if (l < 0 && j < acc + c) { l = q; idx = j - acc; }
-    acc += c;
-  }
-  if (j == 0 && lane == 0) nout[f] = min(acc, cap);
-  if (l < 0 || j >= cap) return;
-  const unsigned pk = sel[(size_t)f * sel_per_frame + lt.sel_off[l] + idx];
-  const int x = kp_x(pk), y = kp_y(pk);
-  // ---- IC_Angle: lane <-> column u = lane-15 (31 columns), loop rows ----
-  const uint8_t* rc = raw.p[l] + (size_t)f * raw.fstride[l] + (size_t)y * raw.pitch[l] + x;
-  const int u = lane - HALF_PATCH_SIZE, au = abs(u);
-  int m10 = 0, m01 = 0;
-  if (lane < 31) {
-    const int rp = raw.pitch[l];
-    m10 = u * rc[u];
-#pragma unroll
-    for (int v = 1; v <= HALF_PATCH_SIZE; ++v) {
-      if (au <= ot.umax[v]) {
-        const int vp = rc[u + v * rp], vm = rc[u - v * rp];
-        m10 += u * (vp + vm);
-        m01 += v * (vp - vm);
-      }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    m10 += __shfl_xor_sync(0xffffffffu, m10, o);
-    m01 += __shfl_xor_sync(0xffffffffu, m01, o);
-  }
-  const float angle = fast_atan2_deg((float)m01, (float)m10);
-  // ---- steered BRIEF ----
-  const float factorPI = (float)(3.14159265358979323846 / 180.f);
-  const float ang = __fmul_rn(angle, factorPI);
-  // cos()/sin() of the reference bind to glibc's cosf/sinf, which are NOT correctly rounded: run the same algorithm
-  const float a = b200_cosf(ang), b = b200_sinf(ang);
-  const uint8_t* bc = blr.p[l] + (size_t)f * blr.fstride[l] + (size_t)y * blr.pitch[l] + x;
-  const int bp = blr.pitch[l];
-  unsigned word = 0;
-  unsigned* dout = reinterpret_cast<unsigned*>(desc + ((size_t)f * cap + j) * 32);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int pr = k * 32 + lane;                 // test index; bit pr of the descriptor
-    const int w0 = spat[pr];                       // bytes: x0,y0,x1,y1
-    const float x0 = (float)(signed char)(w0 & 0xff), y0 = (float)(signed char)((w0 >> 8) & 0xff);
-    const float x1 = (float)(signed char)((w0 >> 16) & 0xff), y1 = (float)(signed char)((w0 >> 24) & 0xff);
-    const int r0 = __float2int_rn(__fadd_rn(__fmul_rn(x0, b), __fmul_rn(y0, a)));
-    const int c0 = __float2int_rn(__fsub_rn(__fmul_rn(x0, a), __fmul_rn(y0, b)));
-    const int r1 = __float2int_rn(__fadd_rn(__fmul_rn(x1, b), __fmul_rn(y1, a)));
-    const int c1 = __float2int_rn(__fsub_rn(__fmul_rn(x1, a), __fmul_rn(y1, b)));
-    const int t0 = bc[r0 * bp + c0], t1 = bc[r1 * bp + c1];
-    const unsigned bits = __ballot_sync(0xffffffffu, t0 < t1);
-    if (lane == k) word = bits;
-  }
-  if (lane < 8) dout[lane] = word;
-  if (lane == 0) {
-    OrbxKeyPoint kp;
-    const float s = lt.sf[l];
-    kp.x = (l != 0) ? __fmul_rn((float)x, s) : (float)x;
-    kp.y = (l != 0) ? __fmul_rn((float)y, s) : (float)y;
-    kp.size = lt.kp_size[l];
-    kp.angle = angle;
-    kp.response = (float)kp_r(pk);
-    kp.octave = l;
-    kp.class_id = -1;
-    kps[(size_t)f * cap + j] = kp;
-  }
-}
-
-// K5, second formulation (bit 0 of experimental_mask() in orbx.cu, B200ORB_EXPERIMENTAL): the same arithmetic with fewer
-// instructions -- the first formulation is issue-bound, with many of its instructions on the XU pipe (I2F / F2I
+// The formulation keeps the instruction count down: the straightforward one (a warp per keypoint, the pattern as int8
+// pairs, the level found by a scan) is issue-bound, with many of its instructions on the XU pipe (I2F / F2I
 // conversions).
 //   * a warp handles KPW keypoints, so the per-CTA set-up (pattern into shared memory, level offsets) is paid once per
 //     8 * KPW keypoints instead of once per 8;
@@ -917,16 +716,15 @@ __global__ void __launch_bounds__(OD_WARPS * 32) k_orient_desc(LevelTab lt, Orie
 //     load, tests the circular mask as v <= vmax(|u|) (umax is non-increasing in v -- checked at create -- so
 //     {v : |u| <= umax[v]} is the prefix 1..vmax), and accumulates sum(vp + vm) with one 3-input add per row, the
 //     multiplication by u once at the end (exact: integers).
-// Results are identical bit for bit (integer moments; the float sequence of the steered BRIEF is unchanged).
 constexpr int OD_KPW = 4;   // keypoints per warp
 
-__global__ void __launch_bounds__(OD_WARPS * 32, 8) k_orient_desc2(LevelTab lt, OrientTab ot, PyrView raw, PyrView blr,
-                                                                const float4* __restrict__ patf /* 256 tests */,
-                                                                const unsigned* __restrict__ sel,
-                                                                const int* __restrict__ selcnt, int sel_per_frame,
-                                                                OrbxKeyPoint* __restrict__ kps,
-                                                                uint8_t* __restrict__ desc, int* __restrict__ nout,
-                                                                int cap) {
+__global__ void __launch_bounds__(OD_WARPS * 32, 8) k_orient_desc(LevelTab lt, OrientTab ot, PyrView raw, PyrView blr,
+                                                               const float4* __restrict__ patf /* 256 tests */,
+                                                               const unsigned* __restrict__ sel,
+                                                               const int* __restrict__ selcnt, int sel_per_frame,
+                                                               OrbxKeyPoint* __restrict__ kps,
+                                                               uint8_t* __restrict__ desc, int* __restrict__ nout,
+                                                               int cap) {
   __shared__ float4 spat[256];   // test pr: points 2 pr and 2 pr + 1 of the pattern, as floats
   for (int i = threadIdx.x; i < 256; i += OD_WARPS * 32) spat[i] = __ldg(patf + i);
   const int f = blockIdx.y, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -1009,14 +807,23 @@ __global__ void __launch_bounds__(OD_WARPS * 32, 8) k_orient_desc2(LevelTab lt, 
   }
 }
 
-// K4 (fast path): same arithmetic, register sliding window.  One thread owns 4 adjacent columns and walks down
-// BLS_ROWS rows of a strip.  Per row it reads the 10 source bytes as three aligned 32-bit words, builds the byte pairs
-// P_k = b[k] | b[k+2] << 16 with one funnel shift + mask each, and evaluates the horizontal pass on two pixels per
-// register (every partial sum stays below 2^16, so the halves never carry into each other).  The last 7 rows of
-// horizontal sums live in a statically rotated register ring for the vertical pass -- no shared memory, no
-// intermediate plane.  Requires 4-byte aligned rows (true for the internal planes; level 0 falls back to k_blur7 when
-// the caller's buffer is not aligned).
+// ---------------------------------------------------------------------------------------------------
+// K4  GaussianBlur 7x7 sigma 2, BORDER_REFLECT_101 (SURVEY App. A.3; call site :1094-1095).
+//     Integer kernel [18,34,48,56,48,34,18]/256 in both passes, (v + 32768) >> 16.
+//     Register sliding window: one thread owns 4 adjacent columns and walks down BLS_ROWS rows of a strip.  Per row it
+//     reads the 10 source bytes as three aligned 32-bit words, builds the byte pairs P_k = b[k] | b[k+2] << 16 with one
+//     funnel shift + mask each, and evaluates the horizontal pass on two pixels per register (every partial sum stays
+//     below 2^16, so the halves never carry into each other).  The last 7 rows of horizontal sums live in a statically
+//     rotated register ring for the vertical pass -- no shared memory, no intermediate plane.  Requires 4-byte aligned
+//     rows, which every plane has.
+// ---------------------------------------------------------------------------------------------------
 constexpr int BLS_ROWS = 35;   // multiple of 7: the ring rotation is unrolled by 7
+
+__device__ __forceinline__ int reflect101(int p, int n) {
+  if (n == 1) return 0;
+  while (p < 0 || p >= n) p = (p < 0) ? -p : 2 * (n - 1) - p;
+  return p;
+}
 
 struct HRow { unsigned h02, h13; };   // horizontal sums of pixels (0,2) and (1,3) of the thread's 4 columns
 

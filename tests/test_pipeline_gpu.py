@@ -9,10 +9,10 @@ from tests.helpers import frame_views
 pytestmark = pytest.mark.gpu
 
 
-def test_stream_batch_matches_oracle(oracle):
+def _stream_batch_matches_oracle(oracle, rows, cols):
     from orb_slam2_ssd_semantic_b200 import StreamTracker
     F = 5
-    ws = synth.WallStream(seed=1234, n=F)
+    ws = synth.WallStream(seed=1234, n=F, h=rows, w=cols)
     frames = [ws.frame(t) for t in range(F)]
     gray = np.stack([f[0] for f in frames])
     depth = np.stack([f[1] for f in frames])
@@ -30,12 +30,21 @@ def test_stream_batch_matches_oracle(oracle):
             assert nm[t] == 0 and (c2l[t, :nkp[t]] == -1).all()
         else:
             cur, last = frame_views(oracle, K, D, depth[t], T[t], prev[0], prev[1], depth[t - 1], T[t - 1],
-                                    R.mvScaleFactor, obs=1)
+                                    R.mvScaleFactor, obs=1, rows=rows, cols=cols)
             n_ref, ref = oracle.search_by_projection_last(cur, last, 15.0, False, 0.9, True)
             assert n_ref > 100
             assert nm[t] == n_ref
             assert (c2l[t, :nkp[t]] == ref).all()
         prev = (K, D)
+
+
+def test_stream_batch_matches_oracle(oracle):
+    _stream_batch_matches_oracle(oracle, 480, 640)
+
+
+def test_stream_batch_matches_oracle_kitti_width(oracle):
+    """376 x 1241 (KITTI): the tracker hands the extractor rows of 1241 bytes, which are not 4-byte aligned."""
+    _stream_batch_matches_oracle(oracle, 376, 1241)
 
 
 def test_u16_depth_path_equals_float_path():

@@ -15,8 +15,8 @@ tmp = tempfile.mkdtemp()
 subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(ROOT, "orb_slam2_ssd_semantic_b200", "libb200orb.so")], cwd=tmp, capture_output=True)
 cubin = max((f for f in os.listdir(tmp) if f.endswith(".cubin")), key=lambda f: os.path.getsize(os.path.join(tmp, f)))
 dis = subprocess.run(["nvdisasm", "-c", os.path.join(tmp, cubin)], capture_output=True, text=True).stdout.splitlines()
-kernels = [("k_fast_cells<48, true>", "k_fast_cellsILi48ELb1"), ("k_orient_desc2", "k_orient_desc2"), ("k_orient_desc", "k_orient_descENS"),
-           ("k_quadtree", "10k_quadtreeENS"), ("k_quadtree_o3", "k_quadtree_o3"), ("k_match_last_fused", "k_match_last_fused"),
+kernels = [("k_fast_cells<48>", "k_fast_cellsILi48E"), ("k_orient_desc", "k_orient_descENS"),
+           ("k_quadtree", "10k_quadtreeENS"), ("k_match_last_fused", "k_match_last_fused"),
            ("k_blur7_strip", "k_blur7_strip"), ("k_resize_g", "k_resize_g"), ("k_ocm_scan_keys", "k_ocm_scan_keys"),
            ("k_ocm_bin", "k_ocm_binE"), ("k_dynm_morph<true>", "k_dynm_morphILb1"), ("k_dynm_flow_mask", "k_dynm_flow_mask")]
 out = ["# SASS of libb200orb.so (sm_90a): `cuobjdump -xelf all` + `nvdisasm -c` of the library built from this tree by",
@@ -65,10 +65,10 @@ def excerpt(name, pat, before, after, title):
     out.append("")
 
 
-excerpt("k_fast_cells<48, true>", r"VIMNMX3\.S16x2", 22, 40,
-        "k_fast_cells<48,true>: exact FAST score of one queued pixel -- LDS.U8 ring loads, IMAD packing (bright | dark in s16x2), VIMNMX3.S16x2 min / max tree")
-excerpt("k_orient_desc2", r"LDS\.128", 4, 34,
-        "k_orient_desc2: steered BRIEF -- LDS.128 pattern fetch, FMUL / FADD / F2I rotation, IMAD + LDG.U8 gathers, VOTE")
+excerpt("k_fast_cells<48>", r"VIMNMX3\.S16x2", 22, 40,
+        "k_fast_cells<48>: exact FAST score of one queued pixel -- LDS.U8 ring loads, IMAD packing (bright | dark in s16x2), VIMNMX3.S16x2 min / max tree")
+excerpt("k_orient_desc", r"LDS\.128", 4, 34,
+        "k_orient_desc: steered BRIEF -- LDS.128 pattern fetch, FMUL / FADD / F2I rotation, IMAD + LDG.U8 gathers, VOTE")
 excerpt("k_resize_g", r"IDP\.2A", 10, 16, "k_resize_g: PRMT + IDP.2A horizontal pass on funnel-shifted source windows")
 with open(out_path, "w") as f:
     f.write("\n".join(out) + "\n")
