@@ -1,6 +1,7 @@
 // orbm.cu -- host side + C-ABI of the ORB matcher (reference: src/ORBmatcher.cc, include/ORBmatcher.h).
 #include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <new>
 #include <vector>
 
@@ -25,17 +26,34 @@ int orbm::reserve(size_t bytes) {
 }
 
 namespace {
-struct Carver {   // sequential sub-allocation out of the arena, 256-byte aligned
+// Sequential sub-allocation out of one device block, 256-byte aligned.  Against a null base it only measures: `off` is
+// then the size the same sequence of take() calls needs.  A take() past `cap` returns null and marks the carver overrun.
+struct Carver {
   char* base;
-  size_t off = 0;
-  explicit Carver(void* b) : base((char*)b) {}
+  size_t cap, off = 0;
+  bool overrun = false;
+  explicit Carver(void* b = nullptr, size_t c = SIZE_MAX) : base((char*)b), cap(c) {}
   template <class T>
   T* take(size_t n) {
-    T* p = (T*)(base + off);
+    const size_t at = off;
     off = align_up_sz(off + std::max<size_t>(n, 1) * sizeof(T), 256);
-    return p;
+    if (off > cap) overrun = true;
+    return (base && !overrun) ? (T*)(base + at) : nullptr;
   }
 };
+
+// Carves the arena with `take_all`, the entry's complete buffer list: once against a null base to measure, then for
+// real once the arena has grown to that size.
+template <class F>
+int carve_arena(orbm* h, F&& take_all) {
+  Carver probe;
+  take_all(probe);
+  B200_CHECK(h->reserve(probe.off));
+  Carver c(h->d_arena, h->arena_bytes);
+  take_all(c);
+  if (c.overrun) { set_error("matcher arena overrun"); return B200ORB_EINVAL; }
+  return B200ORB_OK;
+}
 
 int resolve_smem(int cmax, size_t* smem, const void* func) {
   *smem = (size_t)cmax * 5 + 16;
@@ -43,59 +61,69 @@ int resolve_smem(int cmax, size_t* smem, const void* func) {
   if (*smem > 48 * 1024) B200_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
   return B200ORB_OK;
 }
+
+// The fused LAST kernel stages a frame pair in shared memory, and its resolve key holds a keypoint index in 12 bits.
+bool match_last_fused(int cmax, int lmax) { return mf_smem_bytes(cmax, align_up(lmax, 16)) <= 200 * 1024 && cmax <= 4096; }
+
+struct LastScratch {   // the non-fused LAST path: query arrays, grids and candidate lists of every pair
+  int *goff, *gidx, *count, *min_level, *max_level;
+  unsigned* list;
+  uint8_t* valid;
+  float *u, *v, *radius, *uright;
+};
+
+LastScratch take_last_scratch(Carver& c, int npairs, size_t cstride, size_t lstride) {
+  const size_t nc = (size_t)npairs * cstride, nq = (size_t)npairs * lstride;
+  LastScratch s;
+  s.goff = c.take<int>((size_t)npairs * (GRID_CELLS + 1)); s.gidx = c.take<int>(nc);
+  s.list = c.take<unsigned>(nq * LCAP); s.count = c.take<int>(nq);
+  s.valid = c.take<uint8_t>(nq); s.u = c.take<float>(nq); s.v = c.take<float>(nq); s.radius = c.take<float>(nq);
+  s.uright = c.take<float>(nq); s.min_level = c.take<int>(nq); s.max_level = c.take<int>(nq);
+  return s;
+}
 }  // namespace
 
-int launch_match_last_unfused(const CurView& cv_in, const LastView& lv, const MatchCam& cam, int npairs, int* d_goff,
-                              int* d_gidx, unsigned* d_list, int* d_count, int* d_accepted, int* d_cur2last,
-                              int* d_nmatch, int cmax, int lmax, cudaStream_t stream, long long* launches);
-
-// Enqueue the LAST search of `npairs` (cur, last) instances.
-int launch_match_last(const CurView& cv_in, const LastView& lv, const MatchCam& cam, int npairs, int* d_goff, int* d_gidx,
-                      unsigned* d_list, int* d_count, int* d_accepted, int* d_cur2last, int* d_nmatch, int cmax,
-                      int lmax, cudaStream_t stream, long long* launches) {
-  const int lmax16 = align_up(lmax, 16);
-  const size_t smem = mf_smem_bytes(cmax, lmax16);
-  if (smem > 200 * 1024 || cmax > 4096)   // frame too large to stage in shared memory (or for the packed resolve key):
-                                          // separate grid / candidate / resolve kernels
-    return launch_match_last_unfused(cv_in, lv, cam, npairs, d_goff, d_gidx, d_list, d_count, d_accepted, d_cur2last,
-                                     d_nmatch, cmax, lmax, stream, launches);
-  B200_CUDA(cudaFuncSetAttribute(k_match_last_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  ListView lsv{d_list, d_count};
-  k_match_last_fused<<<npairs, MF_THREADS, smem, stream>>>(cv_in, lv, cam, lsv, d_accepted, d_cur2last, d_nmatch, cmax, lmax16);
-  if (launches) *launches += 1;
-  B200_CUDA(cudaGetLastError());
-  return B200ORB_OK;
+size_t match_last_scratch_bytes(int npairs, size_t cstride, size_t lstride) {
+  if (match_last_fused(align_up((int)cstride, 16), (int)lstride)) return 0;
+  Carver probe;
+  take_last_scratch(probe, npairs, cstride, lstride);
+  return probe.off;
 }
 
-// The unfused three-kernel path (grid / candidates / resolve as separate launches); kept for A/B timing.
-int launch_match_last_unfused(const CurView& cv_in, const LastView& lv, const MatchCam& cam, int npairs, int* d_goff,
-                              int* d_gidx, unsigned* d_list, int* d_count, int* d_accepted, int* d_cur2last,
-                              int* d_nmatch, int cmax, int lmax, cudaStream_t stream, long long* launches) {
+int launch_match_last(const CurView& cv_in, const LastView& lv, const MatchCam& cam, int npairs, void* d_scratch,
+                      int* d_accepted, int* d_cur2last, int* d_nmatch, cudaStream_t stream, long long* launches) {
+  const int cmax = align_up((int)cv_in.stride, 16), lmax = (int)lv.stride;
+  if (match_last_fused(cmax, lmax)) {
+    const int lmax16 = align_up(lmax, 16);
+    const size_t smem = mf_smem_bytes(cmax, lmax16);
+    B200_CUDA(cudaFuncSetAttribute(k_match_last_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_match_last_fused<<<npairs, MF_THREADS, smem, stream>>>(cv_in, lv, cam, d_accepted, d_cur2last, d_nmatch, cmax, lmax16);
+    if (launches) *launches += 1;
+    B200_CUDA(cudaGetLastError());
+    return B200ORB_OK;
+  }
+  if (!d_scratch) { set_error("no scratch for the non-fused LAST search"); return B200ORB_EINVAL; }
+  Carver c(d_scratch);
+  const LastScratch s = take_last_scratch(c, npairs, cv_in.stride, lv.stride);
   CurView cv = cv_in;
-  k_grid_build<<<npairs, 256, 0, stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, d_goff,
-                                          d_gidx);
-  cv.goff = d_goff; cv.gidx = d_gidx;
-  ListView lsv{d_list, d_count};
-  k_cand_last<<<dim3((lmax + CAND_WARPS - 1) / CAND_WARPS, npairs), CAND_WARPS * 32, 0, stream>>>(cv, lv, cam, lsv);
+  cv.goff = s.goff; cv.gidx = s.gidx;
+  k_last_queries<<<dim3((lmax + 255) / 256, npairs), 256, 0, stream>>>(cv, lv, cam, s.valid, s.u, s.v, s.radius, s.uright,
+                                                                      s.min_level, s.max_level);
+  k_grid_build<<<npairs, 256, 0, stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, s.goff,
+                                          s.gidx);
+  const QueriesView qv{s.valid, s.u, s.v, s.radius, s.uright, lv.ang, s.min_level, s.max_level, lv.obs, lv.desc, lv.n,
+                       lv.stride};
+  const ListView lsv{s.list, s.count};
+  k_cand_generic<<<dim3((lmax + CAND_WARPS - 1) / CAND_WARPS, npairs), CAND_WARPS * 32, 0, stream>>>(cv, qv, cam, 0, lsv);
   size_t smem;
-  B200_CHECK(resolve_smem(cmax, &smem, (const void*)k_resolve_last));
-  k_resolve_last<<<npairs, 32, smem, stream>>>(cv, lv, cam, lsv, d_accepted, d_cur2last, d_nmatch, cmax);
-  if (launches) *launches += 3;
+  B200_CHECK(resolve_smem(cmax, &smem, (const void*)k_resolve_generic));
+  k_resolve_generic<<<npairs, 32, smem, stream>>>(cv, qv, cam, ORBM_TH_HIGH, 0, lsv, d_accepted, d_cur2last, d_nmatch, cmax);
+  if (launches) *launches += 4;
   B200_CUDA(cudaGetLastError());
   return B200ORB_OK;
 }
 
 extern "C" {
-
-#ifdef B200ORB_TIMING
-int orbm_debug_read(unsigned long long* out16) {   // profiling builds only: phase cycle counters of k_match_last_fused
-  cudaDeviceSynchronize();
-  if (cudaMemcpyFromSymbol(out16, g_mf_dbg, sizeof(unsigned long long) * 16) != cudaSuccess) return B200ORB_ECUDA;
-  unsigned long long z[16] = {0};
-  cudaMemcpyToSymbol(g_mf_dbg, z, sizeof(z));
-  return B200ORB_OK;
-}
-#endif
 
 int orbm_hamming(const uint8_t a[32], const uint8_t b[32]) {   // DescriptorDistance, src/ORBmatcher.cc:1968-1984
   int d = 0;
@@ -136,25 +164,31 @@ static int fill_cam(const OrbmFrame* f, float th, int mono, float nnratio, int c
 }
 
 #define UP(dst, src, count, T)                                                                              \
-  B200_CUDA(cudaMemcpyAsync((dst), (src), sizeof(T) * (size_t)(count), cudaMemcpyHostToDevice, h->stream))
+  B200_CUDA(cudaMemcpyAsync((void*)(dst), (src), sizeof(T) * (size_t)(count), cudaMemcpyHostToDevice, h->stream))
 
-// uploads the current-frame arrays; fills cv (single instance)
-static int upload_cur(orbm* h, Carver& cv_mem, const OrbmFrame* cur, CurView* cv, int** d_goff, int** d_gidx) {
+// the current-frame arrays and grid of a single instance
+static void take_cur(Carver& c, const OrbmFrame* cur, CurView* cv) {
   const size_t nc = cur->n;
-  float* d_cx = cv_mem.take<float>(nc); float* d_cy = cv_mem.take<float>(nc); float* d_cang = cv_mem.take<float>(nc);
-  float* d_cur = cv_mem.take<float>(nc); int* d_coct = cv_mem.take<int>(nc); uint8_t* d_cdesc = cv_mem.take<uint8_t>(nc * 32);
-  int* d_cobs = cur->mp_obs ? cv_mem.take<int>(nc) : nullptr;
-  int* d_cn = cv_mem.take<int>(1); float* d_cT = cv_mem.take<float>(16);
-  *d_goff = cv_mem.take<int>(GRID_CELLS + 1); *d_gidx = cv_mem.take<int>(nc);
-  UP(d_cx, cur->x, nc, float); UP(d_cy, cur->y, nc, float); UP(d_cang, cur->angle, nc, float);
-  UP(d_cur, cur->uright, nc, float); UP(d_coct, cur->octave, nc, int); UP(d_cdesc, cur->desc, nc * 32, uint8_t);
-  if (d_cobs) UP(d_cobs, cur->mp_obs, nc, int);
-  const int cn = cur->n;
-  UP(d_cn, &cn, 1, int); UP(d_cT, cur->Tcw, 16, float);
   memset(cv, 0, sizeof(*cv));
-  cv->x = d_cx; cv->y = d_cy; cv->ang = d_cang; cv->uright = d_cur; cv->oct = d_coct; cv->desc = d_cdesc; cv->obs = d_cobs;
-  cv->n = d_cn; cv->Tcw = d_cT; cv->stride = nc; cv->goff = *d_goff; cv->gidx = *d_gidx;
+  cv->x = c.take<float>(nc); cv->y = c.take<float>(nc); cv->ang = c.take<float>(nc); cv->uright = c.take<float>(nc);
+  cv->oct = c.take<int>(nc); cv->desc = c.take<uint8_t>(nc * 32); cv->obs = cur->mp_obs ? c.take<int>(nc) : nullptr;
+  cv->n = c.take<int>(1); cv->Tcw = c.take<float>(16);
+  cv->goff = c.take<int>(GRID_CELLS + 1); cv->gidx = c.take<int>(nc);
+  cv->stride = nc;
+}
+
+static int upload_cur(orbm* h, const OrbmFrame* cur, const CurView& cv) {
+  const size_t nc = cur->n;
+  UP(cv.x, cur->x, nc, float); UP(cv.y, cur->y, nc, float); UP(cv.ang, cur->angle, nc, float);
+  UP(cv.uright, cur->uright, nc, float); UP(cv.oct, cur->octave, nc, int); UP(cv.desc, cur->desc, nc * 32, uint8_t);
+  if (cv.obs) UP(cv.obs, cur->mp_obs, nc, int);
+  UP(cv.n, &cur->n, 1, int); UP(cv.Tcw, cur->Tcw, 16, float);
   return B200ORB_OK;
+}
+
+static void grid_build(orbm* h, const CurView& cv, const MatchCam& cam) {
+  k_grid_build<<<1, 256, 0, h->stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y,
+                                         (int*)cv.goff, (int*)cv.gidx);
 }
 
 static int check_cur(const OrbmFrame* cur) {
@@ -184,27 +218,24 @@ int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLa
   cam.last_obs_default = 0;
   DeviceGuard g(h->device);
   const size_t nc = cur->n, nl = last->n;
-  const size_t need = nc * (4 * 4 + 4 + 32 + 4 + 4 + 4) + nl * (12 + 1 + 4 + 4 + 32 + 4 + 4 * LCAP + 4 + 4) + 4 * (GRID_CELLS + 1) +
-                      64 * 256 + 4096;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
   CurView cv;
-  int *d_goff, *d_gidx;
-  B200_CHECK(upload_cur(h, cm, cur, &cv, &d_goff, &d_gidx));
-  float* d_lxw = cm.take<float>(nl * 3); uint8_t* d_lvalid = cm.take<uint8_t>(nl); int* d_loct = cm.take<int>(nl);
-  float* d_lang = cm.take<float>(nl); uint8_t* d_ldesc = cm.take<uint8_t>(nl * 32);
-  int* d_lobs = last->mp_obs ? cm.take<int>(nl) : nullptr;
-  int* d_ln = cm.take<int>(1); float* d_lT = cm.take<float>(16);
-  int* d_out = cm.take<int>(nc); int* d_nm = cm.take<int>(1);
-  unsigned* d_list = cm.take<unsigned>(nl * LCAP); int* d_count = cm.take<int>(nl); int* d_acc = cm.take<int>(nl);
-  UP(d_lxw, last->xw, nl * 3, float); UP(d_lvalid, last->valid, nl, uint8_t); UP(d_loct, last->octave, nl, int);
-  UP(d_lang, last->angle, nl, float); UP(d_ldesc, last->mp_desc, nl * 32, uint8_t);
-  if (d_lobs) UP(d_lobs, last->mp_obs, nl, int);
-  const int ln = last->n;
-  UP(d_ln, &ln, 1, int); UP(d_lT, last->Tcw, 16, float);
-  LastView lv{d_lxw, d_lvalid, d_loct, d_lang, d_ldesc, d_lobs, d_ln, d_lT, nl};
-  B200_CHECK(launch_match_last(cv, lv, cam, 1, d_goff, d_gidx, d_list, d_count, d_acc, d_out, d_nm, align_up((int)nc, 16),
-                               (int)nl, h->stream, &h->launches));
+  LastView lv{};
+  int *d_out, *d_nm, *d_acc;
+  uint8_t* d_scratch;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    take_cur(c, cur, &cv);
+    lv.xw = c.take<float>(nl * 3); lv.valid = c.take<uint8_t>(nl); lv.oct = c.take<int>(nl); lv.ang = c.take<float>(nl);
+    lv.desc = c.take<uint8_t>(nl * 32); lv.obs = last->mp_obs ? c.take<int>(nl) : nullptr;
+    lv.n = c.take<int>(1); lv.Tcw = c.take<float>(16); lv.stride = nl;
+    d_out = c.take<int>(nc); d_nm = c.take<int>(1); d_acc = c.take<int>(nl);
+    d_scratch = c.take<uint8_t>(match_last_scratch_bytes(1, nc, nl));
+  }));
+  B200_CHECK(upload_cur(h, cur, cv));
+  UP(lv.xw, last->xw, nl * 3, float); UP(lv.valid, last->valid, nl, uint8_t); UP(lv.oct, last->octave, nl, int);
+  UP(lv.ang, last->angle, nl, float); UP(lv.desc, last->mp_desc, nl * 32, uint8_t);
+  if (lv.obs) UP(lv.obs, last->mp_obs, nl, int);
+  UP(lv.n, &last->n, 1, int); UP(lv.Tcw, last->Tcw, 16, float);
+  B200_CHECK(launch_match_last(cv, lv, cam, 1, d_scratch, d_acc, d_out, d_nm, h->stream, &h->launches));
   B200_CUDA(cudaMemcpyAsync(cur2last, d_out, sizeof(int) * nc, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaMemcpyAsync(nmatches, d_nm, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
@@ -222,39 +253,50 @@ int orbm_search_by_projection_points(orbm_t* h, const OrbmFrame* f, const OrbmTr
     for (int j = 0; j < f->n; ++j) f2pt[j] = (f->mp_obs && f->mp_obs[j] >= 0) ? -2 : -1;
     return B200ORB_OK;
   }
-  for (int i = 0; i < pts->n; ++i)
-    if (pts->track_in_view[i] && (pts->scale_level[i] < 0 || pts->scale_level[i] >= f->nlevels)) {
-      set_error("scale level out of range");
-      return B200ORB_EINVAL;
-    }
   MatchCam cam;
   B200_CHECK(fill_cam(f, th, 0, nnratio, 0, &cam));
   cam.last_obs_default = 1;
-  DeviceGuard g(h->device);
+  // the window of every point in view (:79-91): radius RadiusByViewingCos (:159-165) * th * mvScaleFactors[level],
+  // levels [level - 1, level]
   const size_t nc = f->n, np = pts->n;
-  const size_t need = nc * (4 * 4 + 4 + 32 + 4 + 4 + 4) + np * (1 + 16 + 4 + 32 + 4 + 4 * LCAP + 4) + 4 * (GRID_CELLS + 1) + 64 * 256 + 4096;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
+  std::vector<float> radius(np, 0.f);
+  std::vector<int> min_level(np, 0), max_level(np, 0);
+  for (size_t i = 0; i < np; ++i) {
+    if (!pts->track_in_view[i]) continue;
+    const int lvl = pts->scale_level[i];
+    if (lvl < 0 || lvl >= f->nlevels) { set_error("scale level out of range"); return B200ORB_EINVAL; }
+    float r = ((double)pts->view_cos[i] > 0.998) ? 2.5f : 4.0f;
+    if (th != 1.0f) r *= th;
+    radius[i] = r * f->scale_factors[lvl];
+    min_level[i] = lvl - 1; max_level[i] = lvl;
+  }
+  DeviceGuard g(h->device);
   CurView cv;
-  int *d_goff, *d_gidx;
-  B200_CHECK(upload_cur(h, cm, f, &cv, &d_goff, &d_gidx));
-  uint8_t* d_inv = cm.take<uint8_t>(np); float* d_px = cm.take<float>(np); float* d_py = cm.take<float>(np);
-  float* d_pxr = cm.take<float>(np); float* d_vc = cm.take<float>(np); int* d_lvl = cm.take<int>(np);
-  uint8_t* d_desc = cm.take<uint8_t>(np * 32); int* d_obs = pts->mp_obs ? cm.take<int>(np) : nullptr;
-  unsigned* d_list = cm.take<unsigned>(np * LCAP); int* d_count = cm.take<int>(np);
-  int* d_out = cm.take<int>(nc); int* d_nm = cm.take<int>(1);
-  UP(d_inv, pts->track_in_view, np, uint8_t); UP(d_px, pts->proj_x, np, float); UP(d_py, pts->proj_y, np, float);
-  UP(d_pxr, pts->proj_xr, np, float); UP(d_vc, pts->view_cos, np, float); UP(d_lvl, pts->scale_level, np, int);
-  UP(d_desc, pts->mp_desc, np * 32, uint8_t);
-  if (d_obs) UP(d_obs, pts->mp_obs, np, int);
-  PointsView pv{d_inv, d_px, d_py, d_pxr, d_vc, d_lvl, d_desc, d_obs, (int)np};
-  ListView lsv{d_list, d_count};
-  k_grid_build<<<1, 256, 0, h->stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, d_goff, d_gidx);
-  k_cand_points<<<((int)np + CAND_WARPS - 1) / CAND_WARPS, CAND_WARPS * 32, 0, h->stream>>>(cv, pv, cam, lsv);
+  QueriesView qv{};
+  ListView lsv;
+  int *d_out, *d_nm;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    take_cur(c, f, &cv);
+    qv.valid = c.take<uint8_t>(np); qv.u = c.take<float>(np); qv.v = c.take<float>(np); qv.radius = c.take<float>(np);
+    qv.uright = c.take<float>(np); qv.min_level = c.take<int>(np); qv.max_level = c.take<int>(np);
+    qv.obs = pts->mp_obs ? c.take<int>(np) : nullptr; qv.desc = c.take<uint8_t>(np * 32); qv.n = c.take<int>(1);
+    qv.stride = np;
+    lsv.list = c.take<unsigned>(np * LCAP); lsv.count = c.take<int>(np);
+    d_out = c.take<int>(nc); d_nm = c.take<int>(1);
+  }));
+  B200_CHECK(upload_cur(h, f, cv));
+  UP(qv.valid, pts->track_in_view, np, uint8_t); UP(qv.u, pts->proj_x, np, float); UP(qv.v, pts->proj_y, np, float);
+  UP(qv.radius, radius.data(), np, float); UP(qv.uright, pts->proj_xr, np, float);
+  UP(qv.min_level, min_level.data(), np, int); UP(qv.max_level, max_level.data(), np, int);
+  UP(qv.desc, pts->mp_desc, np * 32, uint8_t);
+  if (qv.obs) UP(qv.obs, pts->mp_obs, np, int);
+  UP(qv.n, &pts->n, 1, int);
+  grid_build(h, cv, cam);
+  k_cand_generic<<<((int)np + CAND_WARPS - 1) / CAND_WARPS, CAND_WARPS * 32, 0, h->stream>>>(cv, qv, cam, 0, lsv);
   size_t smem;
   const int cmax = align_up((int)nc, 16);
   B200_CHECK(resolve_smem(cmax, &smem, (const void*)k_resolve_points));
-  k_resolve_points<<<1, 32, smem, h->stream>>>(cv, pv, cam, lsv, d_out, d_nm, cmax);
+  k_resolve_points<<<1, 32, smem, h->stream>>>(cv, qv, cam, lsv, d_out, d_nm, cmax);
   h->launches += 3;
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(f2pt, d_out, sizeof(int) * nc, cudaMemcpyDeviceToHost, h->stream));
@@ -280,28 +322,31 @@ int orbm_search_projected(orbm_t* h, const OrbmFrame* cur, const OrbmQueries* q,
   }
   MatchCam cam;
   B200_CHECK(fill_cam(cur, 0.f, 0, 0.f, check_ori, &cam));
+  cam.last_obs_default = 1;   // OrbmQueries::obs NULL: every query claims its match
   DeviceGuard g(h->device);
   const size_t nc = cur->n, nq = q->n;
-  const size_t need = nc * (4 * 4 + 4 + 32 + 4 + 4 + 4) + nq * (1 + 4 * 5 + 8 + 32 + 4 + 4 * LCAP + 8) + 4 * (GRID_CELLS + 1) + 64 * 256 + 4096;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
   CurView cv;
-  int *d_goff, *d_gidx;
-  B200_CHECK(upload_cur(h, cm, cur, &cv, &d_goff, &d_gidx));
-  uint8_t* d_valid = cm.take<uint8_t>(nq); float* d_u = cm.take<float>(nq); float* d_v = cm.take<float>(nq);
-  float* d_r = cm.take<float>(nq); int* d_mn = cm.take<int>(nq); int* d_mx = cm.take<int>(nq);
-  float* d_ur = q->uright ? cm.take<float>(nq) : nullptr; float* d_ang = cm.take<float>(nq);
-  int* d_obs = q->obs ? cm.take<int>(nq) : nullptr; uint8_t* d_desc = cm.take<uint8_t>(nq * 32);
-  unsigned* d_list = cm.take<unsigned>(nq * LCAP); int* d_count = cm.take<int>(nq); int* d_acc = cm.take<int>(nq);
-  int* d_out = cm.take<int>(nc); int* d_nm = cm.take<int>(1);
-  UP(d_valid, q->valid, nq, uint8_t); UP(d_u, q->u, nq, float); UP(d_v, q->v, nq, float); UP(d_r, q->radius, nq, float);
-  UP(d_mn, q->min_level, nq, int); UP(d_mx, q->max_level, nq, int); UP(d_desc, q->desc, nq * 32, uint8_t);
-  if (d_ur) UP(d_ur, q->uright, nq, float);
-  if (q->angle) UP(d_ang, q->angle, nq, float);
-  if (d_obs) UP(d_obs, q->obs, nq, int);
-  QueriesView qv{d_valid, d_u, d_v, d_r, d_ur, d_ang, d_mn, d_mx, d_obs, d_desc, (int)nq};
-  ListView lsv{d_list, d_count};
-  k_grid_build<<<1, 256, 0, h->stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, d_goff, d_gidx);
+  QueriesView qv{};
+  ListView lsv;
+  int *d_acc, *d_out, *d_nm;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    take_cur(c, cur, &cv);
+    qv.valid = c.take<uint8_t>(nq); qv.u = c.take<float>(nq); qv.v = c.take<float>(nq); qv.radius = c.take<float>(nq);
+    qv.min_level = c.take<int>(nq); qv.max_level = c.take<int>(nq); qv.uright = q->uright ? c.take<float>(nq) : nullptr;
+    qv.ang = c.take<float>(nq); qv.obs = q->obs ? c.take<int>(nq) : nullptr; qv.desc = c.take<uint8_t>(nq * 32);
+    qv.n = c.take<int>(1); qv.stride = nq;
+    lsv.list = c.take<unsigned>(nq * LCAP); lsv.count = c.take<int>(nq);
+    d_acc = c.take<int>(nq); d_out = c.take<int>(nc); d_nm = c.take<int>(1);
+  }));
+  B200_CHECK(upload_cur(h, cur, cv));
+  UP(qv.valid, q->valid, nq, uint8_t); UP(qv.u, q->u, nq, float); UP(qv.v, q->v, nq, float);
+  UP(qv.radius, q->radius, nq, float); UP(qv.min_level, q->min_level, nq, int); UP(qv.max_level, q->max_level, nq, int);
+  UP(qv.desc, q->desc, nq * 32, uint8_t);
+  if (qv.uright) UP(qv.uright, q->uright, nq, float);
+  if (q->angle) UP(qv.ang, q->angle, nq, float);
+  if (qv.obs) UP(qv.obs, q->obs, nq, int);
+  UP(qv.n, &q->n, 1, int);
+  grid_build(h, cv, cam);
   k_cand_generic<<<((int)nq + CAND_WARPS - 1) / CAND_WARPS, CAND_WARPS * 32, 0, h->stream>>>(cv, qv, cam, claim_rule, lsv);
   size_t smem;
   const int cmax = align_up((int)nc, 16);
@@ -328,27 +373,29 @@ int orbm_search_best(orbm_t* h, const OrbmFrame* kf, const OrbmQueries* q, int g
   MatchCam cam;
   B200_CHECK(fill_cam(kf, 0.f, 0, 0.f, 0, &cam));
   DeviceGuard g(h->device);
-  const size_t nc = kf->n, nq = q->n;
-  const size_t need = nc * (4 * 4 + 4 + 32 + 4 + 4 + 4) + nq * (1 + 4 * 6 + 8 + 32 + 8) + 4 * (GRID_CELLS + 1) + 64 * 256 + 8192;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
-  CurView cv;
-  int *d_goff, *d_gidx;
+  const size_t nq = q->n;
   OrbmFrame kf2 = *kf;
   kf2.mp_obs = nullptr;
-  B200_CHECK(upload_cur(h, cm, &kf2, &cv, &d_goff, &d_gidx));
-  uint8_t* d_valid = cm.take<uint8_t>(nq); float* d_u = cm.take<float>(nq); float* d_v = cm.take<float>(nq);
-  float* d_r = cm.take<float>(nq); int* d_mn = cm.take<int>(nq); int* d_mx = cm.take<int>(nq);
-  float* d_ur = q->uright ? cm.take<float>(nq) : nullptr; uint8_t* d_desc = cm.take<uint8_t>(nq * 32);
-  float* d_is2 = cm.take<float>(MAX_LEVELS);
-  int* d_bi = cm.take<int>(nq); int* d_bd = cm.take<int>(nq);
-  UP(d_valid, q->valid, nq, uint8_t); UP(d_u, q->u, nq, float); UP(d_v, q->v, nq, float); UP(d_r, q->radius, nq, float);
-  UP(d_mn, q->min_level, nq, int); UP(d_mx, q->max_level, nq, int); UP(d_desc, q->desc, nq * 32, uint8_t);
-  if (d_ur) UP(d_ur, q->uright, nq, float);
+  CurView cv;
+  QueriesView qv{};
+  float* d_is2;
+  int *d_bi, *d_bd;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    take_cur(c, &kf2, &cv);
+    qv.valid = c.take<uint8_t>(nq); qv.u = c.take<float>(nq); qv.v = c.take<float>(nq); qv.radius = c.take<float>(nq);
+    qv.min_level = c.take<int>(nq); qv.max_level = c.take<int>(nq); qv.uright = q->uright ? c.take<float>(nq) : nullptr;
+    qv.desc = c.take<uint8_t>(nq * 32); qv.n = c.take<int>(1); qv.stride = nq;
+    d_is2 = c.take<float>(MAX_LEVELS); d_bi = c.take<int>(nq); d_bd = c.take<int>(nq);
+  }));
+  B200_CHECK(upload_cur(h, &kf2, cv));
+  UP(qv.valid, q->valid, nq, uint8_t); UP(qv.u, q->u, nq, float); UP(qv.v, q->v, nq, float);
+  UP(qv.radius, q->radius, nq, float); UP(qv.min_level, q->min_level, nq, int); UP(qv.max_level, q->max_level, nq, int);
+  UP(qv.desc, q->desc, nq * 32, uint8_t);
+  if (qv.uright) UP(qv.uright, q->uright, nq, float);
+  UP(qv.n, &q->n, 1, int);
   if (gate == 1) UP(d_is2, inv_level_sigma2, kf->nlevels, float);
-  QueriesView qv{d_valid, d_u, d_v, d_r, d_ur, nullptr, d_mn, d_mx, nullptr, d_desc, (int)nq};
   BestGate bg{gate, d_is2, cv.uright};
-  k_grid_build<<<1, 256, 0, h->stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, d_goff, d_gidx);
+  grid_build(h, cv, cam);
   k_best_generic<<<((int)nq + CAND_WARPS - 1) / CAND_WARPS, CAND_WARPS * 32, 0, h->stream>>>(cv, qv, cam, bg, d_bi, d_bd);
   h->launches += 2;
   B200_CUDA(cudaGetLastError());
@@ -370,26 +417,27 @@ int orbm_search_for_initialization(orbm_t* h, const OrbmFrame* f1, const OrbmFra
   B200_CHECK(fill_cam(f2, 0.f, 0, nnratio, check_ori, &cam));
   DeviceGuard g(h->device);
   const size_t n1 = f1->n, n2 = f2->n;
-  const size_t need = n2 * (4 * 4 + 4 + 32 + 4 + 4 + 4 + 8) + n1 * (4 + 4 + 32 + 8 + 4 + 4) + 4 * (GRID_CELLS + 1) + 64 * 256 + 8192;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
-  CurView cv;
-  int *d_goff, *d_gidx;
   OrbmFrame f2c = *f2;
   f2c.mp_obs = nullptr;
-  B200_CHECK(upload_cur(h, cm, &f2c, &cv, &d_goff, &d_gidx));
-  int* d_oct1 = cm.take<int>(n1); float* d_ang1 = cm.take<float>(n1); uint8_t* d_desc1 = cm.take<uint8_t>(n1 * 32);
-  float* d_prev = cm.take<float>(n1 * 2); int* d_md = cm.take<int>(n2); int* d_m21 = cm.take<int>(n2);
-  int* d_bin = cm.take<int>(n1); int* d_out = cm.take<int>(n1); int* d_nm = cm.take<int>(1);
-  UP(d_oct1, f1->octave, n1, int); UP(d_ang1, f1->angle, n1, float); UP(d_desc1, f1->desc, n1 * 32, uint8_t);
-  UP(d_prev, prev_xy, n1 * 2, float);
-  InitView iv{d_oct1, d_ang1, d_desc1, d_prev, (int)n1, d_md, d_m21, d_bin};
-  k_grid_build<<<1, 256, 0, h->stream>>>(cv.x, cv.y, cv.n, cv.stride, cam.min_x, cam.max_x, cam.min_y, cam.max_y, d_goff, d_gidx);
+  CurView cv;
+  InitView iv{};
+  int *d_out, *d_nm;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    take_cur(c, &f2c, &cv);
+    iv.oct1 = c.take<int>(n1); iv.ang1 = c.take<float>(n1); iv.desc1 = c.take<uint8_t>(n1 * 32);
+    iv.prev_xy = c.take<float>(n1 * 2); iv.matched_dist = c.take<int>(n2); iv.match21 = c.take<int>(n2);
+    iv.bin1 = c.take<int>(n1); iv.n1 = (int)n1;
+    d_out = c.take<int>(n1); d_nm = c.take<int>(1);
+  }));
+  B200_CHECK(upload_cur(h, &f2c, cv));
+  UP(iv.oct1, f1->octave, n1, int); UP(iv.ang1, f1->angle, n1, float); UP(iv.desc1, f1->desc, n1 * 32, uint8_t);
+  UP(iv.prev_xy, prev_xy, n1 * 2, float);
+  grid_build(h, cv, cam);
   k_init_search<<<1, 32, 0, h->stream>>>(cv, iv, cam, window, nnratio, check_ori, d_out, d_nm);
   h->launches += 2;
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(matches12, d_out, sizeof(int) * n1, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaMemcpyAsync(prev_xy, d_prev, sizeof(float) * 2 * n1, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(prev_xy, iv.prev_xy, sizeof(float) * 2 * n1, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaMemcpyAsync(nmatches, d_nm, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
@@ -433,28 +481,25 @@ int orbm_search_for_triangulation(orbm_t* h, const OrbmTriKF* k1, const OrbmTriK
     if (k2->idx[i] >= (uint32_t)k2->n) { set_error("KF2 index out of range"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
   const size_t n1 = k1->n, n2 = k2->n;
-  const size_t need = nq * 12 + nfi * 4 + n1 * (32 + 16 + 4) + n2 * (32 + 16 + 4 + 1) + 64 * 256 + 8192;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
-  int* d_q1 = cm.take<int>(nq); int* d_qb = cm.take<int>(nq); int* d_qe = cm.take<int>(nq); unsigned* d_fidx = cm.take<unsigned>(nfi);
-  uint8_t* d_d1 = cm.take<uint8_t>(n1 * 32); uint8_t* d_d2 = cm.take<uint8_t>(n2 * 32);
-  float *d_x1 = cm.take<float>(n1), *d_y1 = cm.take<float>(n1), *d_a1 = cm.take<float>(n1), *d_u1 = cm.take<float>(n1);
-  float *d_x2 = cm.take<float>(n2), *d_y2 = cm.take<float>(n2), *d_a2 = cm.take<float>(n2), *d_u2 = cm.take<float>(n2);
-  int* d_o2 = cm.take<int>(n2); uint8_t* d_b2 = cm.take<uint8_t>(n2);
-  int* d_out = cm.take<int>(n1); int* d_nm = cm.take<int>(1);
-  std::vector<uint8_t> blocked(n2, 0);
-  if (k2->has_mp) memcpy(blocked.data(), k2->has_mp, n2);
-  UP(d_q1, q1.data(), nq, int); UP(d_qb, qb.data(), nq, int); UP(d_qe, qe.data(), nq, int); UP(d_fidx, k2->idx, nfi, unsigned);
-  UP(d_d1, k1->desc, n1 * 32, uint8_t); UP(d_d2, k2->desc, n2 * 32, uint8_t);
-  UP(d_x1, k1->x, n1, float); UP(d_y1, k1->y, n1, float); UP(d_a1, k1->angle, n1, float); UP(d_u1, k1->uright, n1, float);
-  UP(d_x2, k2->x, n2, float); UP(d_y2, k2->y, n2, float); UP(d_a2, k2->angle, n2, float); UP(d_u2, k2->uright, n2, float);
-  UP(d_o2, k2->octave, n2, int); UP(d_b2, blocked.data(), n2, uint8_t);
-  B200_CUDA(cudaMemsetAsync(d_out, 0xff, sizeof(int) * n1, h->stream));
   TriView t;
   memset(&t, 0, sizeof(t));
-  t.q_idx1 = d_q1; t.f_beg = d_qb; t.f_end = d_qe; t.f_idx = d_fidx; t.desc1 = d_d1; t.desc2 = d_d2;
-  t.x1 = d_x1; t.y1 = d_y1; t.ang1 = d_a1; t.ur1 = d_u1; t.x2 = d_x2; t.y2 = d_y2; t.ang2 = d_a2; t.ur2 = d_u2; t.oct2 = d_o2;
-  t.blocked2 = d_b2;
+  int *d_out, *d_nm;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    t.q_idx1 = c.take<int>(nq); t.f_beg = c.take<int>(nq); t.f_end = c.take<int>(nq); t.f_idx = c.take<unsigned>(nfi);
+    t.desc1 = c.take<uint8_t>(n1 * 32); t.desc2 = c.take<uint8_t>(n2 * 32);
+    t.x1 = c.take<float>(n1); t.y1 = c.take<float>(n1); t.ang1 = c.take<float>(n1); t.ur1 = c.take<float>(n1);
+    t.x2 = c.take<float>(n2); t.y2 = c.take<float>(n2); t.ang2 = c.take<float>(n2); t.ur2 = c.take<float>(n2);
+    t.oct2 = c.take<int>(n2); t.blocked2 = c.take<uint8_t>(n2);
+    d_out = c.take<int>(n1); d_nm = c.take<int>(1);
+  }));
+  std::vector<uint8_t> blocked(n2, 0);
+  if (k2->has_mp) memcpy(blocked.data(), k2->has_mp, n2);
+  UP(t.q_idx1, q1.data(), nq, int); UP(t.f_beg, qb.data(), nq, int); UP(t.f_end, qe.data(), nq, int);
+  UP(t.f_idx, k2->idx, nfi, unsigned); UP(t.desc1, k1->desc, n1 * 32, uint8_t); UP(t.desc2, k2->desc, n2 * 32, uint8_t);
+  UP(t.x1, k1->x, n1, float); UP(t.y1, k1->y, n1, float); UP(t.ang1, k1->angle, n1, float); UP(t.ur1, k1->uright, n1, float);
+  UP(t.x2, k2->x, n2, float); UP(t.y2, k2->y, n2, float); UP(t.ang2, k2->angle, n2, float); UP(t.ur2, k2->uright, n2, float);
+  UP(t.oct2, k2->octave, n2, int); UP(t.blocked2, blocked.data(), n2, uint8_t);
+  B200_CUDA(cudaMemsetAsync(d_out, 0xff, sizeof(int) * n1, h->stream));
   for (int i = 0; i < 9; ++i) t.F12[i] = F12[i];
   t.ex = ex; t.ey = ey;
   for (int i = 0; i < nlevels; ++i) { t.sf2[i] = scale_factors2[i]; t.sigma2_2[i] = level_sigma2_2[i]; }
@@ -501,11 +546,14 @@ int orbm_is_in_frustum(orbm_t* h, const OrbmFrame* f, const OrbmFrustumPoints* p
   if (!p->xw || !p->normal || !p->min_dist || !p->max_dist) { set_error("null point array"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
   const size_t n = p->n;
-  B200_CHECK(h->reserve(n * (12 + 12 + 4 + 4 + 1 + 4 * 5) + 8192));
-  Carver cm(h->d_arena);
-  float* d_xw = cm.take<float>(n * 3); float* d_nrm = cm.take<float>(n * 3); float* d_mn = cm.take<float>(n); float* d_mx = cm.take<float>(n);
-  uint8_t* d_in = cm.take<uint8_t>(n); float* d_px = cm.take<float>(n); float* d_py = cm.take<float>(n); float* d_pxr = cm.take<float>(n);
-  int* d_lvl = cm.take<int>(n); float* d_vc = cm.take<float>(n);
+  float *d_xw, *d_nrm, *d_mn, *d_mx, *d_px, *d_py, *d_pxr, *d_vc;
+  uint8_t* d_in;
+  int* d_lvl;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    d_xw = c.take<float>(n * 3); d_nrm = c.take<float>(n * 3); d_mn = c.take<float>(n); d_mx = c.take<float>(n);
+    d_in = c.take<uint8_t>(n); d_px = c.take<float>(n); d_py = c.take<float>(n); d_pxr = c.take<float>(n);
+    d_lvl = c.take<int>(n); d_vc = c.take<float>(n);
+  }));
   UP(d_xw, p->xw, n * 3, float); UP(d_nrm, p->normal, n * 3, float); UP(d_mn, p->min_dist, n, float); UP(d_mx, p->max_dist, n, float);
   B200_CUDA(cudaMemsetAsync(d_px, 0, 4 * n, h->stream)); B200_CUDA(cudaMemsetAsync(d_py, 0, 4 * n, h->stream));
   B200_CUDA(cudaMemsetAsync(d_pxr, 0, 4 * n, h->stream)); B200_CUDA(cudaMemsetAsync(d_lvl, 0, 4 * n, h->stream));
@@ -540,9 +588,10 @@ int orbm_undistort_keypoints(orbm_t* h, const float* xy_in, int n, const float K
     return B200ORB_OK;
   }
   DeviceGuard g(h->device);
-  B200_CHECK(h->reserve((size_t)n * 16 + 4096));
-  Carver cm(h->d_arena);
-  float* d_in = cm.take<float>((size_t)n * 2); float* d_out = cm.take<float>((size_t)n * 2);
+  float *d_in, *d_out;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    d_in = c.take<float>((size_t)n * 2); d_out = c.take<float>((size_t)n * 2);
+  }));
   UP(d_in, xy_in, (size_t)n * 2, float);
   UndistortParams p;
   p.fx = K[0]; p.fy = K[4]; p.cx = K[2]; p.cy = K[5];
@@ -589,16 +638,18 @@ static int bow_impl(orbm_t* h, const OrbmBow* kf, const OrbmBow* f, float nnrati
   for (size_t i = 0; i < nfi; ++i)
     if (f->idx[i] >= (uint32_t)f->n) { set_error("F index out of range"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  const size_t need = nq * (12 + 4 * LCAP + 8) + nfi * 4 + (size_t)kf->n * (36 + 4) + (size_t)f->n * (36 + 4 + 1) + 64 * 256 + 4096;
-  B200_CHECK(h->reserve(need));
-  Carver cm(h->d_arena);
-  int* d_qkf = cm.take<int>(nq); int* d_qb = cm.take<int>(nq); int* d_qe = cm.take<int>(nq);
-  unsigned* d_fidx = cm.take<unsigned>(nfi);
-  uint8_t* d_kd = cm.take<uint8_t>((size_t)kf->n * 32); uint8_t* d_fd = cm.take<uint8_t>((size_t)f->n * 32);
-  float* d_ka = cm.take<float>(kf->n); float* d_fa = cm.take<float>(f->n);
-  unsigned* d_list = cm.take<unsigned>(nq * LCAP); int* d_count = cm.take<int>(nq); int* d_acc = cm.take<int>(nq);
-  int* d_out = cm.take<int>(nout); int* d_nm = cm.take<int>(1);
-  uint8_t* d_fvalid = (kfkf && f->valid) ? cm.take<uint8_t>(f->n) : nullptr;
+  int *d_qkf, *d_qb, *d_qe, *d_count, *d_acc, *d_out, *d_nm;
+  unsigned *d_fidx, *d_list;
+  uint8_t *d_kd, *d_fd, *d_fvalid;
+  float *d_ka, *d_fa;
+  B200_CHECK(carve_arena(h, [&](Carver& c) {
+    d_qkf = c.take<int>(nq); d_qb = c.take<int>(nq); d_qe = c.take<int>(nq); d_fidx = c.take<unsigned>(nfi);
+    d_kd = c.take<uint8_t>((size_t)kf->n * 32); d_fd = c.take<uint8_t>((size_t)f->n * 32);
+    d_ka = c.take<float>(kf->n); d_fa = c.take<float>(f->n);
+    d_list = c.take<unsigned>(nq * LCAP); d_count = c.take<int>(nq); d_acc = c.take<int>(nq);
+    d_out = c.take<int>(nout); d_nm = c.take<int>(1);
+    d_fvalid = (kfkf && f->valid) ? c.take<uint8_t>(f->n) : nullptr;
+  }));
   if (d_fvalid) UP(d_fvalid, f->valid, f->n, uint8_t);
   UP(d_qkf, q_kf.data(), nq, int); UP(d_qb, q_beg.data(), nq, int); UP(d_qe, q_end.data(), nq, int);
   UP(d_fidx, f->idx, nfi, unsigned); UP(d_kd, kf->desc, (size_t)kf->n * 32, uint8_t); UP(d_fd, f->desc, (size_t)f->n * 32, uint8_t);

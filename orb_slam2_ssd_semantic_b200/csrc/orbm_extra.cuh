@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(CAND_WARPS * 32) k_best_generic(CurView cv, Qu
                                                                   int* __restrict__ best_idx, int* __restrict__ best_dist) {
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * CAND_WARPS + (threadIdx.x >> 5);
-  if (i >= qv.n) return;
+  if (i >= qv.n[0]) return;
   int bi = -1, bd = 0x7fffffff;
   QueryGeom q;
   if (setup_generic_query(qv, i, q)) {

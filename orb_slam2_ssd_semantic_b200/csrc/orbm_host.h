@@ -12,7 +12,10 @@ struct orbm {
   int reserve(size_t bytes);
 };
 
-// shared with the stream pipeline (orbs.cu): grid build + candidate lists + order-exact resolve of `npairs` pairs
-int launch_match_last(const b200::CurView& cv, const b200::LastView& lv, const b200::MatchCam& cam, int npairs, int* d_goff,
-                      int* d_gidx, unsigned* d_list, int* d_count, int* d_accepted, int* d_cur2last, int* d_nmatch,
-                      int cmax, int lmax, cudaStream_t stream, long long* launches);
+// Shared with the stream pipeline (orbs.cu): the LAST search of `npairs` (cur, last) pairs.  Frame pairs that fit in
+// shared memory run the fused kernel; larger ones run separate query / grid / candidate / resolve kernels on device
+// scratch of match_last_scratch_bytes(npairs, cv.stride, lv.stride) bytes (0, and d_scratch may be null, when fused).
+size_t match_last_scratch_bytes(int npairs, size_t cstride, size_t lstride);
+int launch_match_last(const b200::CurView& cv, const b200::LastView& lv, const b200::MatchCam& cam, int npairs,
+                      void* d_scratch, int* d_accepted, int* d_cur2last, int* d_nmatch, cudaStream_t stream,
+                      long long* launches);

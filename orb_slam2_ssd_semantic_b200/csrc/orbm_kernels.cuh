@@ -6,14 +6,18 @@
 // distance per candidate, and a loop-carried "already claimed" state that makes query i depend on queries < i
 // (src/ORBmatcher.cc:113-115, 273-274, 1656-1658).  The GPU splits that into
 //   K7  k_grid_build     AssignFeaturesToGrid (src/Frame.cc:319-334): 64x48 CSR per frame, cell lists in ascending
-//                        keypoint index (= push_back order)
-//   K8  k_cand_*         one WARP per query, all queries of all pairs in parallel: everything that does not depend on
-//                        the claimed state -- projection, window walk in the reference's (ix, iy, insertion) order,
-//                        static filters, Hamming distances -> candidate list  list[q][ord] = dist << 20 | idx
-//   K9  k_resolve_*      one warp per frame pair walks the queries IN ORDER; per query a warp-wide redux.min over
+//                        keypoint index (= push_back order); block_grid_build, which k_match_last_fused also runs
+//   K8  k_cand_generic   one WARP per query, all queries of all instances in parallel: everything that does not depend
+//                        on the claimed state -- window walk in the reference's (ix, iy, insertion) order, static
+//                        filters, Hamming distances -> candidate list  list[q][ord] = dist << 20 | idx.  The window
+//                        geometry comes from query arrays (LAST: k_last_queries projects the last frame's points);
+//                        k_cand_bow lists the features of one BoW node instead
+//   K9  k_resolve_generic one warp per instance walks the queries IN ORDER; per query a warp-wide redux.min over
 //                        (dist << 6 | ord) of the unclaimed entries reproduces "first minimum wins" exactly; then
-//                        the rotation histogram / ComputeThreeMaxima prune (K10).
+//                        the rotation histogram / ComputeThreeMaxima prune (K10).  k_resolve_points (best-two ratio
+//                        test) and k_resolve_bow are the variants of the other claim rules.
 // A query with more than LCAP candidates is flagged and re-walked inside the resolve (exact, just slower).
+// k_match_last_fused does K7-K10 of one LAST frame pair in one CTA when the pair fits in shared memory.
 #pragma once
 #include "common.cuh"
 
@@ -65,22 +69,12 @@ __device__ __forceinline__ int grid_cell(float x, float y, float min_x, float mi
   return px * GRID_ROWS + py;
 }
 
-// K7: one CTA per frame.  goff[f][GRID_CELLS+1], gidx[f][stride].
-__global__ void __launch_bounds__(256) k_grid_build(const float* __restrict__ x, const float* __restrict__ y,
-                                                    const int* __restrict__ nkp, size_t stride, float min_x,
-                                                    float max_x, float min_y, float max_y, int* __restrict__ goff,
-                                                    int* __restrict__ gidx) {
-  __shared__ int off[GRID_CELLS + 1];
-  __shared__ int cur[GRID_CELLS];
-  __shared__ int ws[33];
-  const int f = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
-  const int n = nkp[f];
-  x += (size_t)f * stride; y += (size_t)f * stride;
-  int* idx = gidx + (size_t)f * stride;
-  const float inv_w = __fdiv_rn((float)GRID_COLS, __fsub_rn(max_x, min_x));   // src/Frame.cc:221-222
-  const float inv_h = __fdiv_rn((float)GRID_ROWS, __fsub_rn(max_y, min_y));
-  for (int c = tid; c < GRID_CELLS; c += nthr) cur[c] = 0;
-  __syncthreads();
+// The 64x48 CSR grid of one frame's n keypoints, built by the whole block: off[GRID_CELLS + 1] and idx[n] receive it,
+// cur[GRID_CELLS] is scratch that the caller has zeroed (and published with a block barrier), ws[33] is scan scratch.
+// No barrier after the last step.
+__device__ __forceinline__ void block_grid_build(const float* x, const float* y, int n, float min_x, float min_y,
+                                                 float inv_w, float inv_h, int* off, int* cur, int* idx, int* ws) {
+  const int tid = threadIdx.x, nthr = blockDim.x;
   for (int i = tid; i < n; i += nthr) {
     const int c = grid_cell(x[i], y[i], min_x, min_y, inv_w, inv_h);
     if (c >= 0) atomicAdd(&cur[c], 1);
@@ -115,6 +109,23 @@ __global__ void __launch_bounds__(256) k_grid_build(const float* __restrict__ x,
       idx[j + 1] = v;
     }
   }
+}
+
+// K7: one CTA per frame.  goff[f][GRID_CELLS+1], gidx[f][stride].
+__global__ void __launch_bounds__(256) k_grid_build(const float* __restrict__ x, const float* __restrict__ y,
+                                                    const int* __restrict__ nkp, size_t stride, float min_x,
+                                                    float max_x, float min_y, float max_y, int* __restrict__ goff,
+                                                    int* __restrict__ gidx) {
+  __shared__ int off[GRID_CELLS + 1];
+  __shared__ int cur[GRID_CELLS];
+  __shared__ int ws[33];
+  const int f = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
+  const float inv_w = __fdiv_rn((float)GRID_COLS, __fsub_rn(max_x, min_x));   // src/Frame.cc:221-222
+  const float inv_h = __fdiv_rn((float)GRID_ROWS, __fsub_rn(max_y, min_y));
+  for (int c = tid; c < GRID_CELLS; c += nthr) cur[c] = 0;
+  __syncthreads();
+  block_grid_build(x + (size_t)f * stride, y + (size_t)f * stride, nkp[f], min_x, min_y, inv_w, inv_h, off, cur,
+                   gidx + (size_t)f * stride, ws);
   int* go = goff + (size_t)f * (GRID_CELLS + 1);
   for (int c = tid; c <= GRID_CELLS; c += nthr) go[c] = off[c];
 }

@@ -21,15 +21,6 @@ struct LastView {            // LastFrame side; instance p reads at p*stride
   size_t stride;
 };
 
-struct PointsView {          // local-map points (fields Frame::isInFrustum fills)
-  const uint8_t* in_view;
-  const float *px, *py, *pxr, *view_cos;
-  const int* level;
-  const uint8_t* desc;
-  const int* obs;            // nullable
-  int n;
-};
-
 struct ListView {            // per query: LCAP entries + count (negative = overflowed, true count = -n)
   unsigned* list;
   int* count;
@@ -88,63 +79,6 @@ __device__ __forceinline__ bool setup_last_query(const MatchCam& cam, const floa
   else if (bBackward) { q.min_level = 0; q.max_level = octave; }
   else { q.min_level = octave - 1; q.max_level = octave + 1; }
   return true;
-}
-
-// window set-up of one local-map point (:79-91)
-__device__ __forceinline__ bool setup_point_query(const MatchCam& cam, const PointsView& pv, int i, QueryGeom& q) {
-  if (!pv.in_view[i]) return false;
-  const int lvl = pv.level[i];
-  float r = ((double)pv.view_cos[i] > 0.998) ? 2.5f : 4.0f;   // RadiusByViewingCos :159-165
-  if (cam.th != 1.0f) r = __fmul_rn(r, cam.th);
-  q.u = pv.px[i]; q.v = pv.py[i];
-  q.r = __fmul_rn(r, cam.sf[lvl]);
-  q.rr = q.r;
-  q.ur = pv.pxr[i];
-  q.min_level = lvl - 1; q.max_level = lvl;
-  return true;
-}
-
-// K8 (LAST): grid = (ceil(lstride / CAND_WARPS), npairs); one warp per last-frame keypoint
-__global__ void __launch_bounds__(CAND_WARPS * 32) k_cand_last(CurView cv, LastView lv, MatchCam cam, ListView out) {
-  const int p = blockIdx.y, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * CAND_WARPS + (threadIdx.x >> 5);
-  if (i >= lv.n[p]) return;
-  const size_t lo = (size_t)p * lv.stride;
-  unsigned* list = out.list + (lo + i) * LCAP;
-  int cnt = 0;
-  if (lv.valid[lo + i]) {
-    bool fwd, bwd;
-    motion_flags(cam, cv.Tcw + (size_t)p * 16, lv.Tcw + (size_t)p * 16, fwd, bwd);
-    QueryGeom q;
-    if (setup_last_query(cam, cv.Tcw + (size_t)p * 16, fwd, bwd, lv.xw + (lo + i) * 3, lv.oct[lo + i], q)) {
-      const uint8_t* d = lv.desc + (lo + i) * 32;
-      const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-      const WalkCtx g = make_ctx(cv, cam, p);
-      cnt = warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
-        if (ord < LCAP) list[ord] = ((unsigned)dist << 20) | (unsigned)idx;
-      });
-    }
-  }
-  if (lane == 0) out.count[lo + i] = (cnt > LCAP) ? -cnt : cnt;
-}
-
-// K8 (POINTS): grid = ceil(n / CAND_WARPS); a single current frame (instance 0)
-__global__ void __launch_bounds__(CAND_WARPS * 32) k_cand_points(CurView cv, PointsView pv, MatchCam cam, ListView out) {
-  const int lane = threadIdx.x & 31;
-  const int i = blockIdx.x * CAND_WARPS + (threadIdx.x >> 5);
-  if (i >= pv.n) return;
-  unsigned* list = out.list + (size_t)i * LCAP;
-  int cnt = 0;
-  QueryGeom q;
-  if (setup_point_query(cam, pv, i, q)) {
-    const uint8_t* d = pv.desc + (size_t)i * 32;
-    const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-    const WalkCtx g = make_ctx(cv, cam, 0);
-    cnt = warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
-      if (ord < LCAP) list[ord] = ((unsigned)dist << 20) | (unsigned)idx;
-    });
-  }
-  if (lane == 0) out.count[i] = (cnt > LCAP) ? -cnt : cnt;
 }
 
 // K8 (BOW): queries are (KF keypoint, F node range) pairs prepared by the host merge-join of the two FeatureVectors
@@ -210,6 +144,19 @@ __device__ __forceinline__ unsigned long long key64(int dist, int ord, int idx) 
   return ((unsigned long long)dist << 44) | ((unsigned long long)ord << 22) | (unsigned long long)idx;
 }
 
+// Resolve of a query whose candidate list overflowed LCAP: the window walk again, first minimum (dist, ord) among the
+// keypoints not claimed so far.  best_idx / best_dist are left alone when there is none.
+__device__ __forceinline__ void first_unclaimed_min(const WalkCtx& g, const QueryGeom& q, const uint8_t* desc,
+                                                    const uint8_t* taken, int& best_idx, int& best_dist) {
+  const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(desc)), d1 = __ldg(reinterpret_cast<const uint4*>(desc) + 1);
+  unsigned long long bk = ~0ull;
+  warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
+    if (!taken[idx]) { const unsigned long long k = key64(dist, ord, idx); bk = (k < bk) ? k : bk; }
+  });
+  bk = warp_min64(bk);
+  if (bk != ~0ull) { best_idx = (int)(bk & 0x3fffffull); best_dist = (int)(bk >> 44); }
+}
+
 // rotation histogram + prune shared by LAST and BOW (:1700-1721 / :338-360).  accepted[q] = claimed cur index or -1;
 // state[] is the pointer state of the current frame; returns the number of pruned entries (warp-uniform).
 __device__ __forceinline__ int prune_rotation(int nq, const int* accepted, const float* qang, const int* qmap,
@@ -240,82 +187,11 @@ __device__ __forceinline__ int prune_rotation(int nq, const int* accepted, const
   return pr;
 }
 
-// K9/K10 (LAST): one warp per pair.  dynamic smem: state[cmax] ints + taken[cmax] bytes
-__global__ void __launch_bounds__(32) k_resolve_last(CurView cv, LastView lv, MatchCam cam, ListView in, int* accepted,
-                                                     int* cur2last, int* nmatch, int cmax) {
-  extern __shared__ __align__(16) unsigned char rsm[];
-  __shared__ int s_hist[ORBM_HISTO_LENGTH];
-  __shared__ int s_keep[3];
-  int* state = reinterpret_cast<int*>(rsm);
-  uint8_t* taken = rsm + (size_t)cmax * 4;
-  const int p = blockIdx.x, lane = threadIdx.x;
-  const int nc = cv.n[p], nl = lv.n[p];
-  const size_t co = (size_t)p * cv.stride, lo = (size_t)p * lv.stride;
-  const int* cobs = cv.obs ? cv.obs + co : nullptr;
-  const int* lobs = lv.obs ? lv.obs + lo : nullptr;
-  int* acc = accepted + lo;
-  for (int j = lane; j < nc; j += 32) {
-    state[j] = (cobs && cobs[j] >= 0) ? -2 : -1;
-    taken[j] = 0;
-  }
-  __syncwarp();
-  bool fwd = false, bwd = false;
-  motion_flags(cam, cv.Tcw + (size_t)p * 16, lv.Tcw + (size_t)p * 16, fwd, bwd);
-  const WalkCtx g = make_ctx(cv, cam, p);
-  int n_acc = 0;
-  // software pipeline: entries of query i+1 are loaded while query i is resolved
-  const unsigned* L = in.list + lo * LCAP;
-  const int* C = in.count + lo;
-  unsigned v0 = 0, v1 = 0;
-  int cn = 0;
-  if (nl > 0) { cn = C[0]; v0 = L[lane]; v1 = L[lane + 32]; }
-  for (int i = 0; i < nl; ++i) {
-    unsigned nv0 = 0, nv1 = 0;
-    int ncn = 0;
-    if (i + 1 < nl) { ncn = C[i + 1]; nv0 = L[(size_t)(i + 1) * LCAP + lane]; nv1 = L[(size_t)(i + 1) * LCAP + lane + 32]; }
-    int best_idx = -1, best_dist = 256;
-    if (cn > 0) {
-      const Pick pk = pick_min(v0, v1, cn, taken, -1, lane);
-      best_idx = pk.idx; best_dist = pk.dist;
-    } else if (cn < 0) {   // overflowed list: exact re-walk with the claimed filter
-      QueryGeom q;
-      if (setup_last_query(cam, cv.Tcw + (size_t)p * 16, fwd, bwd, lv.xw + (lo + i) * 3, lv.oct[lo + i], q)) {
-        const uint8_t* d = lv.desc + (lo + i) * 32;
-        const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-        unsigned long long bk = ~0ull;
-        warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
-          if (!taken[idx]) { const unsigned long long k = key64(dist, ord, idx); bk = (k < bk) ? k : bk; }
-        });
-        bk = warp_min64(bk);
-        if (bk != ~0ull) { best_idx = (int)(bk & 0x3fffffull); best_dist = (int)(bk >> 44); }
-      }
-    }
-    int a = -1;
-    if (best_idx >= 0 && best_dist <= ORBM_TH_HIGH) {
-      a = best_idx;
-      ++n_acc;
-      if (lane == 0) {
-        state[best_idx] = i;
-        if ((lobs ? lobs[i] : cam.last_obs_default) > 0) taken[best_idx] = 1;
-      }
-    }
-    if (lane == 0) acc[i] = a;
-    __syncwarp();
-    v0 = nv0; v1 = nv1; cn = ncn;
-  }
-  int pruned = 0;
-  if (cam.check_ori) pruned = prune_rotation(nl, acc, lv.ang + lo, nullptr, cv.ang + co, state, s_hist, s_keep, lane);
-  __syncwarp();
-  int* out = cur2last + co;
-  for (int j = lane; j < nc; j += 32) out[j] = state[j];
-  if (lane == 0) nmatch[p] = n_acc - pruned;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // Fused LAST search: one CTA per frame pair does K7 + K8 + K9 + K10 with the current frame's keypoints, descriptors
-// and 64x48 grid staged in shared memory (every dependent load of the window walk becomes a shared-memory load), the
-// candidate lists written to L2 once, and the ordered resolve fed through a double-buffered shared-memory ring that the
-// other warps refill while warp 0 resolves.
+// and 64x48 grid staged in shared memory (every dependent load of the window walk becomes a shared-memory load), and
+// the ordered resolve fed through a shared-memory ring of candidate lists that the other warps refill while warp 0
+// resolves.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int MF_THREADS = 512;
 constexpr int MF_RING = 64;   // candidate lists in flight between the producer warps and the resolving warp
@@ -331,18 +207,8 @@ __host__ __device__ inline size_t mf_smem_bytes(int cmax, int lmax) {
          (size_t)lmax * 20 + 64;
 }
 
-#ifdef B200ORB_TIMING
-__device__ unsigned long long g_mf_dbg[16];
-#define MF_T(var) const long long var = clock64()
-#define MF_ADD(slot, v) atomicAdd(&g_mf_dbg[slot], (unsigned long long)(v))
-#else
-#define MF_T(var)
-#define MF_ADD(slot, v)
-#endif
-
-__global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, LastView lv, MatchCam cam, ListView lists,
-                                                                 int* accepted, int* cur2last, int* nmatch, int cmax,
-                                                                 int lmax) {
+__global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, LastView lv, MatchCam cam, int* accepted,
+                                                                 int* cur2last, int* nmatch, int cmax, int lmax) {
   extern __shared__ __align__(16) unsigned char fsm[];
   __shared__ int ws[33];
   __shared__ int s_hist[ORBM_HISTO_LENGTH];
@@ -370,7 +236,6 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
   uint8_t* taken = q;
   const int* cobs = cv.obs ? cv.obs + co : nullptr;
 
-  MF_T(T0);
   // ---- stage the current frame -------------------------------------------------------------------------------------
   for (int j = tid; j < nc; j += nthr) {
     s_x[j] = cv.x[co + j]; s_y[j] = cv.y[co + j]; s_ur[j] = cv.uright[co + j]; s_oct[j] = cv.oct[co + j];
@@ -388,42 +253,8 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
   // ---- K7 grid in shared memory ---------------------------------------------------------------------------------------
   const float inv_w = __fdiv_rn((float)GRID_COLS, __fsub_rn(cam.max_x, cam.min_x));
   const float inv_h = __fdiv_rn((float)GRID_ROWS, __fsub_rn(cam.max_y, cam.min_y));
-  for (int i = tid; i < nc; i += nthr) {
-    const int c = grid_cell(s_x[i], s_y[i], cam.min_x, cam.min_y, inv_w, inv_h);
-    if (c >= 0) atomicAdd(&s_cur[c], 1);
-  }
+  block_grid_build(s_x, s_y, nc, cam.min_x, cam.min_y, inv_w, inv_h, s_off, s_cur, s_idx, ws);
   __syncthreads();
-  {
-    const int per = (GRID_CELLS + nthr - 1) / nthr;
-    const int beg = min(GRID_CELLS, tid * per), end = min(GRID_CELLS, beg + per);
-    int s = 0;
-    for (int c = beg; c < end; ++c) s += s_cur[c];
-    int total;
-    int run = block_excl_scan(s, ws, &total);
-    for (int c = beg; c < end; ++c) {
-      s_off[c] = run;
-      run += s_cur[c];
-      s_cur[c] = 0;
-    }
-    if (tid == 0) s_off[GRID_CELLS] = total;
-    __syncthreads();
-  }
-  for (int i = tid; i < nc; i += nthr) {
-    const int c = grid_cell(s_x[i], s_y[i], cam.min_x, cam.min_y, inv_w, inv_h);
-    if (c >= 0) s_idx[s_off[c] + atomicAdd(&s_cur[c], 1)] = i;
-  }
-  __syncthreads();
-  for (int c = tid; c < GRID_CELLS; c += nthr) {
-    const int b = s_off[c], e = s_off[c + 1];
-    for (int i = b + 1; i < e; ++i) {
-      const int v = s_idx[i];
-      int j = i - 1;
-      while (j >= b && s_idx[j] > v) { s_idx[j + 1] = s_idx[j]; --j; }
-      s_idx[j + 1] = v;
-    }
-  }
-  __syncthreads();
-  MF_T(T1);
   WalkCtx g;
   g.off = s_off; g.idx = s_idx; g.x = s_x; g.y = s_y; g.uright = s_ur; g.oct = s_oct; g.obs = cobs;
   g.desc = reinterpret_cast<const uint8_t*>(s_desc);
@@ -431,7 +262,6 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
   bool fwd, bwd;
   motion_flags(cam, cv.Tcw + (size_t)p * 16, lv.Tcw + (size_t)p * 16, fwd, bwd);
   const float* Tc = cv.Tcw + (size_t)p * 16;
-  (void)lists;   // the candidate lists of the fused path never leave shared memory
   // ---- K8a: projection + window of every query, one THREAD per query (scalar double-precision chain off the
   //      warp-serial path) -----------------------------------------------------------------------------------------
   for (int i = tid; i < nl; i += nthr) {
@@ -461,10 +291,6 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
   for (int j = tid; j < MF_RING; j += nthr) ready[j] = 0;
   if (tid == 0) { s_next = 0; s_consumed = 0; }
   __syncthreads();
-  MF_T(T2);
-#ifdef B200ORB_TIMING
-  long long tw_wait = 0, tw_walk = 0, tw_n = 0;
-#endif
   if (warp > 0) {
     const uint4* dbase = reinterpret_cast<const uint4*>(lv.desc + lo * 32);
     for (;;) {
@@ -481,10 +307,8 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
       if (lobs && lane == 0) qobs = __ldg(lobs + i);
       // slot still holds query i - MF_RING?  Every lane polls (one broadcast load per iteration, warp-uniform exit): a
       // lane-0-only spin leaves the warp split in two for the whole walk below.
-      MF_T(Ta);
       while (i - *(volatile int*)&s_consumed >= MF_RING) __nanosleep(32);
       __syncwarp();
-      MF_T(Tb);
       if (packed >> 16) {
         QueryGeom qg;
         qg.u = q_u[i]; qg.v = q_v[i]; qg.r = q_r[i]; qg.rr = qg.r; qg.ur = q_ur[i];
@@ -501,13 +325,7 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
         __threadfence_block();
         ready[slot] = i + 1;
       }
-#ifdef B200ORB_TIMING
-      tw_wait += Tb - Ta; tw_walk += clock64() - Tb; ++tw_n;
-#endif
     }
-#ifdef B200ORB_TIMING
-    if (warp == 1 && lane == 0 && blockIdx.x == 0) { MF_ADD(4, tw_wait); MF_ADD(5, tw_walk); MF_ADD(6, tw_n); MF_ADD(7, clock64() - T2); }
-#endif
   } else {
     // Resolving warp: 32 consecutive queries per step, lane = query.  Every lane picks the first minimum of its own
     // list among the keypoints not claimed so far (speculatively ignoring the other lanes of the step).  A pick is
@@ -521,13 +339,7 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
       const int i = base + lane;
       const bool active = i < nl;
       const int slot = i % MF_RING;
-      {
-        MF_T(Tc0);
-        while (!__all_sync(0xffffffffu, !active || ready[slot] == i + 1)) __nanosleep(20);
-#ifdef B200ORB_TIMING
-        tw_wait += clock64() - Tc0;
-#endif
-      }
+      while (!__all_sync(0xffffffffu, !active || ready[slot] == i + 1)) __nanosleep(20);
       __syncwarp();
       const int cn = active ? rcnt[slot] : 0;
       const int claims = active ? robs[slot] : 0;
@@ -549,16 +361,8 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
             if (m != KEY_INF) { best_idx = (int)(m & 0xfffu); best_dist = (int)(m >> 18); }
           } else if (cnt_t < 0) {
             QueryGeom qg;
-            if (setup_last_query(cam, Tc, fwd, bwd, lv.xw + (lo + it) * 3, lv.oct[lo + it], qg)) {
-              const uint8_t* d = lv.desc + (lo + it) * 32;
-              const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-              unsigned long long bk = ~0ull;
-              warp_walk(g, qg, d0, d1, [&](int ord, int idx, int dist) {
-                if (!taken[idx]) { const unsigned long long kk = key64(dist, ord, idx); bk = (kk < bk) ? kk : bk; }
-              });
-              bk = warp_min64(bk);
-              if (bk != ~0ull) { best_idx = (int)(bk & 0x3fffffull); best_dist = (int)(bk >> 44); }
-            }
+            if (setup_last_query(cam, Tc, fwd, bwd, lv.xw + (lo + it) * 3, lv.oct[lo + it], qg))
+              first_unclaimed_min(g, qg, lv.desc + (lo + it) * 32, taken, best_idx, best_dist);
           }
           const bool acc_t = best_idx >= 0 && best_dist <= ORBM_TH_HIGH;
           if (acc_t) {
@@ -606,15 +410,8 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
       if (lane == 0) *(volatile int*)&s_consumed = min(base + 32, nl);
     }
   }
-#ifdef B200ORB_TIMING
-  if (tid == 0 && blockIdx.x == 0) { MF_ADD(8, tw_wait); MF_ADD(9, clock64() - T2); }
-#endif
   __syncthreads();
   for (int i = tid; i < nl; i += nthr) acc[i] = q_lv[i];
-  MF_T(T3);
-#ifdef B200ORB_TIMING
-  if (tid == 0 && blockIdx.x == 0) { MF_ADD(0, T1 - T0); MF_ADD(1, T2 - T1); MF_ADD(2, T3 - T2); MF_ADD(10, 1); }
-#endif
   if (tid == 0) s_nacc = n_acc;
   __syncthreads();
   // ---- K10 rotation consistency -------------------------------------------------------------------------------------
@@ -645,17 +442,19 @@ __global__ void __launch_bounds__(MF_THREADS) k_match_last_fused(CurView cv, Las
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Generic guided search (orbm_search_projected): query geometry supplied by the caller
+// Windowed searches on query geometry held in arrays: every projection search except the fused LAST kernel.  Instance
+// p matches queries [p*stride, p*stride + n[p]) against current frame p.
 // ---------------------------------------------------------------------------------------------------------------------
 struct QueriesView {
   const uint8_t* valid;
-  const float *u, *v, *radius, *uright, *ang;
-  const int *min_level, *max_level, *obs;
+  const float *u, *v, *radius, *uright, *ang;   // uright nullable: no stereo gate
+  const int *min_level, *max_level, *obs;       // obs nullable: every query has MatchCam::last_obs_default
   const uint8_t* desc;
-  int n;
+  const int* n;                                 // per instance
+  size_t stride;
 };
 
-__device__ __forceinline__ bool setup_generic_query(const QueriesView& qv, int i, QueryGeom& q) {
+__device__ __forceinline__ bool setup_generic_query(const QueriesView& qv, size_t i, QueryGeom& q) {
   if (!qv.valid[i]) return false;
   q.u = qv.u[i]; q.v = qv.v[i]; q.r = qv.radius[i]; q.rr = q.r;
   q.ur = qv.uright ? qv.uright[i] : 0.f;
@@ -663,27 +462,56 @@ __device__ __forceinline__ bool setup_generic_query(const QueriesView& qv, int i
   return !(isnan(q.u) || isnan(q.v));
 }
 
+// window walk context of instance p; claim rule 1 lets any pre-existing MapPoint block its keypoint
+__device__ __forceinline__ WalkCtx query_ctx(const CurView& cv, const QueriesView& qv, const MatchCam& cam, int p,
+                                             int claim_rule) {
+  WalkCtx g = make_ctx(cv, cam, p);
+  g.obs_block_min = claim_rule ? 0 : 1;
+  if (!qv.uright) g.uright = nullptr;
+  return g;
+}
+
+// K8a of the LAST search when the frames do not fit the fused kernel: projection + window of every last-frame point
+// into query arrays laid out like the last frame.  grid = (ceil(lstride / 256), npairs), one thread per query.
+__global__ void __launch_bounds__(256) k_last_queries(CurView cv, LastView lv, MatchCam cam, uint8_t* valid, float* u,
+                                                      float* v, float* radius, float* uright, int* min_level,
+                                                      int* max_level) {
+  const int p = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= lv.n[p]) return;
+  const size_t k = (size_t)p * lv.stride + i;
+  const float* Tc = cv.Tcw + (size_t)p * 16;
+  bool fwd, bwd;
+  motion_flags(cam, Tc, lv.Tcw + (size_t)p * 16, fwd, bwd);
+  QueryGeom q;
+  const bool ok = lv.valid[k] && setup_last_query(cam, Tc, fwd, bwd, lv.xw + k * 3, lv.oct[k], q);
+  if (ok) { u[k] = q.u; v[k] = q.v; radius[k] = q.r; uright[k] = q.ur; min_level[k] = q.min_level; max_level[k] = q.max_level; }
+  valid[k] = ok;
+}
+
+// K8: grid = (ceil(stride / CAND_WARPS), instances); one warp per query
 __global__ void __launch_bounds__(CAND_WARPS * 32) k_cand_generic(CurView cv, QueriesView qv, MatchCam cam, int claim_rule,
                                                                   ListView out) {
-  const int lane = threadIdx.x & 31;
+  const int p = blockIdx.y, lane = threadIdx.x & 31;
   const int i = blockIdx.x * CAND_WARPS + (threadIdx.x >> 5);
-  if (i >= qv.n) return;
-  unsigned* list = out.list + (size_t)i * LCAP;
+  if (i >= qv.n[p]) return;
+  const size_t k = (size_t)p * qv.stride + i;
+  unsigned* list = out.list + k * LCAP;
   int cnt = 0;
   QueryGeom q;
-  if (setup_generic_query(qv, i, q)) {
-    const uint8_t* d = qv.desc + (size_t)i * 32;
+  if (setup_generic_query(qv, k, q)) {
+    const uint8_t* d = qv.desc + k * 32;
     const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-    WalkCtx g = make_ctx(cv, cam, 0);
-    g.obs_block_min = claim_rule ? 0 : 1;
-    if (!qv.uright) g.uright = nullptr;
+    const WalkCtx g = query_ctx(cv, qv, cam, p, claim_rule);
     cnt = warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
       if (ord < LCAP) list[ord] = ((unsigned)dist << 20) | (unsigned)idx;
     });
   }
-  if (lane == 0) out.count[i] = (cnt > LCAP) ? -cnt : cnt;
+  if (lane == 0) out.count[k] = (cnt > LCAP) ? -cnt : cnt;
 }
 
+// K9/K10: one warp per instance.  The queries in order take the first minimum among the unclaimed candidates up to
+// max_dist; a query claims its keypoint under claim rule 1, or under rule 0 when its MapPoint has observations.  Then
+// the rotation prune.  dynamic smem: state[cmax] ints + taken[cmax] bytes
 __global__ void __launch_bounds__(32) k_resolve_generic(CurView cv, QueriesView qv, MatchCam cam, int max_dist,
                                                         int claim_rule, ListView in, int* accepted, int* cur2q,
                                                         int* nmatch, int cmax) {
@@ -692,35 +520,36 @@ __global__ void __launch_bounds__(32) k_resolve_generic(CurView cv, QueriesView 
   __shared__ int s_keep[3];
   int* state = reinterpret_cast<int*>(rsm);
   uint8_t* taken = rsm + (size_t)cmax * 4;
-  const int lane = threadIdx.x;
-  const int nc = cv.n[0];
+  const int p = blockIdx.x, lane = threadIdx.x;
+  const int nc = cv.n[p], nq = qv.n[p];
+  const size_t co = (size_t)p * cv.stride, qo = (size_t)p * qv.stride;
+  const int* cobs = cv.obs ? cv.obs + co : nullptr;
+  const int* qobs = qv.obs ? qv.obs + qo : nullptr;
+  int* acc = accepted + qo;
   for (int j = lane; j < nc; j += 32) {
-    state[j] = (cv.obs && cv.obs[j] >= 0) ? -2 : -1;
+    state[j] = (cobs && cobs[j] >= 0) ? -2 : -1;
     taken[j] = 0;
   }
   __syncwarp();
-  WalkCtx g = make_ctx(cv, cam, 0);
-  g.obs_block_min = claim_rule ? 0 : 1;
-  if (!qv.uright) g.uright = nullptr;
+  const WalkCtx g = query_ctx(cv, qv, cam, p, claim_rule);
   int n_acc = 0;
-  for (int i = 0; i < qv.n; ++i) {
-    const int cn = in.count[i];
+  // software pipeline: entries of query i+1 are loaded while query i is resolved
+  const unsigned* L = in.list + qo * LCAP;
+  const int* C = in.count + qo;
+  unsigned v0 = 0, v1 = 0;
+  int cn = 0;
+  if (nq > 0) { cn = C[0]; v0 = L[lane]; v1 = L[lane + 32]; }
+  for (int i = 0; i < nq; ++i) {
+    unsigned nv0 = 0, nv1 = 0;
+    int ncn = 0;
+    if (i + 1 < nq) { ncn = C[i + 1]; nv0 = L[(size_t)(i + 1) * LCAP + lane]; nv1 = L[(size_t)(i + 1) * LCAP + lane + 32]; }
     int best_idx = -1, best_dist = 256;
     if (cn > 0) {
-      const Pick pk = pick_min(in.list[(size_t)i * LCAP + lane], in.list[(size_t)i * LCAP + lane + 32], cn, taken, -1, lane);
+      const Pick pk = pick_min(v0, v1, cn, taken, -1, lane);
       best_idx = pk.idx; best_dist = pk.dist;
-    } else if (cn < 0) {
+    } else if (cn < 0) {   // overflowed list: exact re-walk with the claimed filter
       QueryGeom q;
-      if (setup_generic_query(qv, i, q)) {
-        const uint8_t* d = qv.desc + (size_t)i * 32;
-        const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
-        unsigned long long bk = ~0ull;
-        warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
-          if (!taken[idx]) { const unsigned long long kk = key64(dist, ord, idx); bk = (kk < bk) ? kk : bk; }
-        });
-        bk = warp_min64(bk);
-        if (bk != ~0ull) { best_idx = (int)(bk & 0x3fffffull); best_dist = (int)(bk >> 44); }
-      }
+      if (setup_generic_query(qv, qo + i, q)) first_unclaimed_min(g, q, qv.desc + (qo + i) * 32, taken, best_idx, best_dist);
     }
     int a = -1;
     if (best_idx >= 0 && best_dist <= max_dist) {
@@ -728,21 +557,23 @@ __global__ void __launch_bounds__(32) k_resolve_generic(CurView cv, QueriesView 
       ++n_acc;
       if (lane == 0) {
         state[best_idx] = i;
-        if (claim_rule || (qv.obs ? qv.obs[i] : 1) > 0) taken[best_idx] = 1;
+        if (claim_rule || (qobs ? qobs[i] : cam.last_obs_default) > 0) taken[best_idx] = 1;
       }
     }
-    if (lane == 0) accepted[i] = a;
+    if (lane == 0) acc[i] = a;
     __syncwarp();
+    v0 = nv0; v1 = nv1; cn = ncn;
   }
   int pruned = 0;
-  if (cam.check_ori) pruned = prune_rotation(qv.n, accepted, qv.ang, nullptr, cv.ang, state, s_hist, s_keep, lane);
+  if (cam.check_ori) pruned = prune_rotation(nq, acc, qv.ang + qo, nullptr, cv.ang + co, state, s_hist, s_keep, lane);
   __syncwarp();
-  for (int j = lane; j < nc; j += 32) cur2q[j] = state[j];
-  if (lane == 0) *nmatch = n_acc - pruned;
+  int* out = cur2q + co;
+  for (int j = lane; j < nc; j += 32) out[j] = state[j];
+  if (lane == 0) nmatch[p] = n_acc - pruned;
 }
 
 // K9 (POINTS): best and second best among unclaimed candidates, level-aware ratio test (:98-152)
-__global__ void __launch_bounds__(32) k_resolve_points(CurView cv, PointsView pv, MatchCam cam, ListView in, int* f2pt,
+__global__ void __launch_bounds__(32) k_resolve_points(CurView cv, QueriesView qv, MatchCam cam, ListView in, int* f2pt,
                                                        int* nmatch, int cmax) {
   extern __shared__ __align__(16) unsigned char rsm[];
   int* state = reinterpret_cast<int*>(rsm);
@@ -756,7 +587,8 @@ __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, PointsView pv
   __syncwarp();
   const WalkCtx g = make_ctx(cv, cam, 0);
   int n_acc = 0;
-  for (int i = 0; i < pv.n; ++i) {
+  const int nq = qv.n[0];
+  for (int i = 0; i < nq; ++i) {
     const int cn = in.count[i];
     if (cn == 0) continue;
     int bestIdx = -1, bestDist = 256, bestDist2 = 256, bestLevel = -1, bestLevel2 = -1;
@@ -770,8 +602,8 @@ __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, PointsView pv
       }
     } else {
       QueryGeom q;
-      if (setup_point_query(cam, pv, i, q)) {
-        const uint8_t* d = pv.desc + (size_t)i * 32;
+      if (setup_generic_query(qv, i, q)) {
+        const uint8_t* d = qv.desc + (size_t)i * 32;
         const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
         unsigned long long b1 = ~0ull, b2 = ~0ull;   // two smallest keys per lane
         warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
@@ -793,7 +625,7 @@ __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, PointsView pv
       ++n_acc;
       if (lane == 0) {
         state[bestIdx] = i;
-        if ((pv.obs ? pv.obs[i] : cam.last_obs_default) > 0) taken[bestIdx] = 1;
+        if ((qv.obs ? qv.obs[i] : cam.last_obs_default) > 0) taken[bestIdx] = 1;
       }
       __syncwarp();
     }

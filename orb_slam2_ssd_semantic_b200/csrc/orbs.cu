@@ -131,8 +131,8 @@ struct orbs {
   float *d_x = nullptr, *d_y = nullptr, *d_ang = nullptr, *d_ur = nullptr, *d_dep = nullptr, *d_xw = nullptr;
   int* d_oct = nullptr;
   uint8_t* d_valid = nullptr;
-  int *d_c2l = nullptr, *d_nm = nullptr, *d_count = nullptr, *d_gidx = nullptr, *d_goff = nullptr, *d_acc = nullptr;
-  unsigned* d_list = nullptr;
+  int *d_c2l = nullptr, *d_nm = nullptr, *d_acc = nullptr;
+  void* d_match_scratch = nullptr;   // only when the frames take the non-fused LAST search
   uint8_t* d_gray = nullptr;
   float *d_depth = nullptr, *d_T = nullptr;
   uint16_t* d_depth16 = nullptr;
@@ -149,11 +149,11 @@ struct orbs {
   bool have = false;
   void free_bufs() {
     auto F = [](void* p) { if (p) cudaFree(p); };
-    F(d_x); F(d_y); F(d_ang); F(d_ur); F(d_dep); F(d_xw); F(d_oct); F(d_valid); F(d_c2l); F(d_nm); F(d_count);
-    F(d_gidx); F(d_goff); F(d_acc); F(d_list); F(d_gray); F(d_depth); F(d_T); F(d_depth16); F(d_kpd16);
+    F(d_x); F(d_y); F(d_ang); F(d_ur); F(d_dep); F(d_xw); F(d_oct); F(d_valid); F(d_c2l); F(d_nm); F(d_acc);
+    F(d_match_scratch); F(d_gray); F(d_depth); F(d_T); F(d_depth16); F(d_kpd16);
     d_depth16 = nullptr; d_kpd16 = nullptr;
     d_x = d_y = d_ang = d_ur = d_dep = d_xw = nullptr; d_oct = nullptr; d_valid = nullptr;
-    d_c2l = d_nm = d_count = d_gidx = d_goff = d_acc = nullptr; d_list = nullptr; d_gray = nullptr; d_depth = d_T = nullptr;
+    d_c2l = d_nm = d_acc = nullptr; d_match_scratch = nullptr; d_gray = nullptr; d_depth = d_T = nullptr;
   }
   ~orbs() {
     DeviceGuard g(device);
@@ -177,9 +177,9 @@ struct orbs {
       B200_CUDA(cudaMalloc(&d_ur, n * 4)); B200_CUDA(cudaMalloc(&d_dep, n * 4)); B200_CUDA(cudaMalloc(&d_xw, n * 12));
       B200_CUDA(cudaMalloc(&d_oct, n * 4)); B200_CUDA(cudaMalloc(&d_valid, n));
       B200_CUDA(cudaMalloc(&d_c2l, n * 4)); B200_CUDA(cudaMalloc(&d_nm, (size_t)maxF * 4));
-      B200_CUDA(cudaMalloc(&d_count, n * 4)); B200_CUDA(cudaMalloc(&d_gidx, n * 4)); B200_CUDA(cudaMalloc(&d_acc, n * 4));
-      B200_CUDA(cudaMalloc(&d_goff, (size_t)maxF * (GRID_CELLS + 1) * 4));
-      B200_CUDA(cudaMalloc(&d_list, n * 4 * LCAP));
+      B200_CUDA(cudaMalloc(&d_acc, n * 4));
+      const size_t scratch = match_last_scratch_bytes(maxF, cap, cap);
+      if (scratch) B200_CUDA(cudaMalloc(&d_match_scratch, scratch));
     }
     if (host_inputs && !d_gray) {
       B200_CUDA(cudaMalloc(&d_gray, (size_t)maxF * rows * cols));
@@ -220,8 +220,7 @@ struct orbs {
       cv.x = d_x + c; cv.y = d_y + c; cv.ang = d_ang + c; cv.uright = d_ur + c; cv.oct = d_oct + c;
       cv.desc = ex->d_desc + c * 32; cv.obs = nullptr; cv.n = ex->d_n + 1; cv.Tcw = dT + 16; cv.stride = c;
       LastView lv{d_xw, d_valid, d_oct, d_ang, ex->d_desc, nullptr, ex->d_n, dT, c};
-      B200_CHECK(launch_match_last(cv, lv, cam, F - 1, d_goff, d_gidx, d_list, d_count, d_acc, d_c2l + c, d_nm + 1,
-                                   align_up(cap, 16), cap, st, &launches));
+      B200_CHECK(launch_match_last(cv, lv, cam, F - 1, d_match_scratch, d_acc, d_c2l + c, d_nm + 1, st, &launches));
     }
     B200_CHECK(ex->prof_mark(ST_MATCH + 1));
     lastF = F;

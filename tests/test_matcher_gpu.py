@@ -165,7 +165,8 @@ def test_search_by_bow(oracle, stream_feats, nwords):
 
 
 def test_projection_last_huge_frame_uses_unfused_path(oracle):
-    """More keypoints than fit the fused kernel's shared memory -> separate grid/candidate/resolve kernels."""
+    """More keypoints than fit the fused kernel's shared memory (and more than its 12-bit keypoint index) -> the separate
+    query / grid / candidate / resolve kernels, on a single frame pair."""
     from orb_slam2_ssd_semantic_b200 import ORBmatcher
     from orb_slam2_ssd_semantic_b200._abi import FrameView, LastView
     rng = np.random.default_rng(21)

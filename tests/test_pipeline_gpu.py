@@ -9,7 +9,7 @@ from tests.helpers import frame_views
 pytestmark = pytest.mark.gpu
 
 
-def _stream_batch_matches_oracle(oracle, rows, cols):
+def _stream_batch_matches_oracle(oracle, rows, cols, nfeatures=1000):
     from orb_slam2_ssd_semantic_b200 import StreamTracker
     F = 5
     ws = synth.WallStream(seed=1234, n=F, h=rows, w=cols)
@@ -17,9 +17,9 @@ def _stream_batch_matches_oracle(oracle, rows, cols):
     gray = np.stack([f[0] for f in frames])
     depth = np.stack([f[1] for f in frames])
     T = np.stack([f[3] for f in frames])
-    st = StreamTracker(1000, 1.2, 8, 20, 7, synth.FX, synth.FY, synth.CX, synth.CY, synth.BF, th=15.0, nnratio=0.9)
+    st = StreamTracker(nfeatures, 1.2, 8, 20, 7, synth.FX, synth.FY, synth.CX, synth.CY, synth.BF, th=15.0, nnratio=0.9)
     kps, desc, nkp, c2l, nm = st.track_batch(gray, depth, T)
-    R = oracle.RefExtractor(1000, 1.2, 8, 20, 7)
+    R = oracle.RefExtractor(nfeatures, 1.2, 8, 20, 7)
     prev = None
     for t in range(F):
         K, D = R(gray[t])
@@ -45,6 +45,12 @@ def test_stream_batch_matches_oracle(oracle):
 def test_stream_batch_matches_oracle_kitti_width(oracle):
     """376 x 1241 (KITTI): the tracker hands the extractor rows of 1241 bytes, which are not 4-byte aligned."""
     _stream_batch_matches_oracle(oracle, 376, 1241)
+
+
+def test_stream_batch_matches_oracle_non_fused(oracle):
+    """3000 features: a frame pair no longer fits the fused LAST kernel's shared memory, so the 4 pairs of the batch go
+    through the separate query / grid / candidate / resolve kernels."""
+    _stream_batch_matches_oracle(oracle, 480, 640, nfeatures=3000)
 
 
 def test_u16_depth_path_equals_float_path():
