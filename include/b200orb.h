@@ -389,7 +389,7 @@ int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_
 /* convertTo(CV_32F, factor) of n CV_16U pixels resident in HBM (n multiple of 4) on the given cudaStream_t. */
 int b200orb_depth_u16_to_f32_device(const uint16_t* d_src, float* d_dst, size_t n, float factor, void* stream);
 /* Device copies of the inputs of the last host-buffer call (gray u8, depth f32 metres), e.g. to hand keyframes to
- * ocm_insert_keyframes_device without a second upload. */
+ * ocm_insert_keyframes_labeled_device without a second upload. */
 int orbs_device_inputs(orbs_t* h, const uint8_t** d_gray, const float** d_depth);
 /* Device-resident entry (inputs already in HBM, results left in HBM; asynchronous on orbs_stream). */
 int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw,
@@ -431,21 +431,6 @@ int ocm_insert_keyframe(ocm_t* h, const float* depth, const uint8_t* rgb, int ro
 int ocm_insert_keyframe_device(ocm_t* h, const float* d_depth, const uint8_t* d_rgb, int rows, int cols,
                                const float Tcw[16], float fx, float fy, float cx, float cy,
                                const uint8_t* d_ground_label);
-/* Batched variant for a resident RGB-D stream: inserts keyframes frame_idx[0..n) (in that order) of a batch laid out
- * as depth[F][rows][cols] f32, rgb[F][rows][cols][3] u8 in HBM, Tcw[n][16] on the host (one pose per inserted
- * keyframe); keyframe i reads depth image depth_idx[i] and colour image rgb_idx[i] of the two batches.  One call
- * enqueues everything on the handle's stream (what UpdateOctomap's loop does,
- * perfect/src/MapDrawer.cc:610-638). */
-int ocm_insert_keyframes_device(ocm_t* h, const float* d_depth, const uint8_t* d_rgb, int rows, int cols,
-                                const int32_t* depth_idx, const int32_t* rgb_idx /* NULL = depth_idx */, int n,
-                                const float* Tcw, float fx, float fy, float cx, float cy);
-/* Host-buffer form for a batch of keyframes as the reference's callers hold them: the sensor's CV_16U depth images
- * (imDepth before convertTo, src/Tracking.cc:353-367; depth_factor = 1.0f / DepthMapFactor) and the colour images
- * handed to insertKeyFrame (src/Tracking.cc:1889), depth_u16[n][rows][cols], rgb[n][rows][cols][3], Tcw[n][16].
- * Uploads, the conversion and the n inserts are enqueued on the map's stream and the call returns; the host buffers
- * (page-locked for a truly asynchronous upload) must stay untouched until ocm_sync(h). */
-int ocm_insert_keyframes_u16(ocm_t* h, const uint16_t* depth_u16, const uint8_t* rgb, int rows, int cols, int n,
-                             float depth_factor, const float* Tcw, float fx, float fy, float cx, float cy);
 /* World-frame points of the LAST inserted keyframe after gating + leaf filter + transform (xyz f32 x n,
  * unordered: compare as sets). */
 int ocm_last_points(ocm_t* h, float* xyz, uint8_t* rgb, int cap, int* n);
@@ -453,21 +438,23 @@ int ocm_last_points(ocm_t* h, float* xyz, uint8_t* rgb, int cap, int* n);
 int64_t ocm_num_leaves(ocm_t* h);
 int ocm_export_leaves(ocm_t* h, uint16_t* keys, float* logodds, uint8_t* rgb, int64_t cap, int64_t* n);
 int ocm_query(ocm_t* h, const float xyz[3], float* logodds, int* found);
-/* Multi-GPU map merge (SURVEY §8(e)): per-voxel clamp-add summaries f(x)=min(max(x+a,L),H) of everything
- * inserted since the last reset; device buffers, n entries: key u64 (x | y<<16 | z<<32), a/L/H f32. */
-int64_t ocm_summary_count(ocm_t* h);
-int ocm_export_summaries_device(ocm_t* h, uint64_t* d_keys, float* d_a, float* d_lo, float* d_hi, int64_t cap,
-                                int64_t* n);
-/* Compose the summaries of a LATER shard onto this map (apply in keyframe order: shard 0, 1, ...). */
-int ocm_apply_summaries_device(ocm_t* h, const uint64_t* d_keys, const float* d_a, const float* d_lo,
-                               const float* d_hi, int64_t n);
-/* The same with a per-pixel ground label batch d_label[F][rows][cols] (NULL = all non-ground); keyframe i reads label
- * image label_idx[i] (NULL = depth_idx).  Labels stand in for the reference's RANSAC floor split
- * (perfect/src/MapDrawer.cc:686-774): ground points only clear space along their rays (:961-969). */
+/* Batched variant for a resident RGB-D stream: inserts keyframes frame_idx[0..n) (in that order) of a batch laid out
+ * as depth[F][rows][cols] f32, rgb[F][rows][cols][3] u8 in HBM, Tcw[n][16] on the host (one pose per inserted
+ * keyframe); keyframe i reads depth image depth_idx[i] and colour image rgb_idx[i] (NULL = depth_idx) of the two
+ * batches.  One call enqueues everything on the handle's stream (what UpdateOctomap's loop does,
+ * perfect/src/MapDrawer.cc:610-638).  d_label[F][rows][cols] is a per-pixel ground label batch (NULL = all
+ * non-ground); keyframe i reads label image label_idx[i] (NULL = depth_idx).  Labels stand in for the reference's
+ * RANSAC floor split (perfect/src/MapDrawer.cc:686-774): ground points only clear space along their rays (:961-969). */
 int ocm_insert_keyframes_labeled_device(ocm_t* h, const float* d_depth, const uint8_t* d_rgb, const uint8_t* d_label,
                                         int rows, int cols, const int32_t* depth_idx, const int32_t* rgb_idx,
                                         const int32_t* label_idx, int n, const float* Tcw, float fx, float fy, float cx,
                                         float cy);
+/* Host-buffer form for a batch of keyframes as the reference's callers hold them: the sensor's CV_16U depth images
+ * (imDepth before convertTo, src/Tracking.cc:353-367; depth_factor = 1.0f / DepthMapFactor) and the colour images
+ * handed to insertKeyFrame (src/Tracking.cc:1889), depth_u16[n][rows][cols], rgb[n][rows][cols][3], Tcw[n][16], and
+ * the ground labels label[n][rows][cols] (NULL = all non-ground).  Uploads, the conversion and the n inserts are
+ * enqueued on the map's stream and the call returns; the host buffers (page-locked for a truly asynchronous upload)
+ * must stay untouched until ocm_sync(h). */
 int ocm_insert_keyframes_u16_labeled(ocm_t* h, const uint16_t* depth_u16, const uint8_t* rgb, const uint8_t* label, int rows,
                                      int cols, int n, float depth_factor, const float* Tcw, float fx, float fy, float cx,
                                      float cy);

@@ -32,9 +32,8 @@ EXPORTS = [
     "orbs_create", "orbs_destroy", "orbs_track_batch", "orbs_track_batch_u16", "orbs_submit_batch_u16", "orbs_device_inputs", "orbs_set_full_depth_upload", "orbs_set_chunk_frames", "orbs_chain_after", "b200orb_depth_u16_to_f32_device", "orbs_track_batch_device", "orbs_device_results", "orbs_read_frame_glue", "orbs_sync",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
-    "ocm_default_params", "ocm_create", "ocm_destroy", "ocm_insert_keyframe", "ocm_insert_keyframe_device", "ocm_insert_keyframes_device", "ocm_insert_keyframes_u16",
-    "ocm_last_points", "ocm_num_leaves", "ocm_export_leaves", "ocm_query", "ocm_summary_count",
-    "ocm_export_summaries_device", "ocm_apply_summaries_device", "ocm_sync", "ocm_stream", "ocm_launch_count",
+    "ocm_default_params", "ocm_create", "ocm_destroy", "ocm_insert_keyframe", "ocm_insert_keyframe_device",
+    "ocm_last_points", "ocm_num_leaves", "ocm_export_leaves", "ocm_query", "ocm_sync", "ocm_stream", "ocm_launch_count",
     "ocm_insert_keyframes_labeled_device", "ocm_insert_keyframes_u16_labeled", "ocm_merge_nccl", "ocm_nccl_unique_id",
     "ocm_nccl_comm_create", "ocm_nccl_comm_destroy", "ocm_last_batch_stats",
     "dynm_create", "dynm_destroy", "dynm_launch_count", "dynm_stream", "dynm_sync", "dynm_element", "dynm_mask_from_flow",
@@ -157,8 +156,6 @@ def lib() -> C.CDLL:
     L.gcm_sync.argtypes = [vp]
     L.gcm_launch_count.argtypes = [vp]
     L.gcm_launch_count.restype = C.c_longlong
-    L.ocm_insert_keyframes_device.argtypes = [vp, vp, vp, i, i, vp, vp, i, vp, f, f, f, f]
-    L.ocm_insert_keyframes_u16.argtypes = [vp, vp, vp, i, i, i, f, vp, f, f, f, f]
     L.ocm_insert_keyframes_labeled_device.argtypes = [vp, vp, vp, vp, i, i, vp, vp, vp, i, vp, f, f, f, f]
     L.ocm_insert_keyframes_u16_labeled.argtypes = [vp, vp, vp, vp, i, i, i, f, vp, f, f, f, f]
     L.ocm_merge_nccl.argtypes = [vp, vp, vp, vp]
@@ -171,10 +168,6 @@ def lib() -> C.CDLL:
     L.ocm_num_leaves.restype = C.c_int64
     L.ocm_export_leaves.argtypes = [vp, vp, vp, vp, C.c_int64, C.POINTER(C.c_int64)]
     L.ocm_query.argtypes = [vp, vp, C.POINTER(f), C.POINTER(i)]
-    L.ocm_summary_count.argtypes = [vp]
-    L.ocm_summary_count.restype = C.c_int64
-    L.ocm_export_summaries_device.argtypes = [vp, vp, vp, vp, vp, C.c_int64, C.POINTER(C.c_int64)]
-    L.ocm_apply_summaries_device.argtypes = [vp, vp, vp, vp, vp, C.c_int64]
     L.ocm_sync.argtypes = [vp]
     L.ocm_stream.argtypes = [vp]
     L.ocm_stream.restype = vp

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
 #include <stdio.h>
 #include <string.h>
 
@@ -28,6 +30,22 @@ void set_error(const char* fmt, ...);
 
 static inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 static inline size_t align_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Sequential sub-allocation out of one device block, 256-byte aligned.  Against a null base it only measures: `off` is
+// then the size the same sequence of take() calls needs.  A take() past `cap` returns null and marks the carver overrun.
+struct Carver {
+  char* base;
+  size_t cap, off = 0;
+  bool overrun = false;
+  explicit Carver(void* b = nullptr, size_t c = SIZE_MAX) : base((char*)b), cap(c) {}
+  template <class T>
+  T* take(size_t n) {
+    const size_t at = off;
+    off = align_up_sz(off + std::max<size_t>(n, 1) * sizeof(T), 256);
+    if (off > cap) overrun = true;
+    return (base && !overrun) ? (T*)(base + at) : nullptr;
+  }
+};
 
 // RAII device guard: every ABI call runs on its handle's device and restores the caller's.
 struct DeviceGuard {

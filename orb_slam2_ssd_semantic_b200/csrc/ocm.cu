@@ -6,7 +6,7 @@
 //
 // HBM layout:
 //   leaf table   open-addressing hash of the 1-cm VoxelGrid cells of ONE keyframe (key = 3 x 21-bit cell index), one
-//                32-byte record per cell: key, count, first pixel, bucket offset, cursor.  Pixels of a cell are bucketed, sorted ascending and
+//                32-byte record per cell: key, count, first pixel, bucket offset.  Pixels of a cell are bucketed, sorted ascending and
 //                summed sequentially in float so the centroid equals the oracle's pixel-order sum bit for bit.
 //   points       world-frame centroids of the last keyframe (xyz f32, rgb, ground label), unordered
 //   map          persistent open-addressing hash: key (3 x u16 OcTreeKey packed in u64) -> float log-odds, colour, the
@@ -47,40 +47,41 @@ __device__ __forceinline__ long long hash_slot(unsigned long long k, long long m
   return (long long)(h & (unsigned)mask);
 }
 
-// find-or-insert; returns slot or -1 when the table is full; *fresh = this call created the entry
-__device__ __forceinline__ long long table_insert(unsigned long long* keys, long long cap_mask, unsigned long long key,
-                                                  bool* fresh) {
-  long long s = hash_slot(key, cap_mask);
+// Linear probe of a power-of-two open-addressing table whose keys lie STRIDE 8-byte words apart (1: a key array;
+// sizeof(LeafRec) / 8: the key field of the leaf records).  Returns whether the key has a slot, and *slot = that slot.
+// INSERT: find-or-insert (false only when the table is full), *fresh = this call created the entry.  Otherwise find
+// only.  (A found flag rather than "slot or -1": the compiler cannot prove a slot non-negative, so a sign test costs
+// the map's callers a compare and a select -- 32 instructions in k_ocm_scan_keys.  k_ocm_bin wants that test.)
+template <int STRIDE, bool INSERT = true>
+__device__ __forceinline__ bool table_probe(unsigned long long* keys, long long mask, unsigned long long key,
+                                            long long* slot, bool* fresh) {
+  long long s = hash_slot(key, mask);
+  bool found = false;
   *fresh = false;
-  for (long long probe = 0; probe <= cap_mask; ++probe) {
-    const unsigned long long cur = keys[s];
-    if (cur == key) return s;
+  for (long long probe = 0; probe <= mask; ++probe) {
+    unsigned long long* p = keys + s * STRIDE;
+    const unsigned long long cur = *p;
+    if (cur == key) { found = true; break; }
     if (cur == EMPTY_KEY) {
-      const unsigned long long old = atomicCAS(&keys[s], EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { *fresh = true; return s; }
-      if (old == key) return s;
+      if (!INSERT) break;
+      const unsigned long long old = atomicCAS(p, EMPTY_KEY, key);
+      if (old == EMPTY_KEY) { *fresh = true; found = true; break; }
+      if (old == key) { found = true; break; }
     }
-    s = (s + 1) & cap_mask;
+    s = (s + 1) & mask;
   }
-  return -1;
+  *slot = s;
+  return found;
 }
 
-__device__ __forceinline__ long long table_find(const unsigned long long* keys, long long cap_mask, unsigned long long key) {
-  long long s = hash_slot(key, cap_mask);
-  for (long long probe = 0; probe <= cap_mask; ++probe) {
-    const unsigned long long cur = keys[s];
-    if (cur == key) return s;
-    if (cur == EMPTY_KEY) return -1;
-    s = (s + 1) & cap_mask;
-  }
-  return -1;
-}
+// Error codes the kernels leave in the handle's error word (check_err turns them into messages).
+constexpr int ERR_LEAF_TABLE_FULL = 1;
+constexpr int ERR_MAP_FULL = 2;
 
 struct OcmConst {
   float fx, fy, cx, cy;
-  float depth_min, depth_max, y_max, leaf, inv_leaf;
+  float depth_min, depth_max, y_max, inv_leaf;
   double res, res_factor;
-  float hit_log, miss_log, cmin, cmax;
   double Rt[9], ti[3];     // Twc = inverse of Tcw, double (pcl::transformPointCloud<.., double>)
   float origin[3];         // translation of Tcw (UpdateOctomap quirk)
   int rows, cols;
@@ -93,35 +94,25 @@ struct __align__(32) LeafRec {
   int count;
   int first;     // smallest pixel index
   int offset;
-  int cursor;
-  int pad[2];
+  int pad[3];
 };
+static_assert(sizeof(LeafRec) == 32, "one L2 sector per leaf record");
+// An unused record: the initial fill of a leaf table, and what k_ocm_centroids leaves behind for the next keyframe.
+__host__ __device__ __forceinline__ LeafRec empty_leaf() {
+  LeafRec r{};
+  r.key = EMPTY_KEY;
+  r.first = 0x7fffffff;
+  return r;
+}
 struct LeafTable {
   LeafRec* rec;
   long long mask;
 };
 
-// find-or-insert on the record table; returns slot or -1 when the table is full
-__device__ __forceinline__ long long leaf_insert(const LeafTable& lt, unsigned long long key, bool* fresh) {
-  long long s = hash_slot(key, lt.mask);
-  *fresh = false;
-  for (long long probe = 0; probe <= lt.mask; ++probe) {
-    const unsigned long long cur = lt.rec[s].key;
-    if (cur == key) return s;
-    if (cur == EMPTY_KEY) {
-      const unsigned long long old = atomicCAS(&lt.rec[s].key, EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { *fresh = true; return s; }
-      if (old == key) return s;
-    }
-    s = (s + 1) & lt.mask;
-  }
-  return -1;
-}
-
 struct MapView {
   unsigned long long* keys;
   float* val;
-  float *a, *lo, *hi;   // clamp-add summary since the last reset: f(x) = min(max(x + a, lo), hi)
+  float *a, *lo, *hi;   // clamp-add summary since the last merge: f(x) = min(max(x + a, lo), hi)
   unsigned* rgb;
   int* nleaves;
   long long mask;
@@ -137,22 +128,19 @@ struct MapView {
   unsigned long long* nupd;   // cumulative number of (voxel, keyframe) log-odds updates (bench.py: U of B_map)
 };
 
+// find-or-insert of a voxel, counting the voxels the map holds; false when the map is full.
+__device__ __forceinline__ bool map_slot(const MapView& m, unsigned long long key, long long* s) {
+  bool fresh;
+  const bool found = table_probe<1>(m.keys, m.mask, key, s, &fresh);
+  if (fresh) atomicAdd(m.nleaves, 1);
+  return found;
+}
+
 // Record "keyframe j of the batch observed voxel `key` as occupied / free".  Order-free (atomicOr), so every keyframe
 // of a batch can be scanned in one launch; k_ocm_apply replays the bits of each voxel in keyframe order.
 __device__ __forceinline__ bool map_touch(const MapView& m, unsigned long long key, int j, bool occupied, unsigned rgb) {
-  long long s = hash_slot(key, m.mask);
-  bool found = false;
-  for (long long probe = 0; probe <= m.mask; ++probe) {
-    const unsigned long long cur = m.keys[s];
-    if (cur == key) { found = true; break; }
-    if (cur == EMPTY_KEY) {
-      const unsigned long long old = atomicCAS(&m.keys[s], EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { atomicAdd(m.nleaves, 1); found = true; break; }
-      if (old == key) { found = true; break; }
-    }
-    s = (s + 1) & m.mask;
-  }
-  if (!found) return false;
+  long long s;
+  if (!map_slot(m, key, &s)) return false;
   // Fire and forget: no atomic here returns a value.  (The free-space rays used to wait on the atomicOr's old value to
   // build a list of touched voxels: 35 % of k_ocm_scan_keys' stall samples.  Dirty-block flags instead of the list were
   // worse: the hash scatters a batch over every block, and millions of flag stores / flag reads land on 64 cache lines.
@@ -235,8 +223,12 @@ __global__ void k_ocm_bin(const KfJob* __restrict__ jobs, int* __restrict__ err)
   int slot = -1, rank = 0;
   if (ok && lane == leader) {   // lowest lane of the group = smallest pixel index of the group
     bool fresh;
-    const long long s = leaf_insert(lt, key, &fresh);
-    if (s < 0) { atomicExch(err, 1); }
+    long long s;
+    // Branch on the slot's sign, not on the flag: the compiler cannot fold a sign test into the probe's exits, so the
+    // leader lanes reconverge before the cell atomics below.  Branching on the flag lets them run those atomics
+    // diverged (k_ocm_bin 12 % slower on an H100).
+    if (!table_probe<sizeof(LeafRec) / 8>(&lt.rec->key, lt.mask, key, &s, &fresh)) s = -1;
+    if (s < 0) { atomicExch(err, ERR_LEAF_TABLE_FULL); }
     else {
       slot = (int)s;
       if (fresh) voxlist[atomicAdd(&counters[1], 1)] = slot;   // list of occupied cells: no table sweep later
@@ -316,10 +308,7 @@ __global__ void k_ocm_centroids(const KfJob* __restrict__ jobs) {
   pts_rgb[(size_t)v * 3 + 1] = (uint8_t)(sg / fn);
   pts_rgb[(size_t)v * 3 + 2] = (uint8_t)(sb / fn);
   pts_label[v] = label ? label[lt.rec[s].first] : 0;
-  LeafRec fresh_rec;
-  fresh_rec.key = EMPTY_KEY; fresh_rec.count = 0; fresh_rec.first = 0x7fffffff; fresh_rec.offset = 0; fresh_rec.cursor = 0;
-  fresh_rec.pad[0] = fresh_rec.pad[1] = 0;
-  lt.rec[s] = fresh_rec;
+  lt.rec[s] = empty_leaf();
 }
 
 // leaf <= 0: no VoxelGrid; every gated pixel is a point (used for the T-variant style clouds)
@@ -393,7 +382,7 @@ __global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__
     if (end_ok) {
       const unsigned rgb = (unsigned)pts_rgb[(size_t)v * 3] | ((unsigned)pts_rgb[(size_t)v * 3 + 1] << 8) |
                            ((unsigned)pts_rgb[(size_t)v * 3 + 2] << 16);
-      if (!map_touch(m, pack_key(ke[0], ke[1], ke[2]), j, true, rgb)) atomicExch(err, 4);
+      if (!map_touch(m, pack_key(ke[0], ke[1], ke[2]), j, true, rgb)) atomicExch(err, ERR_MAP_FULL);
     }
     return;
   }
@@ -402,7 +391,7 @@ __global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__
       !coord_to_key(c, c.origin[2], ko[2]))
     return;
   if (ko[0] == ke[0] && ko[1] == ke[1] && ko[2] == ke[2]) return;
-  if (!scan_touch_free(m, s_seen, pack_key(ko[0], ko[1], ko[2]), j)) atomicExch(err, 4);
+  if (!scan_touch_free(m, s_seen, pack_key(ko[0], ko[1], ko[2]), j)) atomicExch(err, ERR_MAP_FULL);
   float dir[3] = {e[0] - c.origin[0], e[1] - c.origin[1], e[2] - c.origin[2]};
   // octomath::Vector3::norm() of octomap 1.9.x: norm_sq() = x*x + y*y + z*z in float, widened for the sqrt only
   const float n2 = __fadd_rn(__fadd_rn(__fmul_rn(dir[0], dir[0]), __fmul_rn(dir[1], dir[1])), __fmul_rn(dir[2], dir[2]));
@@ -438,7 +427,7 @@ __global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__
     const double tmin = a2 ? t01 : tMax[2];
     if (pending) {
       if (tmin > dlen) break;
-      if (!scan_touch_free(m, s_seen, pending_key, j)) { atomicExch(err, 4); break; }
+      if (!scan_touch_free(m, s_seen, pending_key, j)) { atomicExch(err, ERR_MAP_FULL); break; }
     }
     const bool d0 = a2 && a01, d1 = a2 && !a01, d2 = !a2;
     // (no dynamic register indexing, no branches: predicated updates)
@@ -494,71 +483,25 @@ __global__ void k_ocm_apply(float hit_log, float miss_log, float cmin, float cma
   if ((threadIdx.x & 31) == 0 && nup) atomicAdd(m.nupd, (unsigned long long)nup);
 }
 
-__global__ void k_ocm_fill_leaf(LeafRec* p, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  LeafRec r;
-  r.key = EMPTY_KEY; r.count = 0; r.first = 0x7fffffff; r.offset = 0; r.cursor = 0; r.pad[0] = r.pad[1] = 0;
-  p[i] = r;
-}
-__global__ void k_ocm_fill_u64(unsigned long long* p, unsigned long long v, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
-__global__ void k_ocm_fill_i32(int* p, int v, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
-__global__ void k_ocm_fill_f32(float* p, float v, long long n) {
+template <class T>
+__global__ void k_ocm_fill(T* p, T v, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
 }
 
-// export: compact the map (or its summaries) into dense arrays
+// export: compact the map's leaves into dense arrays
 __global__ void k_ocm_export(MapView m, long long* __restrict__ counter, long long cap, unsigned short* __restrict__ keys3,
-                             unsigned long long* __restrict__ keys64, float* __restrict__ val, unsigned char* __restrict__ rgb,
-                             float* __restrict__ a, float* __restrict__ lo, float* __restrict__ hi, int only_touched) {
+                             float* __restrict__ val, unsigned char* __restrict__ rgb) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i > m.mask) return;
   const unsigned long long k = m.keys[i];
   if (k == EMPTY_KEY) return;
-  if (only_touched && m.a[i] == 0.f && m.lo[i] == -INFINITY) return;
   const long long o = (long long)atomicAdd((unsigned long long*)counter, 1ull);
   if (o >= cap) return;
-  if (keys3) { keys3[o * 3] = (unsigned short)(k & 0xffff); keys3[o * 3 + 1] = (unsigned short)((k >> 16) & 0xffff); keys3[o * 3 + 2] = (unsigned short)((k >> 32) & 0xffff); }
-  if (keys64) keys64[o] = k;
-  if (val) val[o] = m.val[i];
-  if (rgb) { const unsigned c = m.rgb[i]; rgb[o * 3] = c & 0xff; rgb[o * 3 + 1] = (c >> 8) & 0xff; rgb[o * 3 + 2] = (c >> 16) & 0xff; }
-  if (a) { a[o] = m.a[i]; lo[o] = m.lo[i]; hi[o] = m.hi[i]; }
-}
-
-// merge: apply a later shard's per-voxel clamp-add summaries onto this map (SURVEY §8(e))
-__global__ void k_ocm_apply_summaries(OcmConst c, MapView m, const unsigned long long* __restrict__ keys,
-                                      const float* __restrict__ a, const float* __restrict__ lo,
-                                      const float* __restrict__ hi, long long n, int* __restrict__ err) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const unsigned long long key = keys[i];
-  long long s = hash_slot(key, m.mask);
-  bool found = false;
-  for (long long probe = 0; probe <= m.mask; ++probe) {
-    const unsigned long long cur = m.keys[s];
-    if (cur == key) { found = true; break; }
-    if (cur == EMPTY_KEY) {
-      const unsigned long long old = atomicCAS(&m.keys[s], EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { atomicAdd(m.nleaves, 1); found = true; break; }
-      if (old == key) { found = true; break; }
-    }
-    s = (s + 1) & m.mask;
-  }
-  if (!found) { atomicExch(err, 4); return; }
-  // value: v <- g(v); summary: f <- g o f  with g = (a, lo, hi)
-  const float ga = a[i], gl = lo[i], gh = hi[i];
-  if (m.a[s] == 0.f && m.lo[s] == -INFINITY) m.elist[atomicAdd(m.nelist, 1)] = (int)s;
-  m.val[s] = fminf(fmaxf(m.val[s] + ga, gl), gh);
-  m.a[s] = m.a[s] + ga;
-  m.lo[s] = fminf(fmaxf(m.lo[s] + ga, gl), gh);
-  m.hi[s] = fminf(fmaxf(m.hi[s] + ga, gl), gh);
+  keys3[o * 3] = (unsigned short)(k & 0xffff); keys3[o * 3 + 1] = (unsigned short)((k >> 16) & 0xffff); keys3[o * 3 + 2] = (unsigned short)((k >> 32) & 0xffff);
+  val[o] = m.val[i];
+  const unsigned c = m.rgb[i];
+  rgb[o * 3] = c & 0xff; rgb[o * 3 + 1] = (c >> 8) & 0xff; rgb[o * 3 + 2] = (c >> 16) & 0xff;
 }
 
 // ---- epoch merge (ocm_merge_nccl) -------------------------------------------------------------------------------------
@@ -597,20 +540,8 @@ __global__ void k_merge_pack(MapView m, int n, MergeShard o) {
 __global__ void k_merge_apply(MapView m, long long n, MergeShard g, int* __restrict__ slots, int* __restrict__ err) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long key = g.keys[i];
-  long long s = hash_slot(key, m.mask);
-  bool found = false;
-  for (long long probe = 0; probe <= m.mask; ++probe) {
-    const unsigned long long cur = m.keys[s];
-    if (cur == key) { found = true; break; }
-    if (cur == EMPTY_KEY) {
-      const unsigned long long old = atomicCAS(&m.keys[s], EMPTY_KEY, key);
-      if (old == EMPTY_KEY) { atomicAdd(m.nleaves, 1); found = true; break; }
-      if (old == key) { found = true; break; }
-    }
-    s = (s + 1) & m.mask;
-  }
-  if (!found) { atomicExch(err, 4); slots[i] = -1; return; }
+  long long s;
+  if (!map_slot(m, g.keys[i], &s)) { atomicExch(err, ERR_MAP_FULL); slots[i] = -1; return; }
   m.val[s] = fminf(fmaxf(m.val[s] + g.a[i], g.lo[i]), g.hi[i]);
   const unsigned c = g.rgb[i];
   if (c != 0xffffffffu) m.rgb[s] = c;
@@ -624,9 +555,11 @@ __global__ void k_merge_commit(MapView m, long long n, const int* __restrict__ s
 }
 
 __global__ void k_ocm_query(MapView m, unsigned long long key, float* out, int* found) {
-  const long long s = table_find(m.keys, m.mask, key);
-  *found = s >= 0;
-  *out = s >= 0 ? m.val[s] : 0.f;
+  bool fresh;
+  long long s;
+  const bool f = table_probe<1, false>(m.keys, m.mask, key, &s, &fresh);
+  *found = f;
+  *out = f ? m.val[s] : 0.f;
 }
 
 }  // namespace b200
@@ -640,29 +573,32 @@ struct ocm {
   cudaStream_t stream = nullptr;
   long long launches = 0;
   float hit_log, miss_log, cmin, cmax;
-  // map
+  // the map and the handle's device words: one allocation (take_block)
+  void* d_block = nullptr;
   MapView map{};
   long long map_cap = 0;
-  // per-keyframe scratch: one slot per keyframe of a batch (grown on demand, self-cleaning between uses)
-  int rows = 0, cols = 0;
   static constexpr int MAX_SLOTS = 32;
-  std::vector<KfScratch> slots;
   int* d_counters = nullptr;          // 4 ints per slot
-  int* d_err = nullptr;
+  int* d_err = nullptr;               // ERR_* of the last failing kernel, 0 = none
+  long long* d_export_counter = nullptr;
+  float* d_query_val = nullptr;       // k_ocm_query's result
+  int* d_query_found = nullptr;
+  // per-keyframe scratch: one slot per keyframe of a batch, one allocation each (grown on demand, self-cleaning
+  // between uses)
+  int rows = 0, cols = 0;
+  std::vector<KfScratch> slots;
   KfJob* d_jobs = nullptr;            // device copy of the running batch, JOB_RING batches deep
   KfJob* h_jobs = nullptr;            // page-locked staging of the same
   static constexpr int JOB_RING = 8;
   cudaEvent_t job_ev[JOB_RING] = {};
   int job_head = 0;
   int last_slot = 0;
-  float* d_depth = nullptr;
-  uint8_t *d_rgb = nullptr, *d_label = nullptr;
-  uint16_t* d_kf_d16 = nullptr;   // staging of ocm_insert_keyframes_u16
-  float* d_kf_depth = nullptr;
-  uint8_t* d_kf_rgb = nullptr;
-  uint8_t* d_kf_label = nullptr;
-  size_t kf_cap = 0;
-  long long* d_export_counter = nullptr;
+  // staging of the host-buffer inserts: one allocation for stage_pix pixels, grown on demand
+  void* d_stage = nullptr;
+  size_t stage_pix = 0;
+  uint16_t* st_d16 = nullptr;         // ocm_insert_keyframes_u16_labeled only
+  float* st_depth = nullptr;
+  uint8_t *st_rgb = nullptr, *st_label = nullptr;
   // ocm_merge_nccl staging (grown on demand)
   void *mg_send = nullptr, *mg_recv = nullptr;
   int* mg_slots = nullptr;
@@ -674,32 +610,34 @@ struct ocm {
   ~ocm() {
     DeviceGuard g(device);
     auto F = [](void* p) { if (p) cudaFree(p); };
-    F(map.keys); F(map.val); F(map.a); F(map.lo); F(map.hi); F(map.rgb); F(map.nleaves); F(map.bm); F(map.bm_rgb);
-    F(map.base); F(map.elist); F(map.nelist); F(map.nupd);
-    F(mg_send); F(mg_recv); F(mg_slots); F(mg_counts);
-    if (mg_counts_h) cudaFreeHost(mg_counts_h);
     free_scratch();
-    F(d_counters); F(d_err); F(d_export_counter); F(d_kf_d16); F(d_kf_depth); F(d_kf_rgb); F(d_kf_label); F(d_jobs);
+    F(d_block); F(d_stage); F(d_jobs); F(mg_send); F(mg_recv); F(mg_slots); F(mg_counts);
+    if (mg_counts_h) cudaFreeHost(mg_counts_h);
     if (h_jobs) cudaFreeHost(h_jobs);
     for (cudaEvent_t e : job_ev) if (e) cudaEventDestroy(e);
     if (stream) cudaStreamDestroy(stream);
   }
-  static void free_slot(KfScratch& k) {
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    F(k.leaf.rec); F(k.pix_slot); F(k.pix_rank); F(k.bucket); F(k.voxlist);
-    F(k.pts); F(k.pts_rgb); F(k.pts_label);
-    k = KfScratch{};
-  }
   void free_scratch() {
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    for (KfScratch& k : slots) free_slot(k);
+    for (KfScratch& k : slots) cudaFree(k.leaf.rec);   // the start of the slot's allocation (ensure_scratch)
     slots.clear();
-    F(d_depth); F(d_rgb); F(d_label);
-    d_depth = nullptr; d_rgb = d_label = nullptr;
+  }
+  // Every array 256-byte aligned by the Carver (k_ocm_apply reads bm in 16-byte words).
+  void take_block(Carver& c) {
+    const long long C = map_cap;
+    map.keys = c.take<unsigned long long>(C); map.val = c.take<float>(C); map.a = c.take<float>(C);
+    map.lo = c.take<float>(C); map.hi = c.take<float>(C); map.rgb = c.take<unsigned>(C); map.nleaves = c.take<int>(1);
+    map.bm = c.take<unsigned long long>(C); map.bm_rgb = c.take<unsigned>(C); map.base = c.take<float>(C);
+    map.elist = c.take<int>(C); map.nelist = c.take<int>(1); map.nupd = c.take<unsigned long long>(1);
+    d_counters = c.take<int>(4 * MAX_SLOTS); d_err = c.take<int>(1); d_export_counter = c.take<long long>(1);
+    d_query_val = c.take<float>(1); d_query_found = c.take<int>(1);
   }
   template <class T>
-  int fill(T* p, T v, long long n);
+  void fill(T* p, T v, long long n) {
+    k_ocm_fill<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, v, n);
+    ++launches;
+  }
   int ensure_scratch(int r, int c, int nslots = 1);
+  int ensure_staging(size_t npix);
   int insert_batch(int n, const float* const* dd, const uint8_t* const* drgb, const uint8_t* const* dlabel, int r, int c,
                    const float* Tcw, float fx, float fy, float cx, float cy);
   int insert(const float* dd, const uint8_t* drgb, const uint8_t* dlabel, int r, int c, const float* Tcw, float fx,
@@ -709,29 +647,23 @@ struct ocm {
   int check_err();
 };
 
-template <>
-int ocm::fill<unsigned long long>(unsigned long long* p, unsigned long long v, long long n) {
-  k_ocm_fill_u64<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, v, n);
-  ++launches;
-  return B200ORB_OK;
-}
-template <>
-int ocm::fill<int>(int* p, int v, long long n) {
-  k_ocm_fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, v, n);
-  ++launches;
-  return B200ORB_OK;
-}
-template <>
-int ocm::fill<float>(float* p, float v, long long n) {
-  k_ocm_fill_f32<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, v, n);
-  ++launches;
-  return B200ORB_OK;
-}
-
 static long long pow2_at_least(long long v) {
   long long p = 1;
   while (p < v) p <<= 1;
   return p;
+}
+
+// One device allocation for a buffer list: `take_all` carves the list, once against a null base to measure it, then
+// out of the new block.  *bytes = the block's size.
+template <class F>
+static int alloc_carved(void** block, F&& take_all, size_t* bytes = nullptr) {
+  Carver probe;
+  take_all(probe);
+  B200_CUDA(cudaMalloc(block, probe.off));
+  Carver c(*block, probe.off);
+  take_all(c);
+  if (bytes) *bytes = probe.off;
+  return B200ORB_OK;
 }
 
 int ocm::ensure_scratch(int r, int c, int nslots) {
@@ -750,18 +682,33 @@ int ocm::ensure_scratch(int r, int c, int nslots) {
   const long long leaf_cap = pow2_at_least(2 * npix);
   while ((int)slots.size() < nslots) {
     KfScratch k{};
-    const int id = (int)slots.size();
+    void* block;
+    B200_CHECK(alloc_carved(&block, [&](Carver& t) {   // the leaf table first: free_scratch frees it
+      k.leaf.rec = t.take<LeafRec>(leaf_cap);
+      k.pix_slot = t.take<int>(npix); k.pix_rank = t.take<int>(npix); k.bucket = t.take<int>(npix);
+      k.voxlist = t.take<int>(npix);
+      k.pts = t.take<float>(3 * npix); k.pts_rgb = t.take<uint8_t>(3 * npix); k.pts_label = t.take<uint8_t>(npix);
+    }));
     k.leaf.mask = leaf_cap - 1;
-    B200_CUDA(cudaMalloc(&k.leaf.rec, sizeof(LeafRec) * leaf_cap));
-    B200_CUDA(cudaMalloc(&k.pix_slot, 4 * npix)); B200_CUDA(cudaMalloc(&k.pix_rank, 4 * npix)); B200_CUDA(cudaMalloc(&k.bucket, 4 * npix));
-    B200_CUDA(cudaMalloc(&k.voxlist, 4 * npix));
-    B200_CUDA(cudaMalloc(&k.pts, 12 * npix)); B200_CUDA(cudaMalloc(&k.pts_rgb, 3 * npix)); B200_CUDA(cudaMalloc(&k.pts_label, npix));
-    k.counters = d_counters + 4 * id;
-    k_ocm_fill_leaf<<<(unsigned)((leaf_cap + 255) / 256), 256, 0, stream>>>(k.leaf.rec, leaf_cap);
-    ++launches;
+    k.counters = d_counters + 4 * slots.size();
+    fill(k.leaf.rec, empty_leaf(), leaf_cap);
     B200_CUDA(cudaGetLastError());
     slots.push_back(k);
   }
+  return B200ORB_OK;
+}
+
+int ocm::ensure_staging(size_t npix) {
+  if (npix <= stage_pix) return B200ORB_OK;
+  B200_CUDA(cudaStreamSynchronize(stream));   // earlier inserts may still read the old staging
+  if (d_stage) cudaFree(d_stage);
+  d_stage = nullptr;
+  stage_pix = 0;
+  B200_CHECK(alloc_carved(&d_stage, [&](Carver& t) {
+    st_d16 = t.take<uint16_t>(npix); st_depth = t.take<float>(npix); st_rgb = t.take<uint8_t>(3 * npix);
+    st_label = t.take<uint8_t>(npix);
+  }));
+  stage_pix = npix;
   return B200ORB_OK;
 }
 
@@ -771,8 +718,8 @@ int ocm::check_err() {
   B200_CUDA(cudaStreamSynchronize(stream));
   if (e) {
     B200_CUDA(cudaMemsetAsync(d_err, 0, 4, stream));
-    static const char* what[] = {"", "VoxelGrid table full", "", "", "map full (raise OcmParams.map_capacity)"};
-    set_error("occupancy insert: %s", what[e < 5 ? e : 0]);
+    set_error("occupancy insert: %s",
+              e == ERR_LEAF_TABLE_FULL ? "VoxelGrid table full" : "map full (raise OcmParams.map_capacity)");
     return B200ORB_ECAP;
   }
   return B200ORB_OK;
@@ -797,10 +744,9 @@ int ocm::insert_batch(int n, const float* const* dd, const uint8_t* const* drgb,
       OcmConst& k = J.c;
       memset(&k, 0, sizeof(k));
       k.fx = fx; k.fy = fy; k.cx = cx; k.cy = cy;
-      k.depth_min = prm.depth_min; k.depth_max = prm.depth_max; k.y_max = prm.y_max; k.leaf = prm.leaf;
+      k.depth_min = prm.depth_min; k.depth_max = prm.depth_max; k.y_max = prm.y_max;
       k.inv_leaf = prm.leaf > 0 ? 1.0f / prm.leaf : 0.f;
       k.res = prm.resolution; k.res_factor = 1.0 / prm.resolution;
-      k.hit_log = hit_log; k.miss_log = miss_log; k.cmin = cmin; k.cmax = cmax;
       double R[9], t[3];
       for (int i = 0; i < 3; ++i) { for (int q = 0; q < 3; ++q) R[i * 3 + q] = (double)Tcw[i * 4 + q]; t[i] = (double)Tcw[i * 4 + 3]; }
       for (int i = 0; i < 3; ++i) {
@@ -876,32 +822,11 @@ int ocm_create(const OcmParams* p, int device, ocm_t** out) {
   }
   const long long C = h->map_cap;
   h->map.mask = C - 1;
-  if ((e = cudaMalloc(&h->map.keys, 8 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.val, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.a, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.lo, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.hi, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.rgb, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.nleaves, 4)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.bm, 8 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.bm_rgb, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.base, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.elist, 4 * C)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.nelist, 4)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->map.nupd, 8)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_counters, 16 * ocm::MAX_SLOTS)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_err, 4)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_export_counter, 8)) != cudaSuccess) return fail(e);
-  h->fill(h->map.keys, EMPTY_KEY, C); h->fill(h->map.val, 0.f, C); h->fill(h->map.a, 0.f, C);
-  h->fill(h->map.lo, -INFINITY, C); h->fill(h->map.hi, INFINITY, C);
+  size_t bytes = 0;
+  if (alloc_carved(&h->d_block, [&](Carver& t) { h->take_block(t); }, &bytes) != B200ORB_OK) { delete h; return B200ORB_ECUDA; }
+  cudaMemsetAsync(h->d_block, 0, bytes, h->stream);
+  h->fill(h->map.keys, EMPTY_KEY, C); h->fill(h->map.lo, -INFINITY, C); h->fill(h->map.hi, INFINITY, C);
   cudaMemsetAsync(h->map.rgb, 0xff, 4 * C, h->stream);
-  cudaMemsetAsync(h->map.nleaves, 0, 4, h->stream);
-  cudaMemsetAsync(h->map.bm, 0, 8 * C, h->stream);
-  cudaMemsetAsync(h->map.bm_rgb, 0, 4 * C, h->stream);
-  cudaMemsetAsync(h->map.base, 0, 4 * C, h->stream);
-  cudaMemsetAsync(h->map.nelist, 0, 4, h->stream);
-  cudaMemsetAsync(h->map.nupd, 0, 8, h->stream);
-  cudaMemsetAsync(h->d_err, 0, 4, h->stream);
   if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return fail(e);
   *out = h;
   return B200ORB_OK;
@@ -935,18 +860,6 @@ int ocm_insert_keyframes_labeled_device(ocm_t* h, const float* d_depth, const ui
   return h->insert_batch(n, dd.data(), dc.data(), d_label ? dl.data() : nullptr, rows, cols, Tcw, fx, fy, cx, cy);
 }
 
-int ocm_insert_keyframes_device(ocm_t* h, const float* d_depth, const uint8_t* d_rgb, int rows, int cols,
-                                const int32_t* depth_idx, const int32_t* rgb_idx, int n, const float* Tcw, float fx,
-                                float fy, float cx, float cy) {
-  return ocm_insert_keyframes_labeled_device(h, d_depth, d_rgb, nullptr, rows, cols, depth_idx, rgb_idx, nullptr, n, Tcw, fx,
-                                             fy, cx, cy);
-}
-
-int ocm_insert_keyframes_u16(ocm_t* h, const uint16_t* depth_u16, const uint8_t* rgb, int rows, int cols, int n,
-                             float depth_factor, const float* Tcw, float fx, float fy, float cx, float cy) {
-  return ocm_insert_keyframes_u16_labeled(h, depth_u16, rgb, nullptr, rows, cols, n, depth_factor, Tcw, fx, fy, cx, cy);
-}
-
 int ocm_insert_keyframes_u16_labeled(ocm_t* h, const uint16_t* depth_u16, const uint8_t* rgb, const uint8_t* label, int rows,
                                      int cols, int n, float depth_factor, const float* Tcw, float fx, float fy, float cx,
                                      float cy) {
@@ -956,23 +869,16 @@ int ocm_insert_keyframes_u16_labeled(ocm_t* h, const uint16_t* depth_u16, const 
   const size_t npix = (size_t)rows * cols, tot = npix * n;
   if ((npix % 4) != 0) { set_error("rows*cols must be a multiple of 4"); return B200ORB_EINVAL; }
   B200_CHECK(h->ensure_scratch(rows, cols));
-  if (tot > h->kf_cap) {   // staging for n keyframes (grown on demand; reused by every later call)
-    B200_CUDA(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_kf_d16); cudaFree(h->d_kf_depth); cudaFree(h->d_kf_rgb); cudaFree(h->d_kf_label);
-    h->d_kf_d16 = nullptr; h->d_kf_depth = nullptr; h->d_kf_rgb = nullptr; h->d_kf_label = nullptr; h->kf_cap = 0;
-    B200_CUDA(cudaMalloc(&h->d_kf_d16, tot * 2)); B200_CUDA(cudaMalloc(&h->d_kf_depth, tot * 4)); B200_CUDA(cudaMalloc(&h->d_kf_rgb, tot * 3));
-    B200_CUDA(cudaMalloc(&h->d_kf_label, tot));
-    h->kf_cap = tot;
-  }
-  if (label) B200_CUDA(cudaMemcpyAsync(h->d_kf_label, label, tot, cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(h->d_kf_d16, depth_u16, tot * 2, cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(h->d_kf_rgb, rgb, tot * 3, cudaMemcpyHostToDevice, h->stream));
+  B200_CHECK(h->ensure_staging(tot));
+  if (label) B200_CUDA(cudaMemcpyAsync(h->st_label, label, tot, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(h->st_d16, depth_u16, tot * 2, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(h->st_rgb, rgb, tot * 3, cudaMemcpyHostToDevice, h->stream));
   k_depth_u16_to_f32<<<(unsigned)((tot / 4 + 255) / 256), 256, 0, h->stream>>>(
-      reinterpret_cast<const ushort4*>(h->d_kf_d16), reinterpret_cast<float4*>(h->d_kf_depth), depth_factor, tot / 4);
+      reinterpret_cast<const ushort4*>(h->st_d16), reinterpret_cast<float4*>(h->st_depth), depth_factor, tot / 4);
   ++h->launches;
   std::vector<const float*> dd(n);
   std::vector<const uint8_t*> dc(n), dl(n);
-  for (int i = 0; i < n; ++i) { dd[i] = h->d_kf_depth + npix * i; dc[i] = h->d_kf_rgb + npix * 3 * i; dl[i] = h->d_kf_label + npix * i; }
+  for (int i = 0; i < n; ++i) { dd[i] = h->st_depth + npix * i; dc[i] = h->st_rgb + npix * 3 * i; dl[i] = h->st_label + npix * i; }
   return h->insert_batch(n, dd.data(), dc.data(), label ? dl.data() : nullptr, rows, cols, Tcw, fx, fy, cx, cy);
 }
 
@@ -982,13 +888,11 @@ int ocm_insert_keyframe(ocm_t* h, const float* depth, const uint8_t* rgb, int ro
   DeviceGuard g(h->device);
   B200_CHECK(h->ensure_scratch(rows, cols));
   const size_t npix = (size_t)rows * cols;
-  if (!h->d_depth) {
-    B200_CUDA(cudaMalloc(&h->d_depth, npix * 4)); B200_CUDA(cudaMalloc(&h->d_rgb, npix * 3)); B200_CUDA(cudaMalloc(&h->d_label, npix));
-  }
-  B200_CUDA(cudaMemcpyAsync(h->d_depth, depth, npix * 4, cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(h->d_rgb, rgb, npix * 3, cudaMemcpyHostToDevice, h->stream));
-  if (ground_label) B200_CUDA(cudaMemcpyAsync(h->d_label, ground_label, npix, cudaMemcpyHostToDevice, h->stream));
-  B200_CHECK(h->insert(h->d_depth, h->d_rgb, ground_label ? h->d_label : nullptr, rows, cols, Tcw, fx, fy, cx, cy));
+  B200_CHECK(h->ensure_staging(npix));
+  B200_CUDA(cudaMemcpyAsync(h->st_depth, depth, npix * 4, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(h->st_rgb, rgb, npix * 3, cudaMemcpyHostToDevice, h->stream));
+  if (ground_label) B200_CUDA(cudaMemcpyAsync(h->st_label, ground_label, npix, cudaMemcpyHostToDevice, h->stream));
+  B200_CHECK(h->insert(h->st_depth, h->st_rgb, ground_label ? h->st_label : nullptr, rows, cols, Tcw, fx, fy, cx, cy));
   return h->check_err();
 }
 
@@ -1018,33 +922,26 @@ int64_t ocm_num_leaves(ocm_t* h) {
   return n;
 }
 
-static int export_common(ocm* h, int64_t cap, int64_t* n, unsigned short* d_k3, unsigned long long* d_k64, float* d_val,
-                         unsigned char* d_rgb, float* d_a, float* d_lo, float* d_hi, int only_touched) {
-  B200_CUDA(cudaMemsetAsync(h->d_export_counter, 0, 8, h->stream));
-  k_ocm_export<<<(unsigned)((h->map_cap + 255) / 256), 256, 0, h->stream>>>(h->map, h->d_export_counter, cap, d_k3, d_k64,
-                                                                          d_val, d_rgb, d_a, d_lo, d_hi, only_touched);
-  ++h->launches;
-  long long cnt = 0;
-  B200_CUDA(cudaMemcpyAsync(&cnt, h->d_export_counter, 8, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaStreamSynchronize(h->stream));
-  if (n) *n = cnt;
-  if (cnt > cap) { set_error("export cap %lld < %lld entries", (long long)cap, cnt); return B200ORB_ECAP; }
-  return B200ORB_OK;
-}
-
 int ocm_export_leaves(ocm_t* h, uint16_t* keys, float* logodds, uint8_t* rgb, int64_t cap, int64_t* n) {
   if (!h || !keys || !logodds || cap < 0) { set_error("bad argument"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
   unsigned short* dk = nullptr; float* dv = nullptr; unsigned char* dc = nullptr;
   const int64_t c = cap > 0 ? cap : 1;
   B200_CUDA(cudaMalloc(&dk, 6 * c)); B200_CUDA(cudaMalloc(&dv, 4 * c)); B200_CUDA(cudaMalloc(&dc, 3 * c));
-  int64_t cnt = 0;
-  int rc = export_common(h, cap, &cnt, dk, nullptr, dv, dc, nullptr, nullptr, nullptr, 0);
-  if (rc == B200ORB_OK) {
+  long long cnt = 0;
+  auto run = [&]() -> int {
+    B200_CUDA(cudaMemsetAsync(h->d_export_counter, 0, 8, h->stream));
+    k_ocm_export<<<(unsigned)((h->map_cap + 255) / 256), 256, 0, h->stream>>>(h->map, h->d_export_counter, cap, dk, dv, dc);
+    ++h->launches;
+    B200_CUDA(cudaMemcpyAsync(&cnt, h->d_export_counter, 8, cudaMemcpyDeviceToHost, h->stream));
+    B200_CUDA(cudaStreamSynchronize(h->stream));
+    if (cnt > cap) { set_error("export cap %lld < %lld entries", (long long)cap, cnt); return B200ORB_ECAP; }
     cudaMemcpy(keys, dk, 6 * cnt, cudaMemcpyDeviceToHost);
     cudaMemcpy(logodds, dv, 4 * cnt, cudaMemcpyDeviceToHost);
     if (rgb) cudaMemcpy(rgb, dc, 3 * cnt, cudaMemcpyDeviceToHost);
-  }
+    return B200ORB_OK;
+  };
+  const int rc = run();
   if (n) *n = cnt;
   cudaFree(dk); cudaFree(dv); cudaFree(dc);
   return rc;
@@ -1060,37 +957,13 @@ int ocm_query(ocm_t* h, const float xyz[3], float* logodds, int* found) {
     if (k[i] < 0 || k[i] >= 65536) { *found = 0; *logodds = 0; return B200ORB_OK; }
   }
   const unsigned long long key = (unsigned long long)k[0] | ((unsigned long long)k[1] << 16) | ((unsigned long long)k[2] << 32);
-  float* dv; int* df;
-  B200_CUDA(cudaMalloc(&dv, 4)); B200_CUDA(cudaMalloc(&df, 4));
-  k_ocm_query<<<1, 1, 0, h->stream>>>(h->map, key, dv, df);
-  ++h->launches;
-  cudaMemcpyAsync(logodds, dv, 4, cudaMemcpyDeviceToHost, h->stream);
-  cudaMemcpyAsync(found, df, 4, cudaMemcpyDeviceToHost, h->stream);
-  cudaStreamSynchronize(h->stream);
-  cudaFree(dv); cudaFree(df);
-  return B200ORB_OK;
-}
-
-int64_t ocm_summary_count(ocm_t* h) { return ocm_num_leaves(h); }
-
-int ocm_export_summaries_device(ocm_t* h, uint64_t* d_keys, float* d_a, float* d_lo, float* d_hi, int64_t cap, int64_t* n) {
-  if (!h || !d_keys || !d_a || !d_lo || !d_hi) { set_error("null argument"); return B200ORB_EINVAL; }
-  DeviceGuard g(h->device);
-  return export_common(h, cap, n, nullptr, (unsigned long long*)d_keys, nullptr, nullptr, d_a, d_lo, d_hi, 1);
-}
-
-int ocm_apply_summaries_device(ocm_t* h, const uint64_t* d_keys, const float* d_a, const float* d_lo, const float* d_hi,
-                               int64_t n) {
-  if (!h || (n > 0 && (!d_keys || !d_a || !d_lo || !d_hi))) { set_error("null argument"); return B200ORB_EINVAL; }
-  if (n <= 0) return B200ORB_OK;
-  DeviceGuard g(h->device);
-  OcmConst k;
-  memset(&k, 0, sizeof(k));
-  k_ocm_apply_summaries<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(k, h->map, (const unsigned long long*)d_keys, d_a,
-                                                                          d_lo, d_hi, n, h->d_err);
+  k_ocm_query<<<1, 1, 0, h->stream>>>(h->map, key, h->d_query_val, h->d_query_found);
   ++h->launches;
   B200_CUDA(cudaGetLastError());
-  return h->check_err();
+  B200_CUDA(cudaMemcpyAsync(logodds, h->d_query_val, 4, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(found, h->d_query_found, 4, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200ORB_OK;
 }
 
 // ---- multi-GPU map merge over NCCL (SURVEY §8(b) ocm_merge_nccl, §8(e)) ---------------------------------------------

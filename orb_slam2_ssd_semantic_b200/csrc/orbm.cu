@@ -26,22 +26,6 @@ int orbm::reserve(size_t bytes) {
 }
 
 namespace {
-// Sequential sub-allocation out of one device block, 256-byte aligned.  Against a null base it only measures: `off` is
-// then the size the same sequence of take() calls needs.  A take() past `cap` returns null and marks the carver overrun.
-struct Carver {
-  char* base;
-  size_t cap, off = 0;
-  bool overrun = false;
-  explicit Carver(void* b = nullptr, size_t c = SIZE_MAX) : base((char*)b), cap(c) {}
-  template <class T>
-  T* take(size_t n) {
-    const size_t at = off;
-    off = align_up_sz(off + std::max<size_t>(n, 1) * sizeof(T), 256);
-    if (off > cap) overrun = true;
-    return (base && !overrun) ? (T*)(base + at) : nullptr;
-  }
-};
-
 // Carves the arena with `take_all`, the entry's complete buffer list: once against a null base to measure, then for
 // real once the arena has grown to that size.
 template <class F>

@@ -1,12 +1,9 @@
 """Multi-GPU plumbing (SURVEY §8(e)): one process per GPU, frames / keyframes sharded in contiguous ranges with no
-data-path collective; the only exchange is the final occupancy-map merge, an all-gather of per-voxel clamp-add
-summaries composed in shard (= keyframe) order.  torch.distributed is plumbing only (NCCL on GPUs, gloo in the CPU
-tests); the map update itself runs in the CUDA kernel behind ocm_apply_summaries_device."""
+data-path collective; the only exchange is the occupancy-map merge, ocm_merge_nccl (PointCloudMapping.merge()), which
+replays the per-voxel clamp-add summaries of every rank in shard (= keyframe) order."""
 from __future__ import annotations
 
-from typing import List, Tuple
-
-import numpy as np
+from typing import Tuple
 
 
 def shard_range(n: int, world: int, rank: int) -> Tuple[int, int]:
@@ -21,79 +18,3 @@ def shard_frames_with_halo(n: int, world: int, rank: int) -> Tuple[int, int, int
     frame begin-1, which the rank re-extracts itself (cheaper than any transfer) -> (halo_begin, begin, end)."""
     b, e = shard_range(n, world, rank)
     return (max(b - 1, 0), b, e)
-
-
-def compose_summaries(a1, lo1, hi1, a2, lo2, hi2):
-    """g o f for clamp-add functions f=(a1,lo1,hi1) applied first, then g=(a2,lo2,hi2):
-    x -> min(max(min(max(x+a1,lo1),hi1)+a2, lo2), hi2) = min(max(x + a1+a2, clip(lo1+a2)), clip(hi1+a2))."""
-    a = a1 + a2
-    lo = np.minimum(np.maximum(lo1 + a2, lo2), hi2)
-    hi = np.minimum(np.maximum(hi1 + a2, lo2), hi2)
-    return a, lo, hi
-
-
-def all_gather_summaries(keys, a, lo, hi, group=None):
-    """All-gather variable-length per-voxel summaries (torch tensors on the backend's device).  Returns a list, one
-    (keys, a, lo, hi) tuple per rank, in rank order."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group)
-    n = torch.tensor([keys.numel()], device=keys.device, dtype=torch.int64)
-    sizes = [torch.zeros_like(n) for _ in range(world)]
-    dist.all_gather(sizes, n, group=group)
-    sizes = [int(s.item()) for s in sizes]
-    m = max(max(sizes), 1)
-
-    def gather(t, dtype):
-        pad = torch.zeros(m, device=t.device, dtype=dtype)
-        pad[: t.numel()] = t
-        outs = [torch.empty_like(pad) for _ in range(world)]
-        dist.all_gather(outs, pad, group=group)
-        return [o[:s] for o, s in zip(outs, sizes)]
-
-    ks = gather(keys.view(torch.int64), torch.int64)
-    as_ = gather(a, torch.float32)
-    los = gather(lo, torch.float32)
-    his = gather(hi, torch.float32)
-    return list(zip(ks, as_, los, his))
-
-
-def merge_occupancy(pcm, group=None, device=None):
-    """Final map merge on GPUs: every rank exports its summaries, NCCL all-gathers them, and every rank applies the
-    shards of the OTHER ranks in rank order onto a fresh composition so all ranks end with the full map.
-    `pcm` is a PointCloudMapping whose map holds only this rank's keyframes (inserted in order)."""
-    import ctypes as C
-
-    import torch
-    import torch.distributed as dist
-
-    from . import _lib
-    from .mapping import PointCloudMapping
-    L = _lib.lib()
-    rank = dist.get_rank(group)
-    world = dist.get_world_size(group)
-    dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
-    n = max(pcm.num_leaves(), 1)
-    keys = torch.empty(n, device=dev, dtype=torch.int64)
-    a = torch.empty(n, device=dev, dtype=torch.float32)
-    lo = torch.empty_like(a)
-    hi = torch.empty_like(a)
-    cnt = C.c_int64(0)
-    _lib.check(L.ocm_export_summaries_device(pcm.handle, C.c_void_p(keys.data_ptr()), C.c_void_p(a.data_ptr()),
-                                             C.c_void_p(lo.data_ptr()), C.c_void_p(hi.data_ptr()), n, C.byref(cnt)))
-    pcm.sync()
-    k = cnt.value
-    shards = all_gather_summaries(keys[:k], a[:k], lo[:k], hi[:k], group)
-    # the gathers ran on torch's current stream; the apply kernels run on the map's own (non-blocking) stream
-    if keys.is_cuda:
-        torch.cuda.current_stream(dev).synchronize()
-    merged = PointCloudMapping(pcm.resolution, pcm.params.prob_hit, pcm.params.prob_miss, pcm.params.clamp_min,
-                               pcm.params.clamp_max, pcm.params.depth_min, pcm.params.depth_max, pcm.params.y_max,
-                               pcm.params.leaf, pcm.params.map_capacity, device=dev.index or 0)
-    for r in range(world):   # keyframe order == rank order
-        ks, as_, los, his = shards[r]
-        if ks.numel():
-            _lib.check(L.ocm_apply_summaries_device(merged.handle, C.c_void_p(ks.data_ptr()), C.c_void_p(as_.data_ptr()),
-                                                    C.c_void_p(los.data_ptr()), C.c_void_p(his.data_ptr()), ks.numel()))
-    merged.sync()
-    return merged, sum(int(s[0].numel()) for s in shards) * 20, rank

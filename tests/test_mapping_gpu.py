@@ -118,8 +118,8 @@ def test_save_octomap_round_trip(oracle, tmp_path):
 
 
 def test_host_u16_keyframe_batch_equals_per_keyframe_inserts(oracle):
-    """ocm_insert_keyframes_u16 (CV_16U depth + colour from host buffers, one asynchronous call) builds the same map as
-    the per-keyframe float-depth inserts and as the oracle."""
+    """ocm_insert_keyframes_u16_labeled (CV_16U depth + colour from host buffers, one asynchronous call) builds the same
+    map as the per-keyframe float-depth inserts and as the oracle."""
     import torch
     from orb_slam2_ssd_semantic_b200 import PointCloudMapping
     scene = _scene(4)
@@ -180,8 +180,8 @@ def test_global_cloud_refilter_matches_oracle(oracle):
 
 
 def test_more_keyframes_than_batch_slots(oracle):
-    """One ocm_insert_keyframes_u16 call with 40 keyframes (the batch masks hold 32: the call is split into rounds and the
-    scratch slots are reused) builds the same map as 40 single inserts."""
+    """One ocm_insert_keyframes_u16_labeled call with 40 keyframes (the batch masks hold 32: the call is split into rounds
+    and the scratch slots are reused) builds the same map as 40 single inserts."""
     from orb_slam2_ssd_semantic_b200 import PointCloudMapping
     base = _scene(5)
     n = 40

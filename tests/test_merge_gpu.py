@@ -1,5 +1,6 @@
-"""GPU, 2 ranks over NCCL: keyframes sharded across GPUs, per-rank occupancy maps merged through the all-gather of
-clamp-add summaries == the sequential single-map result of the CPU oracle (log-odds within 1e-5, same leaf set)."""
+"""GPU, 2 ranks over NCCL: keyframes sharded across GPUs, per-rank occupancy maps merged by ocm_merge_nccl (the
+exchange of per-voxel clamp-add summaries) == the sequential single-map result of the CPU oracle (log-odds within
+1e-5, same leaf set)."""
 import os
 import socket
 
@@ -42,13 +43,14 @@ def _worker(rank, world, port, q):
         scene = _scene(6)
         b, e = D.shard_range(len(scene), world, rank)
         pcm = PointCloudMapping(0.05, device=rank)
+        pcm.nccl_init(rank, world, rank)
         label = np.zeros((480, 640), np.uint8)
         label[320:, :] = 1
         for depth, rgb, T in scene[b:e]:
             pcm.insertKeyFrame(T, depth, rgb, synth.FX, synth.FY, synth.CX, synth.CY, label)
-        merged, nbytes, _ = D.merge_occupancy(pcm, device=torch.device("cuda", rank))
-        keys, lo, _ = merged.export_leaves()
-        q.put((rank, keys, lo, nbytes))
+        st = pcm.merge()
+        keys, lo, _ = pcm.export_leaves()
+        q.put((rank, keys, lo, st.bytes_sent))
     finally:
         dist.destroy_process_group()
 
