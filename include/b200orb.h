@@ -359,38 +359,33 @@ void orbs_destroy(orbs_t* h);
 int orbs_track_batch(orbs_t* h, const uint8_t* gray, const float* depth, const float* Tcw, int nframes,
                      int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp, int32_t* cur2last,
                      int32_t* nmatch, int cap);
-/* Same with the depth image as the sensor delivers it (CV_16U, e.g. TUM PNGs): the conversion
- * imDepth.convertTo(CV_32F, mDepthMapFactor) of Tracking::GrabImageRGBD (src/Tracking.cc:366-367; float multiply by
- * depth_factor = 1.0f / DepthMapFactor) runs on the device, halving the host->device traffic of the depth stream. */
+/* Same with the depth image as the sensor delivers it (CV_16U, e.g. TUM PNGs).  The tracking path reads depth only
+ * under the keypoints (Frame::ComputeStereoFromRGBD, src/Frame.cc:850-871): the device gathers those pixels and converts
+ * them as imDepth.convertTo(CV_32F, mDepthMapFactor) of Tracking::GrabImageRGBD does (src/Tracking.cc:366-367; float
+ * multiply by depth_factor = 1.0f / DepthMapFactor).  When depth_u16 is page-locked host memory (cudaHostAlloc /
+ * cudaHostRegister) the pixels are read in place over PCIe and the depth images are not uploaded at all; pageable
+ * depth is uploaded as CV_16U, half the host->device traffic of f32 depth. */
 int orbs_track_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
                          int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
                          int32_t* cur2last, int32_t* nmatch, int cap);
-/* When depth_u16 is page-locked host memory (cudaHostAlloc / cudaHostRegister) orbs_track_batch_u16 does not upload
- * the depth images at all: the tracking path reads depth only under the keypoints (Frame::ComputeStereoFromRGBD,
- * src/Frame.cc:850-871), so the device gathers those pixels in place over PCIe.  orbs_set_full_depth_upload(h, 1)
- * forces the full upload (then orbs_device_inputs returns the converted f32 batch). */
-int orbs_set_full_depth_upload(orbs_t* h, int on);
 /* Pipelining aid for two handles used alternately: the next batch submitted to h starts its kernels only when the kernels
  * of prev's last submitted batch are done; h's uploads and prev's downloads proceed meanwhile, so the stages upload(k+1) |
  * kernels(k) | download(k-1) overlap without two batches' kernels sharing the SMs.  The dependency is consumed by h's next
  * submit; prev must stay alive until then. */
 int orbs_chain_after(orbs_t* h, orbs_t* prev);
 /* Frames per upload chunk of the host-buffer entries (default 128, at most 7 chunks per call): the extraction of a chunk
- * starts as soon as it has arrived while the next one is still crossing PCIe. */
+ * starts as soon as it has arrived while the next one is still crossing PCIe.  Gray images and any depth that is
+ * uploaded go up chunk by chunk. */
 int orbs_set_chunk_frames(orbs_t* h, int frames);
 /* Streaming form of orbs_track_batch_u16: enqueues uploads, kernels and result downloads on the handle's streams and
  * returns; the outputs are valid after orbs_sync(h).  All host buffers must be page-locked and stay untouched until
- * then.  Two handles used alternately keep two batches in flight, so the upload of batch k+1 and the download of
- * batch k-1 overlap the kernels of batch k (what the reference's grab thread / tracking thread split does for one
- * frame, Examples/RGB-D/rgbd_tum.cc:88-109, done here for whole batches). */
+ * then; depth_u16 is then read in place under the keypoints.  Two handles used alternately keep two batches in
+ * flight, so the upload of batch k+1 and the download of batch k-1 overlap the kernels of batch k (what the reference's
+ * grab thread / tracking thread split does for one frame, Examples/RGB-D/rgbd_tum.cc:88-109, done here for whole
+ * batches). */
 int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
                           int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
                           int32_t* cur2last, int32_t* nmatch, int cap);
-/* convertTo(CV_32F, factor) of n CV_16U pixels resident in HBM (n multiple of 4) on the given cudaStream_t. */
-int b200orb_depth_u16_to_f32_device(const uint16_t* d_src, float* d_dst, size_t n, float factor, void* stream);
-/* Device copies of the inputs of the last host-buffer call (gray u8, depth f32 metres), e.g. to hand keyframes to
- * ocm_insert_keyframes_labeled_device without a second upload. */
-int orbs_device_inputs(orbs_t* h, const uint8_t** d_gray, const float** d_depth);
 /* Device-resident entry (inputs already in HBM, results left in HBM; asynchronous on orbs_stream). */
 int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw,
                             int nframes, int rows, int cols);

@@ -47,6 +47,19 @@ struct Carver {
   }
 };
 
+// One device allocation for a buffer list: `take_all` carves the list, once against a null base to measure it, then
+// out of the new block.  *bytes = the block's size.
+template <class F>
+static int alloc_carved(void** block, F&& take_all, size_t* bytes = nullptr) {
+  Carver probe;
+  take_all(probe);
+  B200_CUDA(cudaMalloc(block, probe.off));
+  Carver c(*block, probe.off);
+  take_all(c);
+  if (bytes) *bytes = probe.off;
+  return B200ORB_OK;
+}
+
 // RAII device guard: every ABI call runs on its handle's device and restores the caller's.
 struct DeviceGuard {
   int prev = -1;

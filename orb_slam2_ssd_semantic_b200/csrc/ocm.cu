@@ -562,6 +562,15 @@ __global__ void k_ocm_query(MapView m, unsigned long long key, float* out, int* 
   *out = f ? m.val[s] : 0.f;
 }
 
+// imDepth.convertTo(CV_32F, mDepthMapFactor) (src/Tracking.cc:366-367): float(u16) * factor, 4 pixels per thread
+__global__ void k_depth_u16_to_f32(const ushort4* __restrict__ src, float4* __restrict__ dst, float factor, size_t n4) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  const ushort4 v = src[i];
+  dst[i] = make_float4(__fmul_rn((float)v.x, factor), __fmul_rn((float)v.y, factor), __fmul_rn((float)v.z, factor),
+                       __fmul_rn((float)v.w, factor));
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -651,19 +660,6 @@ static long long pow2_at_least(long long v) {
   long long p = 1;
   while (p < v) p <<= 1;
   return p;
-}
-
-// One device allocation for a buffer list: `take_all` carves the list, once against a null base to measure it, then
-// out of the new block.  *bytes = the block's size.
-template <class F>
-static int alloc_carved(void** block, F&& take_all, size_t* bytes = nullptr) {
-  Carver probe;
-  take_all(probe);
-  B200_CUDA(cudaMalloc(block, probe.off));
-  Carver c(*block, probe.off);
-  take_all(c);
-  if (bytes) *bytes = probe.off;
-  return B200ORB_OK;
 }
 
 int ocm::ensure_scratch(int r, int c, int nslots) {

@@ -20,7 +20,6 @@ struct GlueOut {     // SoA per frame, stride cap
 // and the AoS -> SoA split the matcher kernel reads.
 __global__ void __launch_bounds__(256) k_frame_glue(const OrbxKeyPoint* __restrict__ kps, const int* __restrict__ nkp,
                                                     int cap, const float* __restrict__ depth,
-                                                    const uint16_t* __restrict__ depth16,
                                                     const uint16_t* __restrict__ kpd16, float depth_factor, int rows,
                                                     int cols, const float* __restrict__ Tcw, float fx, float fy,
                                                     float cx, float cy, float bf, GlueOut o) {
@@ -30,13 +29,10 @@ __global__ void __launch_bounds__(256) k_frame_glue(const OrbxKeyPoint* __restri
   const OrbxKeyPoint kp = kps[g];
   const float* T = Tcw + (size_t)f * 16;
   const float u = kp.x, v = kp.y;
-  // imDepth.at<float>(v,u) (src/Frame.cc:863).  With depth16 the CV_16U sensor image is read in place -- possibly
-  // straight out of pinned host memory over PCIe, one 2-byte read per keypoint instead of uploading 0.6 MB per frame
-  // -- and converted like convertTo(CV_32F, mDepthMapFactor) does (src/Tracking.cc:366-367).
-  const size_t di = (size_t)f * rows * cols + (size_t)(int)v * cols + (int)u;
-  // kpd16: the same CV_16U pixel, already fetched per keypoint by k_depth_prefetch
+  // imDepth.at<float>(v,u) (src/Frame.cc:863).  kpd16: the CV_16U sensor pixel, already fetched per keypoint by
+  // k_depth_prefetch, converted like convertTo(CV_32F, mDepthMapFactor) does (src/Tracking.cc:366-367).
   const float d = kpd16 ? __fmul_rn((float)kpd16[g], depth_factor)
-                        : (depth16 ? __fmul_rn((float)depth16[di], depth_factor) : depth[di]);
+                        : depth[(size_t)f * rows * cols + (size_t)(int)v * cols + (int)u];
   o.x[g] = u; o.y[g] = v; o.ang[g] = kp.angle; o.oct[g] = kp.octave;
   float ur = -1.f, dd = -1.f;
   uint8_t ok = 0;
@@ -106,15 +102,6 @@ __global__ void __launch_bounds__(DEPTH_PF_THREADS) k_depth_prefetch(LevelTab lt
   }
 }
 
-// imDepth.convertTo(CV_32F, mDepthMapFactor) (src/Tracking.cc:366-367): float(u16) * factor, 4 pixels per thread
-__global__ void k_depth_u16_to_f32(const ushort4* __restrict__ src, float4* __restrict__ dst, float factor, size_t n4) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  const ushort4 v = src[i];
-  dst[i] = make_float4(__fmul_rn((float)v.x, factor), __fmul_rn((float)v.y, factor), __fmul_rn((float)v.z, factor),
-                       __fmul_rn((float)v.w, factor));
-}
-
 __global__ void k_fill_i32(int* p, int v, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -122,80 +109,100 @@ __global__ void k_fill_i32(int* p, int v, size_t n) {
 
 }  // namespace b200
 
+// The host-buffer entries upload a batch in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
+constexpr int MAX_CHUNKS = 7;
+
 struct orbs {
   OrbsParams prm{};
   int device = 0;
   orbx* ex = nullptr;
   long long launches = 0;
   int rows = 0, cols = 0, maxF = 0, cap = 0, lastF = 0;
+  // Geometry block, carved for (rows, cols, maxF, cap): the glue's SoA, the match results and the scratch of the
+  // non-fused LAST search.
+  void* d_geom = nullptr;
   float *d_x = nullptr, *d_y = nullptr, *d_ang = nullptr, *d_ur = nullptr, *d_dep = nullptr, *d_xw = nullptr;
   int* d_oct = nullptr;
   uint8_t* d_valid = nullptr;
   int *d_c2l = nullptr, *d_nm = nullptr, *d_acc = nullptr;
-  void* d_match_scratch = nullptr;   // only when the frames take the non-fused LAST search
+  void* d_match_scratch = nullptr;
+  // Host-input block, carved by the first host-buffer call: the uploaded inputs and the depth under the keypoints.
+  void* d_in = nullptr;
+  int in_depth_bytes = 0;   // depth staging per pixel it holds: 4 for f32 input, 2 for pageable CV_16U, 0 for page-locked
   uint8_t* d_gray = nullptr;
-  float *d_depth = nullptr, *d_T = nullptr;
-  uint16_t* d_depth16 = nullptr;
-  bool full_depth_valid = false, force_full_depth_upload = false;
+  float* d_T = nullptr;
+  uint16_t* d_kpd16 = nullptr;    // [maxF][cap] CV_16U depth under the keypoints
+  void* d_depth = nullptr;        // [maxF][rows][cols] uploaded depth, f32 or CV_16U
+  const uint16_t* gather_src = nullptr;   // the CV_16U batch k_depth_prefetch reads during a call
   int chunk_frames = 128;   // frames per upload chunk of the host-buffer entries
   cudaStream_t copy_stream = nullptr;
-  cudaStream_t gather_stream = nullptr;   // in-place depth reads under the keypoints (sparse mode)
+  cudaStream_t gather_stream = nullptr;   // k_depth_prefetch, beside the extractor's stream
+  cudaEvent_t chunk_ev[MAX_CHUNKS] = {};
+  cudaEvent_t inputs_free_ev = nullptr;    // the previous call's kernels are done with the host-input block
   cudaEvent_t sel_ev = nullptr, gather_ev = nullptr;
   cudaEvent_t compute_done_ev = nullptr;   // recorded after the last kernel of a host-buffer batch (before its downloads)
   orbs* chain_prev = nullptr;              // orbs_chain_after: the next batch's kernels wait for that handle's kernels
-  uint16_t* d_kpd16 = nullptr;            // [maxF][cap] depth under the keypoints
-  const uint16_t* sparse_d16 = nullptr;   // device alias of the caller's page-locked depth during a sparse call
-  cudaEvent_t chunk_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool have = false;
-  void free_bufs() {
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    F(d_x); F(d_y); F(d_ang); F(d_ur); F(d_dep); F(d_xw); F(d_oct); F(d_valid); F(d_c2l); F(d_nm); F(d_acc);
-    F(d_match_scratch); F(d_gray); F(d_depth); F(d_T); F(d_depth16); F(d_kpd16);
-    d_depth16 = nullptr; d_kpd16 = nullptr;
-    d_x = d_y = d_ang = d_ur = d_dep = d_xw = nullptr; d_oct = nullptr; d_valid = nullptr;
-    d_c2l = d_nm = d_acc = nullptr; d_match_scratch = nullptr; d_gray = nullptr; d_depth = d_T = nullptr;
-  }
   ~orbs() {
     DeviceGuard g(device);
-    free_bufs();
+    cudaFree(d_geom);
+    cudaFree(d_in);
     if (copy_stream) cudaStreamDestroy(copy_stream);
     if (gather_stream) cudaStreamDestroy(gather_stream);
-    if (sel_ev) cudaEventDestroy(sel_ev);
-    if (compute_done_ev) cudaEventDestroy(compute_done_ev);
-    if (gather_ev) cudaEventDestroy(gather_ev);
     for (cudaEvent_t e : chunk_ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : {inputs_free_ev, sel_ev, gather_ev, compute_done_ev}) if (e) cudaEventDestroy(e);
     delete ex;
   }
-  int ensure(int r, int c, int F, bool host_inputs) {
+  int create_streams() {
+    B200_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
+    B200_CUDA(cudaStreamCreateWithFlags(&gather_stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : chunk_ev) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    for (cudaEvent_t* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev})
+      B200_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    return B200ORB_OK;
+  }
+  // depth_bytes: depth staging per pixel a host-buffer call needs; -1 for the device entry, which needs no host-input
+  // block.  Either block is replaced only after the stream is synchronised: every copy-stream and gather-stream
+  // operation of earlier calls is joined into it by an event.
+  int ensure(int r, int c, int F, int depth_bytes) {
     B200_CHECK(ex->ensure_geometry(r, c, F));
     if (!(r == rows && c == cols && F <= maxF && ex->cap == cap)) {
       B200_CUDA(cudaStreamSynchronize(ex->stream));
-      free_bufs();
-      rows = r; cols = c; maxF = std::max(F, ex->maxF); cap = ex->cap;
-      const size_t n = (size_t)maxF * cap;
-      B200_CUDA(cudaMalloc(&d_x, n * 4)); B200_CUDA(cudaMalloc(&d_y, n * 4)); B200_CUDA(cudaMalloc(&d_ang, n * 4));
-      B200_CUDA(cudaMalloc(&d_ur, n * 4)); B200_CUDA(cudaMalloc(&d_dep, n * 4)); B200_CUDA(cudaMalloc(&d_xw, n * 12));
-      B200_CUDA(cudaMalloc(&d_oct, n * 4)); B200_CUDA(cudaMalloc(&d_valid, n));
-      B200_CUDA(cudaMalloc(&d_c2l, n * 4)); B200_CUDA(cudaMalloc(&d_nm, (size_t)maxF * 4));
-      B200_CUDA(cudaMalloc(&d_acc, n * 4));
-      const size_t scratch = match_last_scratch_bytes(maxF, cap, cap);
-      if (scratch) B200_CUDA(cudaMalloc(&d_match_scratch, scratch));
+      cudaFree(d_geom);
+      cudaFree(d_in);
+      d_geom = d_in = nullptr;
+      rows = 0;   // no geometry until its block exists
+      const int nF = std::max(F, ex->maxF), ncap = ex->cap;
+      const size_t n = (size_t)nF * ncap;
+      B200_CHECK(alloc_carved(&d_geom, [&](Carver& t) {
+        d_x = t.take<float>(n); d_y = t.take<float>(n); d_ang = t.take<float>(n); d_ur = t.take<float>(n);
+        d_dep = t.take<float>(n); d_xw = t.take<float>(3 * n); d_oct = t.take<int>(n); d_valid = t.take<uint8_t>(n);
+        d_c2l = t.take<int>(n); d_nm = t.take<int>(nF); d_acc = t.take<int>(n);
+        d_match_scratch = t.take<char>(match_last_scratch_bytes(nF, ncap, ncap));
+      }));
+      rows = r; cols = c; maxF = nF; cap = ncap;
     }
-    if (host_inputs && !d_gray) {
-      B200_CUDA(cudaMalloc(&d_gray, (size_t)maxF * rows * cols));
-      B200_CUDA(cudaMalloc(&d_depth, (size_t)maxF * rows * cols * 4));
-      B200_CUDA(cudaMalloc(&d_T, (size_t)maxF * 64));
-      B200_CUDA(cudaMalloc(&d_depth16, (size_t)maxF * rows * cols * 2));
-      B200_CUDA(cudaMalloc(&d_kpd16, (size_t)maxF * cap * 2));
+    if (depth_bytes >= 0 && (!d_in || depth_bytes > in_depth_bytes)) {
+      if (d_in) {
+        B200_CUDA(cudaStreamSynchronize(ex->stream));
+        cudaFree(d_in);
+        d_in = nullptr;
+      }
+      const size_t px = (size_t)maxF * rows * cols;
+      B200_CHECK(alloc_carved(&d_in, [&](Carver& t) {
+        d_gray = t.take<uint8_t>(px); d_T = t.take<float>((size_t)maxF * 16);
+        d_kpd16 = t.take<uint16_t>((size_t)maxF * cap); d_depth = t.take<uint8_t>(px * depth_bytes);
+      }));
+      in_depth_bytes = depth_bytes;
     }
     return B200ORB_OK;
   }
-  int run(const uint8_t* dg, const float* dd, const float* dT, int F, const uint16_t* dd16 = nullptr, float factor = 0.f,
-          bool extracted = false, const uint16_t* kpd16 = nullptr) {
+  // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  Depth is the gathered CV_16U
+  // value under each keypoint times `factor` when kpd16 is given, else the f32 image batch dd.
+  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F) {
     cudaStream_t st = ex->stream;
-    if (!extracted) B200_CHECK(ex->run(dg, cols, (size_t)rows * cols, F));
     GlueOut go{d_x, d_y, d_ang, d_ur, d_dep, d_xw, d_oct, d_valid};
-    k_frame_glue<<<dim3((cap + 255) / 256, F), 256, 0, st>>>(ex->d_kps, ex->d_n, cap, dd, dd16, kpd16, factor, rows, cols, dT, prm.fx, prm.fy,
+    k_frame_glue<<<dim3((cap + 255) / 256, F), 256, 0, st>>>(ex->d_kps, ex->d_n, cap, dd, kpd16, factor, rows, cols, dT, prm.fx, prm.fy,
                                                             prm.cx, prm.cy, prm.bf, go);
     ++launches;
     B200_CHECK(ex->prof_mark(ST_GLUE + 1));
@@ -241,6 +248,9 @@ int orbs_create(const OrbsParams* p, int device, orbs_t** out) {
   h->prm = *p;
   h->device = device;
   h->ex = ex;
+  DeviceGuard g(device);
+  const int rc = h->create_streams();
+  if (rc != B200ORB_OK) { delete h; return rc; }
   *out = h;
   return B200ORB_OK;
 }
@@ -250,8 +260,9 @@ int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_dep
                             int rows, int cols) {
   if (!h || !d_gray || !d_depth || !d_Tcw || nframes <= 0 || rows <= 0 || cols <= 0) { set_error("bad argument"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  B200_CHECK(h->ensure(rows, cols, nframes, false));
-  return h->run(d_gray, d_depth, d_Tcw, nframes);
+  B200_CHECK(h->ensure(rows, cols, nframes, -1));
+  B200_CHECK(h->ex->run(d_gray, cols, (size_t)rows * cols, nframes));
+  return h->run(d_depth, nullptr, 0.f, d_Tcw, nframes);
 }
 
 int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d_desc, const int32_t** d_nkp,
@@ -281,7 +292,7 @@ int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, floa
   return B200ORB_OK;
 }
 
-// orbx::after_select hook of the sparse-depth mode: the keypoints of frames [f0, f0 + F) are selected -> fetch the depth
+// orbx::after_select hook of the CV_16U entries: the keypoints of frames [f0, f0 + F) are selected -> fetch the depth
 // under them on the side stream (the stream of the extractor goes on with blur and descriptors meanwhile)
 static int orbs_after_select(void* ctx, int f0, int F) {
   orbs* h = static_cast<orbs*>(ctx);
@@ -291,7 +302,7 @@ static int orbs_after_select(void* ctx, int f0, int F) {
   const long long items = (long long)F * h->cap;
   const int pf_grid = (int)std::min<long long>(DEPTH_PF_CTAS, (items + DEPTH_PF_THREADS - 1) / DEPTH_PF_THREADS);
   k_depth_prefetch<<<pf_grid, DEPTH_PF_THREADS, 0, h->gather_stream>>>(ex->ltab, ex->d_sel, ex->d_selcnt, ex->sel_per_frame, h->cap,
-                                                                       h->sparse_d16, h->rows, h->cols, f0, F, h->d_kpd16);
+                                                                       h->gather_src, h->rows, h->cols, f0, F, h->d_kpd16);
   ++h->launches;
   B200_CUDA(cudaEventRecord(h->gather_ev, h->gather_stream));
   return B200ORB_OK;
@@ -306,72 +317,56 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
     return B200ORB_EINVAL;
   }
   DeviceGuard g(h->device);
-  B200_CHECK(h->ensure(rows, cols, nframes, true));
-  if (cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", cap, h->cap); return B200ORB_ECAP; }
-  cudaStream_t st = h->ex->stream;
-  const size_t px = (size_t)rows * cols, F = nframes;
-  // gray images go up in chunks on a copy stream while the extractor already works on the chunks that have arrived
-  // (PCIe and SMs overlap); everything after extraction runs on the whole batch.
-  if (!h->copy_stream) {
-    B200_CUDA(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-    for (cudaEvent_t& e : h->chunk_ev) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  }
-  const int nchunk = (int)std::min<size_t>(7, (F + h->chunk_frames - 1) / h->chunk_frames);   // >= 64-frame chunks keep each launch wide enough
-  // Page-locked CV_16U depth (cudaHostAlloc / cudaHostRegister, e.g. torch.pin_memory): the only depth pixels the
-  // tracking path ever reads are the ones under the keypoints (Frame::ComputeStereoFromRGBD), so the 0.6 MB/frame
-  // images are never uploaded; the pixels are read in place over PCIe as soon as a chunk's keypoints are selected.
-  const uint16_t* d16_sparse = nullptr;
-  if (depth16 && !h->force_full_depth_upload) {
+  // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
+  // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
+  // Page-locked depth (cudaHostAlloc / cudaHostRegister, e.g. torch.pin_memory) is read in place over PCIe, so its
+  // 0.6 MB/frame images are never uploaded; pageable depth is uploaded next to the gray images and read from HBM.
+  const uint16_t* d16_alias = nullptr;
+  if (depth16) {
     cudaPointerAttributes at;
     void* dev_alias = nullptr;
     if (cudaPointerGetAttributes(&at, depth16) == cudaSuccess && at.type == cudaMemoryTypeHost &&
         cudaHostGetDevicePointer(&dev_alias, const_cast<uint16_t*>(depth16), 0) == cudaSuccess && dev_alias)
-      d16_sparse = reinterpret_cast<const uint16_t*>(dev_alias);
+      d16_alias = reinterpret_cast<const uint16_t*>(dev_alias);
     else
       cudaGetLastError();
   }
-  if (d16_sparse && !h->gather_stream) {
-    B200_CUDA(cudaStreamCreateWithFlags(&h->gather_stream, cudaStreamNonBlocking));
-    B200_CUDA(cudaEventCreateWithFlags(&h->sel_ev, cudaEventDisableTiming));
-    B200_CUDA(cudaEventCreateWithFlags(&h->gather_ev, cudaEventDisableTiming));
-  }
-  h->sparse_d16 = d16_sparse;
-  h->ex->after_select = d16_sparse ? &orbs_after_select : nullptr;
+  const int depth_bytes = depth ? 4 : (d16_alias ? 0 : 2);   // per pixel uploaded
+  const char* depth_up = depth ? (const char*)depth : (const char*)depth16;
+  B200_CHECK(h->ensure(rows, cols, nframes, depth_bytes));
+  if (cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", cap, h->cap); return B200ORB_ECAP; }
+  cudaStream_t st = h->ex->stream;
+  const size_t px = (size_t)rows * cols, F = nframes;
+  // the inputs go up in chunks on a copy stream while the extractor already works on the chunks that have arrived
+  // (PCIe and SMs overlap); everything after extraction runs on the whole batch.
+  const int nchunk = (int)std::min<size_t>(MAX_CHUNKS, (F + h->chunk_frames - 1) / h->chunk_frames);   // >= 64-frame chunks keep each launch wide enough
+  h->gather_src = d16_alias ? d16_alias : static_cast<const uint16_t*>(h->d_depth);
+  h->ex->after_select = depth16 ? &orbs_after_select : nullptr;
   h->ex->after_select_ctx = h;
   {
-    // the copy stream may only overwrite d_gray once the previous call's kernels are done with it
-    B200_CUDA(cudaEventRecord(h->chunk_ev[7], st));
-    B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[7], 0));
+    B200_CUDA(cudaEventRecord(h->inputs_free_ev, st));
+    B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->inputs_free_ev, 0));
     // orbs_chain_after: this batch's kernels start when the other handle's kernels are done -- the uploads enqueued
     // below (copy stream) and that handle's downloads run meanwhile, and kernels of two batches never share the SMs
-    if (h->chain_prev && h->chain_prev->compute_done_ev) B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
+    if (h->chain_prev) B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
     h->chain_prev = nullptr;
     for (int c = 0; c < nchunk; ++c) {
       const size_t f0 = F * c / nchunk, f1 = F * (c + 1) / nchunk;
       B200_CUDA(cudaMemcpyAsync(h->d_gray + px * f0, gray + px * f0, px * (f1 - f0), cudaMemcpyHostToDevice, h->copy_stream));
+      const size_t o = px * f0 * depth_bytes;
+      if (depth_bytes)
+        B200_CUDA(cudaMemcpyAsync((char*)h->d_depth + o, depth_up + o, px * (f1 - f0) * depth_bytes, cudaMemcpyHostToDevice,
+                                  h->copy_stream));
       B200_CUDA(cudaEventRecord(h->chunk_ev[c], h->copy_stream));
       B200_CUDA(cudaStreamWaitEvent(st, h->chunk_ev[c], 0));
       B200_CHECK(h->ex->run(h->d_gray + px * f0, cols, px, (int)(f1 - f0), (int)f0));
     }
   }
   h->ex->after_select = nullptr;
-  h->full_depth_valid = true;
-  if (d16_sparse) {
-    h->full_depth_valid = false;
-    B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
-  } else if (depth16) {
-    if ((px * F) % 4) { set_error("u16 depth path needs rows*cols*nframes to be a multiple of 4"); return B200ORB_EINVAL; }
-    B200_CUDA(cudaMemcpyAsync(h->d_depth16, depth16, px * F * 2, cudaMemcpyHostToDevice, st));
-    const size_t n4 = px * F / 4;
-    k_depth_u16_to_f32<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(reinterpret_cast<const ushort4*>(h->d_depth16),
-                                                                     reinterpret_cast<float4*>(h->d_depth), factor, n4);
-    ++h->launches;
-  } else {
-    B200_CUDA(cudaMemcpyAsync(h->d_depth, depth, px * F * 4, cudaMemcpyHostToDevice, st));
-  }
+  if (depth16) B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
   B200_CUDA(cudaMemcpyAsync(h->d_T, Tcw, F * 64, cudaMemcpyHostToDevice, st));
-  B200_CHECK(h->run(h->d_gray, h->d_depth, h->d_T, nframes, d16_sparse, factor, /*extracted=*/true, d16_sparse ? h->d_kpd16 : nullptr));
-  if (!h->compute_done_ev) B200_CUDA(cudaEventCreateWithFlags(&h->compute_done_ev, cudaEventDisableTiming));
+  B200_CHECK(h->run(depth ? static_cast<const float*>(h->d_depth) : nullptr, depth16 ? h->d_kpd16 : nullptr, factor, h->d_T,
+                    nframes));
   B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
   const size_t hc = h->cap;
   if ((size_t)cap == hc) {
@@ -410,31 +405,7 @@ int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_
                           nmatch, cap, /*wait=*/false);
 }
 
-int orbs_device_inputs(orbs_t* h, const uint8_t** d_gray, const float** d_depth) {
-  if (!h || !h->d_gray) { set_error("no host-buffer call yet"); return B200ORB_EINVAL; }
-  if (d_gray) *d_gray = h->d_gray;
-  if (d_depth) *d_depth = h->full_depth_valid ? h->d_depth : nullptr;   // NULL after a sparse (zero-copy) depth call
-  return B200ORB_OK;
-}
-
-// 1: always upload the whole CV_16U depth batch (device copy available through orbs_device_inputs); 0 (default): read
-// the depth under the keypoints in place when the host buffer is page-locked.
-int orbs_set_full_depth_upload(orbs_t* h, int on) {
-  if (!h) return B200ORB_EINVAL;
-  h->force_full_depth_upload = on != 0;
-  return B200ORB_OK;
-}
-
-// convertTo(CV_32F, factor) of n CV_16U pixels already in HBM (n multiple of 4), on `stream` (cudaStream_t)
-int b200orb_depth_u16_to_f32_device(const uint16_t* d_src, float* d_dst, size_t n, float factor, void* stream) {
-  if (!d_src || !d_dst || (n % 4)) { set_error("bad argument (n must be a multiple of 4)"); return B200ORB_EINVAL; }
-  k_depth_u16_to_f32<<<(unsigned)((n / 4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const ushort4*>(d_src), reinterpret_cast<float4*>(d_dst), factor, n / 4);
-  B200_CUDA(cudaGetLastError());
-  return B200ORB_OK;
-}
-
-// frames per upload chunk of the host-buffer entries (default 128; at most 7 chunks per call): smaller chunks start the
+// frames per upload chunk of the host-buffer entries (default 128; at most MAX_CHUNKS per call): smaller chunks start the
 // extraction earlier, larger ones keep the launches wider
 int orbs_set_chunk_frames(orbs_t* h, int frames) {
   if (!h || frames <= 0) { set_error("bad argument"); return B200ORB_EINVAL; }

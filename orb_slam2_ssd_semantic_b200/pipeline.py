@@ -86,10 +86,6 @@ class StreamTracker:
                                                  F, rows, cols, ptr(kps), ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
         return out
 
-    def set_full_depth_upload(self, on: bool):
-        """False (default): page-locked CV_16U depth is read under the keypoints in place; True: always upload it."""
-        _lib.check(self._L.orbs_set_full_depth_upload(self._h, int(on)))
-
     def set_chunk_frames(self, frames: int):
         """Frames per upload chunk of the host-buffer calls (default 128)."""
         _lib.check(self._L.orbs_set_chunk_frames(self._h, int(frames)))
@@ -97,12 +93,6 @@ class StreamTracker:
     def chain_after(self, prev: "StreamTracker"):
         """The next submitted batch starts its kernels when `prev`'s kernels are done (uploads are not held back)."""
         _lib.check(self._L.orbs_chain_after(self._h, prev._h))
-
-    def device_inputs(self):
-        """(d_gray, d_depth) device pointers of the last host-buffer batch (depth as f32 metres)."""
-        g, d = C.c_void_p(), C.c_void_p()
-        _lib.check(self._L.orbs_device_inputs(self._h, C.byref(g), C.byref(d)))
-        return g.value, d.value
 
     def track_batch_device(self, d_gray: int, d_depth: int, d_Tcw: int, nframes: int, rows: int, cols: int):
         """Device pointers (ints) in; results stay in HBM (device_results()). Asynchronous."""

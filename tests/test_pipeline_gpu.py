@@ -74,30 +74,46 @@ def test_u16_depth_path_equals_float_path():
     assert b[4][1:].min() > 100
 
 
-def test_u16_depth_zero_copy_gather_from_pinned_memory():
-    """Page-locked CV_16U depth is gathered under the keypoints in place (no depth upload); results equal the
-    full-upload path, and orbs_device_inputs reports no device depth copy in that mode."""
-    import torch
-    from orb_slam2_ssd_semantic_b200 import StreamTracker
-    F = 3
-    ws = synth.WallStream(seed=78, n=F)
+def _u16_batch(seed, F, **geom):
+    ws = synth.WallStream(seed=seed, n=F, **geom)
     frames = [ws.frame(t) for t in range(F)]
     gray = np.stack([f[0] for f in frames])
     depth = np.stack([f[1] for f in frames])
     T = np.stack([f[3] for f in frames])
     d16 = np.rint(depth.astype(np.float64) * synth.DEPTH_FACTOR).astype(np.uint16)
     factor = np.float32(1.0 / synth.DEPTH_FACTOR)
-    st = StreamTracker(1000, 1.2, 8, 20, 7, synth.FX, synth.FY, synth.CX, synth.CY, synth.BF)
-    a = st.track_batch_u16(gray, d16, factor, T)                       # pageable numpy -> full upload
-    assert st.device_inputs()[1] is not None
+    return gray, d16, d16.astype(np.float32) * factor, factor, T
+
+
+def test_host_depth_kinds_equal_on_one_handle():
+    """One handle fed page-locked CV_16U depth (read in place under the keypoints), pageable CV_16U depth (uploaded,
+    then gathered), f32 depth and page-locked CV_16U again: the depth staging of the handle grows between the calls,
+    and every output is byte-identical across the four."""
+    import torch
+    from orb_slam2_ssd_semantic_b200 import StreamTracker
+    gray, d16, depth, factor, T = _u16_batch(78, 3)
     pinned = torch.from_numpy(d16).pin_memory()
-    b = st.track_batch_u16(gray, pinned.numpy(), factor, T)            # page-locked -> in-place gather
-    assert st.device_inputs()[1] is None
-    st.set_full_depth_upload(True)
-    c = st.track_batch_u16(gray, pinned.numpy(), factor, T)
-    assert st.device_inputs()[1] is not None
-    for x, y, z in zip(a, b, c):
-        assert x.tobytes() == y.tobytes() == z.tobytes()
+    st = StreamTracker(1000, 1.2, 8, 20, 7, synth.FX, synth.FY, synth.CX, synth.CY, synth.BF)
+    outs = [st.track_batch_u16(gray, pinned.numpy(), factor, T), st.track_batch_u16(gray, d16, factor, T),
+            st.track_batch(gray, depth, T), st.track_batch_u16(gray, pinned.numpy(), factor, T)]
+    for o in outs[1:]:
+        for x, y in zip(outs[0], o):
+            assert x.tobytes() == y.tobytes()
+    assert outs[0][4][1:].min() > 100
+
+
+def test_u16_pageable_depth_odd_pixel_count():
+    """Pageable CV_16U depth whose batch holds an odd number of pixels (3 x 401 x 533) == orbs_track_batch on the
+    matching f32 depth."""
+    from orb_slam2_ssd_semantic_b200 import StreamTracker
+    gray, d16, depth, factor, T = _u16_batch(79, 3, h=401, w=533)
+    assert d16.size % 4
+    st = StreamTracker(1000, 1.2, 8, 20, 7, synth.FX, synth.FY, synth.CX, synth.CY, synth.BF)
+    a = st.track_batch(gray, depth, T)
+    b = st.track_batch_u16(gray, d16, factor, T)
+    for x, y in zip(a, b):
+        assert x.tobytes() == y.tobytes()
+    assert b[4][1:].min() > 50
 
 
 @pytest.mark.gpu

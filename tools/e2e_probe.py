@@ -40,6 +40,8 @@ def dev():
     st.track_batch_device(gray.data_ptr(), depth.data_ptr(), T.data_ptr(), F, 480, 640); st.sync()
 def host():
     st.track_batch_u16(p_gray.numpy(), p_d16.numpy(), factor, p_T.numpy(), out)
+def host_pageable_depth():
+    st.track_batch_u16(p_gray.numpy(), d16_h, factor, p_T.numpy(), out)
 def kdev():
     pcm.insert_keyframes_device(depth.data_ptr(), rgb.data_ptr(), 480, 640, kfs, Th[kfs], synth.FX, synth.FY, synth.CX, synth.CY,
                                 d_label=lab.data_ptr()); pcm.sync()
@@ -50,10 +52,8 @@ def h2d():
 dback = [torch.empty(a.shape, dtype=torch.uint8).pin_memory() if False else None for a in ()]
 
 timeit("tracker, inputs resident", dev)
-timeit("tracker, host buffers (zero-copy depth)", host)
-st.set_full_depth_upload(True)
-timeit("tracker, host buffers (full depth upload)", host)
-st.set_full_depth_upload(False)
+timeit("tracker, host buffers (page-locked depth)", host)
+timeit("tracker, host buffers (pageable depth)", host_pageable_depth)
 timeit("gray H2D alone (%.1f MB)" % (gray_h.nbytes / 1e6), h2d)
 timeit("mapper, inputs resident (%d kf)" % len(kfs), kdev)
 timeit("mapper, host buffers", khost)
