@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <stdio.h>
 #include <string.h>
+#include <utility>
 
 #include "../../include/b200orb.h"
 
@@ -47,18 +48,96 @@ struct Carver {
   }
 };
 
-// One device allocation for a buffer list: `take_all` carves the list, once against a null base to measure it, then
-// out of the new block.  *bytes = the block's size.
-template <class F>
-static int alloc_carved(void** block, F&& take_all, size_t* bytes = nullptr) {
-  Carver probe;
-  take_all(probe);
-  B200_CUDA(cudaMalloc(block, probe.off));
-  Carver c(*block, probe.off);
-  take_all(c);
-  if (bytes) *bytes = probe.off;
-  return B200ORB_OK;
+// One allocation holding a buffer list, device (cudaMalloc) or page-locked host (cudaHostAlloc) memory.  `take_all`
+// carves the list: once against a null base to measure it, which also nulls every buffer pointer, then out of the
+// block.  A block is replaced only after `stream`, the last stream that used it, is synchronised, and `bytes` is set
+// only once its allocation exists: after a failed allocation the block is empty and the next call allocates again.
+// The destructor frees without a stream: cudaFree and cudaFreeHost synchronise with the device.
+template <bool PINNED>
+struct Block {
+  void* p = nullptr;
+  size_t bytes = 0;
+  Block() = default;
+  Block(Block&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  Block& operator=(Block&& o) noexcept {   // swaps: `o` frees the old block
+    std::swap(p, o.p);
+    std::swap(bytes, o.bytes);
+    return *this;
+  }
+  ~Block() { release(); }
+  // exactly the size of the list
+  template <class F>
+  int carve(cudaStream_t stream, F&& take_all) {
+    Carver probe;
+    take_all(probe);
+    return alloc(stream, probe.off, take_all);
+  }
+  // grow-only: re-carved in place when the list fits, else grown to 1.5x the list, rounded up to 1 MiB
+  template <class F>
+  int reserve(cudaStream_t stream, F&& take_all) {
+    Carver probe;
+    take_all(probe);
+    if (probe.off > bytes) return alloc(stream, align_up_sz(probe.off + probe.off / 2, 1 << 20), take_all);
+    return cut(take_all);
+  }
+
+ private:
+  void release() {
+    if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    bytes = 0;
+  }
+  template <class F>
+  int alloc(cudaStream_t stream, size_t n, F& take_all) {
+    if (p) {
+      B200_CUDA(cudaStreamSynchronize(stream));
+      release();
+    }
+    void* q = nullptr;
+    B200_CUDA(PINNED ? cudaHostAlloc(&q, n, cudaHostAllocDefault) : cudaMalloc(&q, n));
+    p = q;
+    bytes = n;
+    return cut(take_all);
+  }
+  template <class F>
+  int cut(F& take_all) {
+    Carver c(p, bytes);
+    take_all(c);
+    if (c.overrun) { set_error("buffer list larger than its block"); return B200ORB_EINVAL; }
+    return B200ORB_OK;
+  }
+};
+using DeviceBlock = Block<false>;
+using HostBlock = Block<true>;
+
+// A stream or event, created once and destroyed with its owner.  create(): a stream is non-blocking, `arg` is its
+// priority; an event records timing only when `arg` is nonzero.
+static inline cudaError_t cuda_create(cudaStream_t* s, int priority) {
+  return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority);
 }
+static inline cudaError_t cuda_create(cudaEvent_t* e, int timing) {
+  return cudaEventCreateWithFlags(e, timing ? cudaEventDefault : cudaEventDisableTiming);
+}
+static inline void cuda_destroy(cudaStream_t s) { cudaStreamDestroy(s); }
+static inline void cuda_destroy(cudaEvent_t e) { cudaEventDestroy(e); }
+template <class T>
+struct Owned {
+  T h = nullptr;
+  Owned() = default;
+  Owned(Owned&& o) noexcept : h(o.h) { o.h = nullptr; }
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() {
+    if (h) cuda_destroy(h);
+  }
+  int create(int arg = 0) {
+    B200_CUDA(cuda_create(&h, arg));
+    return B200ORB_OK;
+  }
+  operator T() const { return h; }
+};
+using Stream = Owned<cudaStream_t>;
+using Event = Owned<cudaEvent_t>;
 
 // RAII device guard: every ABI call runs on its handle's device and restores the caller's.
 struct DeviceGuard {
@@ -72,6 +151,14 @@ struct DeviceGuard {
     if (prev >= 0) cudaSetDevice(prev);
   }
 };
+
+// Every *_destroy: the handle's members free themselves, on its device.
+template <class H>
+static void destroy_handle(H* h) {
+  if (!h) return;
+  DeviceGuard g(h->device);
+  delete h;
+}
 
 int check_device(int device);   // B200ORB_OK or ENOGPU/EINVAL with message
 

@@ -11,6 +11,7 @@
 // against cv2 4.13 (tools/make_dynmask_golden.py -> tests/golden/dynmask_*.npz).
 #include <math.h>
 
+#include <memory>
 #include <new>
 
 #include "common.cuh"
@@ -148,22 +149,20 @@ using namespace b200;
 
 struct dynm {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   long long launches = 0;
   EllipseTab tab;
-  void* d_buf = nullptr;
-  size_t buf_bytes = 0;
-  ~dynm() {
-    DeviceGuard g(device);
-    if (d_buf) cudaFree(d_buf);
-    if (stream) cudaStreamDestroy(stream);
-  }
-  int reserve(size_t need) {
-    if (need <= buf_bytes) return B200ORB_OK;
-    if (d_buf) { cudaStreamSynchronize(stream); cudaFree(d_buf); d_buf = nullptr; buf_bytes = 0; }
-    B200_CUDA(cudaMalloc(&d_buf, need));
-    buf_bytes = need;
-    return B200ORB_OK;
+  DeviceBlock buf;   // each entry carves its buffer list out of it
+};
+
+struct FilterScratch {   // dynm_filter_core's outputs before they are copied back over the inputs
+  unsigned long long* sums;
+  OrbxKeyPoint* kps;
+  uint8_t* desc;
+  int* cnt;
+  void take(Carver& c, int F, int cap) {
+    sums = c.take<unsigned long long>(F); kps = c.take<OrbxKeyPoint>((size_t)F * cap);
+    desc = c.take<uint8_t>((size_t)F * cap * 32); cnt = c.take<int>(F);
   }
 };
 
@@ -183,26 +182,16 @@ static int dynm_mask_core(dynm* h, const float* d_flow, int F, int rows, int col
 }
 
 static int dynm_filter_core(dynm* h, const uint8_t* d_mask, int F, int rows, int cols, OrbxKeyPoint* d_kps, uint8_t* d_desc,
-                            int32_t* d_counts, int cap, char* scratch) {
-  // scratch: sums [F] u64, kps [F][cap], desc [F][cap][32], counts [F]
-  unsigned long long* d_sums = (unsigned long long*)scratch; scratch += align_up_sz((size_t)F * 8, 256);
-  OrbxKeyPoint* t_kps = (OrbxKeyPoint*)scratch; scratch += align_up_sz((size_t)F * cap * sizeof(OrbxKeyPoint), 256);
-  uint8_t* t_desc = (uint8_t*)scratch; scratch += align_up_sz((size_t)F * cap * 32, 256);
-  int* t_cnt = (int*)scratch;
-  B200_CUDA(cudaMemsetAsync(d_sums, 0, (size_t)F * 8, h->stream));
-  k_dynm_mask_sum<<<dim3(64, F), 256, 0, h->stream>>>(d_mask, (size_t)rows * cols, d_sums);
-  k_dynm_filter<<<F, 256, 0, h->stream>>>(d_mask, rows, cols, d_sums, d_kps, d_desc, d_counts, cap, t_kps, t_desc, t_cnt);
+                            int32_t* d_counts, int cap, const FilterScratch& t) {
+  B200_CUDA(cudaMemsetAsync(t.sums, 0, (size_t)F * 8, h->stream));
+  k_dynm_mask_sum<<<dim3(64, F), 256, 0, h->stream>>>(d_mask, (size_t)rows * cols, t.sums);
+  k_dynm_filter<<<F, 256, 0, h->stream>>>(d_mask, rows, cols, t.sums, d_kps, d_desc, d_counts, cap, t.kps, t.desc, t.cnt);
   h->launches += 2;
   B200_CUDA(cudaGetLastError());
-  B200_CUDA(cudaMemcpyAsync(d_kps, t_kps, (size_t)F * cap * sizeof(OrbxKeyPoint), cudaMemcpyDeviceToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(d_desc, t_desc, (size_t)F * cap * 32, cudaMemcpyDeviceToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(d_counts, t_cnt, (size_t)F * 4, cudaMemcpyDeviceToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d_kps, t.kps, (size_t)F * cap * sizeof(OrbxKeyPoint), cudaMemcpyDeviceToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d_desc, t.desc, (size_t)F * cap * 32, cudaMemcpyDeviceToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d_counts, t.cnt, (size_t)F * 4, cudaMemcpyDeviceToDevice, h->stream));
   return B200ORB_OK;
-}
-
-static size_t dynm_filter_scratch(int F, int cap) {
-  return align_up_sz((size_t)F * 8, 256) + align_up_sz((size_t)F * cap * sizeof(OrbxKeyPoint), 256) +
-         align_up_sz((size_t)F * cap * 32, 256) + align_up_sz((size_t)F * 4, 256);
 }
 
 extern "C" {
@@ -212,7 +201,7 @@ int dynm_create(int device, dynm_t** out) {
   *out = nullptr;
   B200_CHECK(check_device(device));
   DeviceGuard g(device);
-  dynm* h = new (std::nothrow) dynm();
+  std::unique_ptr<dynm> h(new (std::nothrow) dynm());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
   h->device = device;
   // cv::getStructuringElement(MORPH_ELLIPSE, Size(21, 21)): row i spans c - dx .. c + dx, dx = cvRound(c sqrt((r^2 - dy^2) / r^2))
@@ -222,14 +211,13 @@ int dynm_create(int device, dynm_t** out) {
     const int dy = i - r;
     h->tab.hw[i] = (int)lrint(c * sqrt((double)(r * r - dy * dy) * inv_r2));
   }
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { set_error("dynm_create: %s", cudaGetErrorString(e)); delete h; return B200ORB_ECUDA; }
-  *out = h;
+  B200_CHECK(h->stream.create());
+  *out = h.release();
   return B200ORB_OK;
 }
-void dynm_destroy(dynm_t* h) { delete h; }
+void dynm_destroy(dynm_t* h) { destroy_handle(h); }
 long long dynm_launch_count(const dynm_t* h) { return h ? h->launches : 0; }
-void* dynm_stream(dynm_t* h) { return h ? (void*)h->stream : nullptr; }
+void* dynm_stream(dynm_t* h) { return h ? (void*)(cudaStream_t)h->stream : nullptr; }
 int dynm_sync(dynm_t* h) {
   if (!h) { set_error("bad argument"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
@@ -259,8 +247,9 @@ int dynm_mask_from_flow_batch_device(dynm_t* h, const float* d_flow, int nframes
   if (nframes == 0) return B200ORB_OK;
   B200_CHECK(dynm_check_geometry(rows, cols, mask_rows, mask_cols));
   DeviceGuard g(h->device);
-  B200_CHECK(h->reserve((size_t)nframes * mask_rows * mask_cols));
-  return dynm_mask_core(h, d_flow, nframes, rows, cols, binary_threshold, d_mask, (uint8_t*)h->d_buf, mask_rows, mask_cols);
+  uint8_t* d_tmp;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) { d_tmp = t.take<uint8_t>((size_t)nframes * mask_rows * mask_cols); }));
+  return dynm_mask_core(h, d_flow, nframes, rows, cols, binary_threshold, d_mask, d_tmp, mask_rows, mask_cols);
 }
 
 int dynm_mask_from_flow(dynm_t* h, const float* flow, int rows, int cols, float binary_threshold, uint8_t* mask, int mask_rows,
@@ -268,11 +257,12 @@ int dynm_mask_from_flow(dynm_t* h, const float* flow, int rows, int cols, float 
   if (!h || !flow || !mask) { set_error("bad argument"); return B200ORB_EINVAL; }
   B200_CHECK(dynm_check_geometry(rows, cols, mask_rows, mask_cols));
   DeviceGuard g(h->device);
-  const size_t fb = align_up_sz((size_t)rows * cols * 8, 256), mb = align_up_sz((size_t)mask_rows * mask_cols, 256);
-  B200_CHECK(h->reserve(fb + 2 * mb));
-  float* d_flow = (float*)h->d_buf;
-  uint8_t* d_mask = (uint8_t*)h->d_buf + fb;
-  uint8_t* d_tmp = d_mask + mb;
+  float* d_flow;
+  uint8_t *d_mask, *d_tmp;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) {
+    d_flow = t.take<float>((size_t)rows * cols * 2);
+    d_mask = t.take<uint8_t>((size_t)mask_rows * mask_cols); d_tmp = t.take<uint8_t>((size_t)mask_rows * mask_cols);
+  }));
   B200_CUDA(cudaMemcpyAsync(d_flow, flow, (size_t)rows * cols * 8, cudaMemcpyHostToDevice, h->stream));
   B200_CHECK(dynm_mask_core(h, d_flow, 1, rows, cols, binary_threshold, d_mask, d_tmp, mask_rows, mask_cols));
   B200_CUDA(cudaMemcpyAsync(mask, d_mask, (size_t)mask_rows * mask_cols, cudaMemcpyDeviceToHost, h->stream));
@@ -289,8 +279,9 @@ int dynm_filter_keypoints_batch_device(dynm_t* h, const uint8_t* d_mask, int nfr
   if (nframes == 0 || cap == 0) return B200ORB_OK;
   if (rows < 1 || cols < 1) { set_error("empty mask"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  B200_CHECK(h->reserve(dynm_filter_scratch(nframes, cap)));
-  return dynm_filter_core(h, d_mask, nframes, rows, cols, d_kps, d_desc, d_counts, cap, (char*)h->d_buf);
+  FilterScratch fs;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) { fs.take(t, nframes, cap); }));
+  return dynm_filter_core(h, d_mask, nframes, rows, cols, d_kps, d_desc, d_counts, cap, fs);
 }
 
 int dynm_filter_keypoints(dynm_t* h, const uint8_t* mask, int rows, int cols, size_t stride, OrbxKeyPoint* kps, uint8_t* desc,
@@ -300,19 +291,20 @@ int dynm_filter_keypoints(dynm_t* h, const uint8_t* mask, int rows, int cols, si
   if (n == 0) return B200ORB_OK;   // :379 the constructor returns on an empty frame either way
   if (rows < 1 || cols < 1 || stride < (size_t)cols) { set_error("bad mask geometry"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  const size_t mb = align_up_sz((size_t)rows * cols, 256), kb = align_up_sz((size_t)n * sizeof(OrbxKeyPoint), 256),
-               db = align_up_sz((size_t)n * 32, 256);
-  B200_CHECK(h->reserve(mb + kb + db + 256 + dynm_filter_scratch(1, n)));
-  char* p = (char*)h->d_buf;
-  uint8_t* d_mask = (uint8_t*)p; p += mb;
-  OrbxKeyPoint* d_kps = (OrbxKeyPoint*)p; p += kb;
-  uint8_t* d_desc = (uint8_t*)p; p += db;
-  int32_t* d_cnt = (int32_t*)p; p += 256;
+  uint8_t *d_mask, *d_desc;
+  OrbxKeyPoint* d_kps;
+  int32_t* d_cnt;
+  FilterScratch fs;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) {
+    d_mask = t.take<uint8_t>((size_t)rows * cols); d_kps = t.take<OrbxKeyPoint>(n); d_desc = t.take<uint8_t>((size_t)n * 32);
+    d_cnt = t.take<int32_t>(1);
+    fs.take(t, 1, n);
+  }));
   B200_CUDA(cudaMemcpy2DAsync(d_mask, cols, mask, stride, cols, rows, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(d_kps, kps, (size_t)n * sizeof(OrbxKeyPoint), cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(d_desc, desc, (size_t)n * 32, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(d_cnt, &n, 4, cudaMemcpyHostToDevice, h->stream));
-  B200_CHECK(dynm_filter_core(h, d_mask, 1, rows, cols, d_kps, d_desc, d_cnt, n, p));
+  B200_CHECK(dynm_filter_core(h, d_mask, 1, rows, cols, d_kps, d_desc, d_cnt, n, fs));
   int m = 0;
   B200_CUDA(cudaMemcpyAsync(&m, d_cnt, 4, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));

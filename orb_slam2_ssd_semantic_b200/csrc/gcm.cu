@@ -10,6 +10,7 @@
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
+#include <memory>
 #include <new>
 
 #include "common.cuh"
@@ -128,64 +129,39 @@ __global__ void k_gcm_centroids(const int* __restrict__ idx_sorted, const int* _
 
 using namespace b200;
 
-// reallocate p to `count` elements, keeping the first `keep`
-template <class T>
-static cudaError_t gcm_grow(T*& p, long long count, long long keep) {
-  T* q = nullptr;
-  cudaError_t e = cudaMalloc(&q, sizeof(T) * (size_t)count);
-  if (e != cudaSuccess) return e;
-  if (p && keep > 0) e = cudaMemcpy(q, p, sizeof(T) * (size_t)keep, cudaMemcpyDeviceToDevice);
-  if (p) cudaFree(p);
-  p = q;
-  return e;
-}
-
 struct gcm {
   int device = 0;
   int sms = 1;
   float leaf = 0.f;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   long long launches = 0;
-  long long n = 0, cap = 0;   // points in the global map / capacity of the point buffers
-  float *d_xyz = nullptr, *d_xyz2 = nullptr;
-  uint8_t *d_rgb = nullptr, *d_rgb2 = nullptr;
-  int *d_idx = nullptr, *d_idx2 = nullptr, *d_pos = nullptr, *d_pos2 = nullptr, *d_starts = nullptr;
-  uint8_t* d_head = nullptr;
+  long long n = 0, cap = 0;   // points in the global map / capacity of the point block
+  DeviceBlock words;
   unsigned* d_mm = nullptr;
   int* d_flag = nullptr;      // [0] overflow, [1] number of cells
   double* d_T = nullptr;      // Rt (9) + ti (3)
-  void* d_tmp = nullptr;
-  size_t tmp_bytes = 0;
-  float* d_in_depth = nullptr;   // staging of the host entry
-  uint8_t* d_in_rgb = nullptr;
-  size_t in_px = 0;
-  ~gcm() {
-    DeviceGuard g(device);
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    F(d_xyz); F(d_xyz2); F(d_rgb); F(d_rgb2); F(d_idx); F(d_idx2); F(d_pos); F(d_pos2); F(d_starts); F(d_head); F(d_mm);
-    F(d_flag); F(d_T); F(d_tmp); F(d_in_depth); F(d_in_rgb);
-    if (stream) cudaStreamDestroy(stream);
-  }
+  DeviceBlock points;         // two sets of `cap` points: the map, and gcm_refilter's output
+  float *d_xyz = nullptr, *d_xyz2 = nullptr;
+  uint8_t *d_rgb = nullptr, *d_rgb2 = nullptr;
+  DeviceBlock sort;           // gcm_refilter's sort of the map and its CUB scratch
+  DeviceBlock stage;          // gcm_add_keyframe's uploads
   int reserve(long long need) {
     if (need <= cap) return B200ORB_OK;
-    long long nc = std::max<long long>(need, cap * 2);
-    B200_CUDA(cudaStreamSynchronize(stream));
-    B200_CUDA(gcm_grow(d_xyz, 3 * nc, 3 * n)); B200_CUDA(gcm_grow(d_rgb, 3 * nc, 3 * n));
-    B200_CUDA(gcm_grow(d_xyz2, 3 * nc, 0)); B200_CUDA(gcm_grow(d_rgb2, 3 * nc, 0));
-    B200_CUDA(gcm_grow(d_idx, nc, 0)); B200_CUDA(gcm_grow(d_idx2, nc, 0)); B200_CUDA(gcm_grow(d_pos, nc, 0)); B200_CUDA(gcm_grow(d_pos2, nc, 0));
-    B200_CUDA(gcm_grow(d_starts, nc, 0)); B200_CUDA(gcm_grow(d_head, nc, 0));
-    cap = nc;
-    // CUB scratch for the largest of the two primitives at this capacity
-    size_t s1 = 0, s2 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, s1, d_idx, d_idx2, d_pos, d_pos2, (int)cap, 0, 32, stream);
-    cub::DeviceSelect::Flagged(nullptr, s2, thrust::counting_iterator<int>(0), d_head, d_starts, d_flag + 1, (int)cap, stream);
-    const size_t need_tmp = std::max(s1, s2);
-    if (need_tmp > tmp_bytes) {
-      if (d_tmp) cudaFree(d_tmp);
-      d_tmp = nullptr;
-      B200_CUDA(cudaMalloc(&d_tmp, need_tmp));
-      tmp_bytes = need_tmp;
+    const long long nc = std::max<long long>(need, cap * 2);
+    DeviceBlock grown;
+    float *xyz, *xyz2;
+    uint8_t *rgb, *rgb2;
+    B200_CHECK(grown.carve(stream, [&](Carver& t) {
+      xyz = t.take<float>(3 * nc); rgb = t.take<uint8_t>(3 * nc); xyz2 = t.take<float>(3 * nc); rgb2 = t.take<uint8_t>(3 * nc);
+    }));
+    if (n > 0) {
+      B200_CUDA(cudaMemcpyAsync(xyz, d_xyz, 12 * n, cudaMemcpyDeviceToDevice, stream));
+      B200_CUDA(cudaMemcpyAsync(rgb, d_rgb, 3 * n, cudaMemcpyDeviceToDevice, stream));
     }
+    B200_CUDA(cudaStreamSynchronize(stream));
+    points = std::move(grown);
+    d_xyz = xyz; d_rgb = rgb; d_xyz2 = xyz2; d_rgb2 = rgb2;
+    cap = nc;
     return B200ORB_OK;
   }
 };
@@ -197,23 +173,19 @@ int gcm_create(float leaf, int device, gcm_t** out) {
   *out = nullptr;
   B200_CHECK(check_device(device));
   DeviceGuard g(device);
-  gcm* h = new (std::nothrow) gcm();
+  std::unique_ptr<gcm> h(new (std::nothrow) gcm());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
   h->device = device;
   h->sms = sm_count(device);
   h->leaf = leaf;
-  cudaError_t e;
-  if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess ||
-      (e = cudaMalloc(&h->d_mm, 24)) != cudaSuccess || (e = cudaMalloc(&h->d_flag, 8)) != cudaSuccess ||
-      (e = cudaMalloc(&h->d_T, 96)) != cudaSuccess) {
-    set_error("gcm_create: %s", cudaGetErrorString(e));
-    delete h;
-    return B200ORB_ECUDA;
-  }
-  *out = h;
+  B200_CHECK(h->stream.create());
+  B200_CHECK(h->words.carve(h->stream, [&](Carver& t) {
+    h->d_mm = t.take<unsigned>(6); h->d_flag = t.take<int>(2); h->d_T = t.take<double>(12);
+  }));
+  *out = h.release();
   return B200ORB_OK;
 }
-void gcm_destroy(gcm_t* h) { delete h; }
+void gcm_destroy(gcm_t* h) { destroy_handle(h); }
 
 int gcm_add_keyframe_device(gcm_t* h, const float* d_depth, const uint8_t* d_bgr, int rows, int cols, const float Tcw[16],
                             float fx, float fy, float cx, float cy) {
@@ -242,17 +214,12 @@ int gcm_add_keyframe(gcm_t* h, const float* depth, const uint8_t* bgr, int rows,
   if (!h || !depth || !bgr || !Tcw || rows <= 0 || cols <= 0) { set_error("bad argument"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
   const size_t npix = (size_t)rows * cols;
-  if (npix > h->in_px) {
-    B200_CUDA(cudaStreamSynchronize(h->stream));
-    if (h->d_in_depth) cudaFree(h->d_in_depth);
-    if (h->d_in_rgb) cudaFree(h->d_in_rgb);
-    h->d_in_depth = nullptr; h->d_in_rgb = nullptr; h->in_px = 0;
-    B200_CUDA(cudaMalloc(&h->d_in_depth, npix * 4)); B200_CUDA(cudaMalloc(&h->d_in_rgb, npix * 3));
-    h->in_px = npix;
-  }
-  B200_CUDA(cudaMemcpyAsync(h->d_in_depth, depth, npix * 4, cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(h->d_in_rgb, bgr, npix * 3, cudaMemcpyHostToDevice, h->stream));
-  B200_CHECK(gcm_add_keyframe_device(h, h->d_in_depth, h->d_in_rgb, rows, cols, Tcw, fx, fy, cx, cy));
+  float* d_depth;
+  uint8_t* d_bgr;
+  B200_CHECK(h->stage.reserve(h->stream, [&](Carver& t) { d_depth = t.take<float>(npix); d_bgr = t.take<uint8_t>(3 * npix); }));
+  B200_CUDA(cudaMemcpyAsync(d_depth, depth, npix * 4, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d_bgr, bgr, npix * 3, cudaMemcpyHostToDevice, h->stream));
+  B200_CHECK(gcm_add_keyframe_device(h, d_depth, d_bgr, rows, cols, Tcw, fx, fy, cx, cy));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
 }
@@ -266,17 +233,30 @@ int gcm_refilter(gcm_t* h) {
   cudaStream_t st = h->stream;
   const long long n = h->n;
   const float inv = 1.0f / h->leaf;
+  // CUB scratch for the larger of the two primitives at n points
+  size_t s1 = 0, s2 = 0;
+  int *d_idx, *d_idx2, *d_pos, *d_pos2, *d_starts;
+  uint8_t* d_head;
+  void* d_tmp;
+  cub::DeviceRadixSort::SortPairs(nullptr, s1, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)n, 0, 32, st);
+  cub::DeviceSelect::Flagged(nullptr, s2, thrust::counting_iterator<int>(0), (uint8_t*)nullptr, (int*)nullptr, (int*)nullptr,
+                             (int)n, st);
+  const size_t tmp_bytes = std::max(s1, s2);
+  B200_CHECK(h->sort.reserve(st, [&](Carver& t) {
+    d_idx = t.take<int>(n); d_idx2 = t.take<int>(n); d_pos = t.take<int>(n); d_pos2 = t.take<int>(n);
+    d_starts = t.take<int>(n); d_head = t.take<uint8_t>(n); d_tmp = t.take<char>(tmp_bytes);
+  }));
   static const unsigned mm0[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
   B200_CUDA(cudaMemcpyAsync(h->d_mm, mm0, 24, cudaMemcpyHostToDevice, st));
   B200_CUDA(cudaMemsetAsync(h->d_flag, 0, 8, st));
   k_gcm_minmax<<<2 * h->sms, 256, 0, st>>>(h->d_xyz, n, h->d_mm);
-  k_gcm_index<<<4 * h->sms, 256, 0, st>>>(h->d_xyz, n, inv, h->d_mm, h->d_idx, h->d_pos, h->d_flag);
-  size_t tb = h->tmp_bytes;
-  B200_CUDA(cub::DeviceRadixSort::SortPairs(h->d_tmp, tb, h->d_idx, h->d_idx2, h->d_pos, h->d_pos2, (int)n, 0, 32, st));
-  k_gcm_heads<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(h->d_idx2, n, h->d_head);
-  tb = h->tmp_bytes;
-  B200_CUDA(cub::DeviceSelect::Flagged(h->d_tmp, tb, thrust::counting_iterator<int>(0), h->d_head, h->d_starts, h->d_flag + 1,
-                                       (int)n, st));
+  k_gcm_index<<<4 * h->sms, 256, 0, st>>>(h->d_xyz, n, inv, h->d_mm, d_idx, d_pos, h->d_flag);
+  size_t tb = tmp_bytes;
+  B200_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_idx, d_idx2, d_pos, d_pos2, (int)n, 0, 32, st));
+  k_gcm_heads<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_idx2, n, d_head);
+  tb = tmp_bytes;
+  B200_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<int>(0), d_head, d_starts, h->d_flag + 1, (int)n,
+                                       st));
   int flag[2] = {0, 0};
   B200_CUDA(cudaMemcpyAsync(flag, h->d_flag, 8, cudaMemcpyDeviceToHost, st));
   B200_CUDA(cudaStreamSynchronize(st));
@@ -287,7 +267,7 @@ int gcm_refilter(gcm_t* h) {
   }
   const int cells = flag[1];
   if (cells > 0) {
-    k_gcm_centroids<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(h->d_idx2, h->d_pos2, h->d_starts, h->d_flag + 1, n, h->d_xyz,
+    k_gcm_centroids<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(d_idx2, d_pos2, d_starts, h->d_flag + 1, n, h->d_xyz,
                                                                     h->d_rgb, h->d_xyz2, h->d_rgb2);
     ++h->launches;
   }

@@ -15,6 +15,7 @@
 //                of a batch only ORs bits (order-free, one launch); one more launch replays each touched voxel's bits in
 //                keyframe order, which reproduces the sequential clamped updates exactly.
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -579,11 +580,11 @@ struct ocm {
   OcmParams prm{};
   int device = 0;
   int sms = 1;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   long long launches = 0;
   float hit_log, miss_log, cmin, cmax;
   // the map and the handle's device words: one allocation (take_block)
-  void* d_block = nullptr;
+  DeviceBlock block;
   MapView map{};
   long long map_cap = 0;
   static constexpr int MAX_SLOTS = 32;
@@ -595,41 +596,30 @@ struct ocm {
   // per-keyframe scratch: one slot per keyframe of a batch, one allocation each (grown on demand, self-cleaning
   // between uses)
   int rows = 0, cols = 0;
-  std::vector<KfScratch> slots;
-  KfJob* d_jobs = nullptr;            // device copy of the running batch, JOB_RING batches deep
-  KfJob* h_jobs = nullptr;            // page-locked staging of the same
+  struct Slot {
+    DeviceBlock block;
+    KfScratch k;
+  };
+  std::vector<Slot> slots;
   static constexpr int JOB_RING = 8;
-  cudaEvent_t job_ev[JOB_RING] = {};
+  DeviceBlock jobs_d;                 // device copy of the running batch, JOB_RING batches deep
+  HostBlock jobs_h;                   // page-locked staging of the same
+  KfJob *d_jobs = nullptr, *h_jobs = nullptr;
+  Event job_ev[JOB_RING];
   int job_head = 0;
   int last_slot = 0;
-  // staging of the host-buffer inserts: one allocation for stage_pix pixels, grown on demand
-  void* d_stage = nullptr;
-  size_t stage_pix = 0;
+  // staging of the host-buffer inserts
+  DeviceBlock stage;
   uint16_t* st_d16 = nullptr;         // ocm_insert_keyframes_u16_labeled only
   float* st_depth = nullptr;
   uint8_t *st_rgb = nullptr, *st_label = nullptr;
-  // ocm_merge_nccl staging (grown on demand)
-  void *mg_send = nullptr, *mg_recv = nullptr;
-  int* mg_slots = nullptr;
-  int* mg_counts = nullptr;        // device, one int per rank
-  int* mg_counts_h = nullptr;      // page-locked mirror
-  long long mg_send_cap = 0, mg_recv_cap = 0;
-  int mg_world_cap = 0;
+  DeviceBlock exp;                    // ocm_export_leaves' outputs
+  // ocm_merge_nccl: the count of every rank (device and page-locked), then the send, receive and slot buffers
+  DeviceBlock mg_counts;
+  HostBlock mg_counts_h;
+  DeviceBlock mg;
+  Event mg_ev[2];                     // orders the merge after the caller's stream, and the caller's stream after it
 
-  ~ocm() {
-    DeviceGuard g(device);
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    free_scratch();
-    F(d_block); F(d_stage); F(d_jobs); F(mg_send); F(mg_recv); F(mg_slots); F(mg_counts);
-    if (mg_counts_h) cudaFreeHost(mg_counts_h);
-    if (h_jobs) cudaFreeHost(h_jobs);
-    for (cudaEvent_t e : job_ev) if (e) cudaEventDestroy(e);
-    if (stream) cudaStreamDestroy(stream);
-  }
-  void free_scratch() {
-    for (KfScratch& k : slots) cudaFree(k.leaf.rec);   // the start of the slot's allocation (ensure_scratch)
-    slots.clear();
-  }
   // Every array 256-byte aligned by the Carver (k_ocm_apply reads bm in 16-byte words).
   void take_block(Carver& c) {
     const long long C = map_cap;
@@ -665,21 +655,18 @@ static long long pow2_at_least(long long v) {
 int ocm::ensure_scratch(int r, int c, int nslots) {
   if (r != rows || c != cols) {
     B200_CUDA(cudaStreamSynchronize(stream));
-    free_scratch();
+    slots.clear();
     rows = r; cols = c;
   }
   nslots = std::min(std::max(nslots, 1), (int)MAX_SLOTS);
-  if (!d_jobs) {
-    B200_CUDA(cudaMalloc(&d_jobs, sizeof(KfJob) * MAX_SLOTS * JOB_RING));
-    B200_CUDA(cudaHostAlloc(&h_jobs, sizeof(KfJob) * MAX_SLOTS * JOB_RING, cudaHostAllocDefault));
-    for (cudaEvent_t& e : job_ev) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  }
+  B200_CHECK(jobs_d.reserve(stream, [&](Carver& t) { d_jobs = t.take<KfJob>(MAX_SLOTS * JOB_RING); }));
+  B200_CHECK(jobs_h.reserve(stream, [&](Carver& t) { h_jobs = t.take<KfJob>(MAX_SLOTS * JOB_RING); }));
   const long long npix = (long long)r * c;
   const long long leaf_cap = pow2_at_least(2 * npix);
   while ((int)slots.size() < nslots) {
-    KfScratch k{};
-    void* block;
-    B200_CHECK(alloc_carved(&block, [&](Carver& t) {   // the leaf table first: free_scratch frees it
+    Slot s;
+    KfScratch& k = s.k;
+    B200_CHECK(s.block.carve(stream, [&](Carver& t) {
       k.leaf.rec = t.take<LeafRec>(leaf_cap);
       k.pix_slot = t.take<int>(npix); k.pix_rank = t.take<int>(npix); k.bucket = t.take<int>(npix);
       k.voxlist = t.take<int>(npix);
@@ -689,23 +676,16 @@ int ocm::ensure_scratch(int r, int c, int nslots) {
     k.counters = d_counters + 4 * slots.size();
     fill(k.leaf.rec, empty_leaf(), leaf_cap);
     B200_CUDA(cudaGetLastError());
-    slots.push_back(k);
+    slots.push_back(std::move(s));
   }
   return B200ORB_OK;
 }
 
 int ocm::ensure_staging(size_t npix) {
-  if (npix <= stage_pix) return B200ORB_OK;
-  B200_CUDA(cudaStreamSynchronize(stream));   // earlier inserts may still read the old staging
-  if (d_stage) cudaFree(d_stage);
-  d_stage = nullptr;
-  stage_pix = 0;
-  B200_CHECK(alloc_carved(&d_stage, [&](Carver& t) {
+  return stage.reserve(stream, [&](Carver& t) {
     st_d16 = t.take<uint16_t>(npix); st_depth = t.take<float>(npix); st_rgb = t.take<uint8_t>(3 * npix);
     st_label = t.take<uint8_t>(npix);
-  }));
-  stage_pix = npix;
-  return B200ORB_OK;
+  });
 }
 
 int ocm::check_err() {
@@ -752,7 +732,7 @@ int ocm::insert_batch(int n, const float* const* dd, const uint8_t* const* drgb,
       k.origin[0] = Tcw[3]; k.origin[1] = Tcw[7]; k.origin[2] = Tcw[11];
       k.rows = r; k.cols = c;
       J.depth = dd[b0 + j]; J.rgb = drgb[b0 + j]; J.label = dlabel ? dlabel[b0 + j] : nullptr;
-      J.s = slots[j];
+      J.s = slots[j].k;
     }
     B200_CUDA(cudaMemcpyAsync(dj, hj, sizeof(KfJob) * B, cudaMemcpyHostToDevice, stream));
     B200_CUDA(cudaEventRecord(job_ev[ring], stream));
@@ -797,7 +777,7 @@ int ocm_create(const OcmParams* p, int device, ocm_t** out) {
   }
   B200_CHECK(check_device(device));
   DeviceGuard g(device);
-  ocm* h = new (std::nothrow) ocm();
+  std::unique_ptr<ocm> h(new (std::nothrow) ocm());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
   h->prm = *p;
   h->device = device;
@@ -806,28 +786,25 @@ int ocm_create(const OcmParams* p, int device, ocm_t** out) {
   h->hit_log = logodds(p->prob_hit); h->miss_log = logodds(p->prob_miss);
   h->cmin = logodds(p->clamp_min); h->cmax = logodds(p->clamp_max);
   h->map_cap = pow2_at_least(p->map_capacity > 0 ? std::max<long long>(p->map_capacity, 2) : (1ll << 23));
-  auto fail = [&](cudaError_t e) { set_error("ocm_create: %s", cudaGetErrorString(e)); delete h; return B200ORB_ECUDA; };
-  cudaError_t e;
-  {
-    // highest stream priority: the mapper is a chain of small dependent kernels running BESIDE the tracking batch;
-    // with default priority every link waits behind thousands of queued tracking CTAs, with high priority its CTAs
-    // take the next free SM slots.
-    int lo_p = 0, hi_p = 0;
-    cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p);
-    if ((e = cudaStreamCreateWithPriority(&h->stream, cudaStreamNonBlocking, hi_p)) != cudaSuccess) return fail(e);
-  }
+  // highest stream priority: the mapper is a chain of small dependent kernels running BESIDE the tracking batch;
+  // with default priority every link waits behind thousands of queued tracking CTAs, with high priority its CTAs
+  // take the next free SM slots.
+  int lo_p = 0, hi_p = 0;
+  cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p);
+  B200_CHECK(h->stream.create(hi_p));
+  for (Event& e : h->job_ev) B200_CHECK(e.create());
+  for (Event& e : h->mg_ev) B200_CHECK(e.create());
   const long long C = h->map_cap;
   h->map.mask = C - 1;
-  size_t bytes = 0;
-  if (alloc_carved(&h->d_block, [&](Carver& t) { h->take_block(t); }, &bytes) != B200ORB_OK) { delete h; return B200ORB_ECUDA; }
-  cudaMemsetAsync(h->d_block, 0, bytes, h->stream);
+  B200_CHECK(h->block.carve(h->stream, [&](Carver& t) { h->take_block(t); }));
+  B200_CUDA(cudaMemsetAsync(h->block.p, 0, h->block.bytes, h->stream));
   h->fill(h->map.keys, EMPTY_KEY, C); h->fill(h->map.lo, -INFINITY, C); h->fill(h->map.hi, INFINITY, C);
-  cudaMemsetAsync(h->map.rgb, 0xff, 4 * C, h->stream);
-  if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return fail(e);
-  *out = h;
+  B200_CUDA(cudaMemsetAsync(h->map.rgb, 0xff, 4 * C, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  *out = h.release();
   return B200ORB_OK;
 }
-void ocm_destroy(ocm_t* h) { delete h; }
+void ocm_destroy(ocm_t* h) { destroy_handle(h); }
 
 int ocm_insert_keyframe_device(ocm_t* h, const float* d_depth, const uint8_t* d_rgb, int rows, int cols,
                                const float Tcw[16], float fx, float fy, float cx, float cy, const uint8_t* d_label) {
@@ -897,7 +874,7 @@ int ocm_last_points(ocm_t* h, float* xyz, uint8_t* rgb, int cap, int* n) {
   DeviceGuard g(h->device);
   int cnt[2] = {0, 0};
   if (h->slots.empty()) { *n = 0; return B200ORB_OK; }
-  const KfScratch& ls = h->slots[h->last_slot];
+  const KfScratch& ls = h->slots[h->last_slot].k;
   B200_CUDA(cudaMemcpyAsync(cnt, ls.counters, 8, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   *n = cnt[1];
@@ -921,26 +898,25 @@ int64_t ocm_num_leaves(ocm_t* h) {
 int ocm_export_leaves(ocm_t* h, uint16_t* keys, float* logodds, uint8_t* rgb, int64_t cap, int64_t* n) {
   if (!h || !keys || !logodds || cap < 0) { set_error("bad argument"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  unsigned short* dk = nullptr; float* dv = nullptr; unsigned char* dc = nullptr;
-  const int64_t c = cap > 0 ? cap : 1;
-  B200_CUDA(cudaMalloc(&dk, 6 * c)); B200_CUDA(cudaMalloc(&dv, 4 * c)); B200_CUDA(cudaMalloc(&dc, 3 * c));
+  unsigned short* dk;
+  float* dv;
+  unsigned char* dc;
+  B200_CHECK(h->exp.reserve(h->stream, [&](Carver& t) {
+    dk = t.take<unsigned short>(3 * cap); dv = t.take<float>(cap); dc = t.take<unsigned char>(3 * cap);
+  }));
   long long cnt = 0;
-  auto run = [&]() -> int {
-    B200_CUDA(cudaMemsetAsync(h->d_export_counter, 0, 8, h->stream));
-    k_ocm_export<<<(unsigned)((h->map_cap + 255) / 256), 256, 0, h->stream>>>(h->map, h->d_export_counter, cap, dk, dv, dc);
-    ++h->launches;
-    B200_CUDA(cudaMemcpyAsync(&cnt, h->d_export_counter, 8, cudaMemcpyDeviceToHost, h->stream));
-    B200_CUDA(cudaStreamSynchronize(h->stream));
-    if (cnt > cap) { set_error("export cap %lld < %lld entries", (long long)cap, cnt); return B200ORB_ECAP; }
-    cudaMemcpy(keys, dk, 6 * cnt, cudaMemcpyDeviceToHost);
-    cudaMemcpy(logodds, dv, 4 * cnt, cudaMemcpyDeviceToHost);
-    if (rgb) cudaMemcpy(rgb, dc, 3 * cnt, cudaMemcpyDeviceToHost);
-    return B200ORB_OK;
-  };
-  const int rc = run();
+  B200_CUDA(cudaMemsetAsync(h->d_export_counter, 0, 8, h->stream));
+  k_ocm_export<<<(unsigned)((h->map_cap + 255) / 256), 256, 0, h->stream>>>(h->map, h->d_export_counter, cap, dk, dv, dc);
+  ++h->launches;
+  B200_CUDA(cudaMemcpyAsync(&cnt, h->d_export_counter, 8, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
   if (n) *n = cnt;
-  cudaFree(dk); cudaFree(dv); cudaFree(dc);
-  return rc;
+  if (cnt > cap) { set_error("export cap %lld < %lld entries", (long long)cap, cnt); return B200ORB_ECAP; }
+  B200_CUDA(cudaMemcpyAsync(keys, dk, 6 * cnt, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(logodds, dv, 4 * cnt, cudaMemcpyDeviceToHost, h->stream));
+  if (rgb) B200_CUDA(cudaMemcpyAsync(rgb, dc, 3 * cnt, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200ORB_OK;
 }
 
 int ocm_query(ocm_t* h, const float xyz[3], float* logodds, int* found) {
@@ -1044,11 +1020,8 @@ int ocm_merge_nccl(ocm_t* h, void* comm_, void* stream_, OcmMergeStats* st) {
   DeviceGuard g(h->device);
   cudaStream_t S = h->stream;
   if (stream_ && (cudaStream_t)stream_ != S) {   // order after the caller's stream
-    cudaEvent_t ev;
-    B200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    B200_CUDA(cudaEventRecord(ev, (cudaStream_t)stream_));
-    B200_CUDA(cudaStreamWaitEvent(S, ev, 0));
-    cudaEventDestroy(ev);
+    B200_CUDA(cudaEventRecord(h->mg_ev[0], (cudaStream_t)stream_));
+    B200_CUDA(cudaStreamWaitEvent(S, h->mg_ev[0], 0));
   }
   NcclApi* N = nullptr;
   ncclComm_t comm = (ncclComm_t)comm_;
@@ -1059,40 +1032,29 @@ int ocm_merge_nccl(ocm_t* h, void* comm_, void* stream_, OcmMergeStats* st) {
     B200_NCCL(N, N->CommCount(comm, &world));
     B200_NCCL(N, N->CommUserRank(comm, &rank));
   }
-  if (world > h->mg_world_cap) {
-    if (h->mg_counts) cudaFree(h->mg_counts);
-    if (h->mg_counts_h) cudaFreeHost(h->mg_counts_h);
-    B200_CUDA(cudaMalloc(&h->mg_counts, 4 * world));
-    B200_CUDA(cudaHostAlloc(&h->mg_counts_h, 4 * world, cudaHostAllocDefault));
-    h->mg_world_cap = world;
-  }
+  int *counts, *counts_h;
+  B200_CHECK(h->mg_counts.reserve(S, [&](Carver& t) { counts = t.take<int>(world); }));
+  B200_CHECK(h->mg_counts_h.reserve(S, [&](Carver& t) { counts_h = t.take<int>(world); }));
   // 1. counts: one int per rank (the only host synchronisation of the merge)
-  if (comm) B200_NCCL(N, N->AllGather(h->map.nelist, h->mg_counts, 1, ncclInt32, comm, S));
-  else B200_CUDA(cudaMemcpyAsync(h->mg_counts, h->map.nelist, 4, cudaMemcpyDeviceToDevice, S));
-  B200_CUDA(cudaMemcpyAsync(h->mg_counts_h, h->mg_counts, 4 * world, cudaMemcpyDeviceToHost, S));
+  if (comm) B200_NCCL(N, N->AllGather(h->map.nelist, counts, 1, ncclInt32, comm, S));
+  else B200_CUDA(cudaMemcpyAsync(counts, h->map.nelist, 4, cudaMemcpyDeviceToDevice, S));
+  B200_CUDA(cudaMemcpyAsync(counts_h, counts, 4 * world, cudaMemcpyDeviceToHost, S));
   B200_CUDA(cudaStreamSynchronize(S));
   std::vector<long long> off(world + 1, 0);   // byte offsets of the shards in the receive buffer (16-byte aligned)
   long long total = 0;
   for (int r = 0; r < world; ++r) {
-    off[r + 1] = (long long)align_up_sz((size_t)(off[r] + 24ll * h->mg_counts_h[r]), 16);
-    total += h->mg_counts_h[r];
+    off[r + 1] = (long long)align_up_sz((size_t)(off[r] + 24ll * counts_h[r]), 16);
+    total += counts_h[r];
   }
-  const long long n_own = h->mg_counts_h[rank];
-  if (24 * n_own > h->mg_send_cap) {
-    if (h->mg_send) cudaFree(h->mg_send);
-    h->mg_send_cap = std::max(24 * n_own * 2, 1ll << 20);
-    B200_CUDA(cudaMalloc(&h->mg_send, h->mg_send_cap));
-  }
-  if (off[world] > h->mg_recv_cap) {
-    if (h->mg_recv) cudaFree(h->mg_recv);
-    if (h->mg_slots) cudaFree(h->mg_slots);
-    h->mg_recv_cap = std::max(off[world] * 2, 1ll << 20);
-    B200_CUDA(cudaMalloc(&h->mg_recv, h->mg_recv_cap));
-    B200_CUDA(cudaMalloc(&h->mg_slots, h->mg_recv_cap / 24 * 4 + 64));
-  }
+  const long long n_own = counts_h[rank];
+  char *send, *recv;
+  int* slots;
+  B200_CHECK(h->mg.reserve(S, [&](Carver& t) {
+    send = t.take<char>(24 * n_own); recv = t.take<char>(off[world]); slots = t.take<int>(total);
+  }));
   // 2. pack own summaries, roll own voxels back to the last merge
   if (n_own > 0) {
-    k_merge_pack<<<(unsigned)((n_own + 255) / 256), 256, 0, S>>>(h->map, (int)n_own, merge_shard_at(h->mg_send, n_own));
+    k_merge_pack<<<(unsigned)((n_own + 255) / 256), 256, 0, S>>>(h->map, (int)n_own, merge_shard_at(send, n_own));
     ++h->launches;
   }
   B200_CUDA(cudaMemsetAsync(h->map.nelist, 0, 4, S));
@@ -1100,35 +1062,32 @@ int ocm_merge_nccl(ocm_t* h, void* comm_, void* stream_, OcmMergeStats* st) {
   if (comm && world > 1) {
     B200_NCCL(N, N->GroupStart());
     for (int r = 0; r < world; ++r) {
-      const size_t bytes = 24 * (size_t)h->mg_counts_h[r];
+      const size_t bytes = 24 * (size_t)counts_h[r];
       if (bytes == 0) continue;
-      B200_NCCL(N, N->Broadcast(r == rank ? h->mg_send : nullptr, (char*)h->mg_recv + off[r], bytes, ncclUint8, r, comm, S));
+      B200_NCCL(N, N->Broadcast(r == rank ? send : nullptr, recv + off[r], bytes, ncclUint8, r, comm, S));
     }
     B200_NCCL(N, N->GroupEnd());
   } else if (n_own > 0) {
-    B200_CUDA(cudaMemcpyAsync(h->mg_recv, h->mg_send, 24 * n_own, cudaMemcpyDeviceToDevice, S));
+    B200_CUDA(cudaMemcpyAsync(recv, send, 24 * n_own, cudaMemcpyDeviceToDevice, S));
   }
   // 4. replay all shards in rank (= keyframe) order, then make the result the base of the next epoch
   long long done = 0;
   for (int r = 0; r < world; ++r) {
-    const long long n = h->mg_counts_h[r];
+    const long long n = counts_h[r];
     if (n == 0) continue;
-    k_merge_apply<<<(unsigned)((n + 255) / 256), 256, 0, S>>>(h->map, n, merge_shard_at((char*)h->mg_recv + off[r], n),
-                                                             h->mg_slots + done, h->d_err);
+    k_merge_apply<<<(unsigned)((n + 255) / 256), 256, 0, S>>>(h->map, n, merge_shard_at(recv + off[r], n),
+                                                             slots + done, h->d_err);
     ++h->launches;
     done += n;
   }
   if (total > 0) {
-    k_merge_commit<<<(unsigned)((total + 255) / 256), 256, 0, S>>>(h->map, total, h->mg_slots);
+    k_merge_commit<<<(unsigned)((total + 255) / 256), 256, 0, S>>>(h->map, total, slots);
     ++h->launches;
   }
   B200_CUDA(cudaGetLastError());
   if (stream_ && (cudaStream_t)stream_ != S) {
-    cudaEvent_t ev;
-    B200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    B200_CUDA(cudaEventRecord(ev, S));
-    B200_CUDA(cudaStreamWaitEvent((cudaStream_t)stream_, ev, 0));
-    cudaEventDestroy(ev);
+    B200_CUDA(cudaEventRecord(h->mg_ev[1], S));
+    B200_CUDA(cudaStreamWaitEvent((cudaStream_t)stream_, h->mg_ev[1], 0));
   }
   if (st) { st->world = world; st->rank = rank; st->records_sent = n_own; st->records_total = total; st->bytes_sent = 24 * n_own; st->bytes_received = 24 * (total - n_own); }
   return B200ORB_OK;
@@ -1155,7 +1114,7 @@ int ocm_sync(ocm_t* h) {
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return h->check_err();
 }
-void* ocm_stream(ocm_t* h) { return h ? (void*)h->stream : nullptr; }
+void* ocm_stream(ocm_t* h) { return h ? (void*)(cudaStream_t)h->stream : nullptr; }
 long long ocm_launch_count(const ocm_t* h) { return h ? h->launches : 0; }
 
 }  // extern "C"

@@ -2,6 +2,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -10,35 +11,7 @@
 
 using namespace b200;
 
-orbm::~orbm() {
-  DeviceGuard g(device);
-  if (d_arena) cudaFree(d_arena);
-  if (stream) cudaStreamDestroy(stream);
-}
-
-int orbm::reserve(size_t bytes) {
-  if (bytes <= arena_bytes) return B200ORB_OK;
-  if (d_arena) { cudaStreamSynchronize(stream); cudaFree(d_arena); d_arena = nullptr; arena_bytes = 0; }
-  const size_t want = align_up_sz(bytes + bytes / 2, 1 << 20);
-  B200_CUDA(cudaMalloc(&d_arena, want));
-  arena_bytes = want;
-  return B200ORB_OK;
-}
-
 namespace {
-// Carves the arena with `take_all`, the entry's complete buffer list: once against a null base to measure, then for
-// real once the arena has grown to that size.
-template <class F>
-int carve_arena(orbm* h, F&& take_all) {
-  Carver probe;
-  take_all(probe);
-  B200_CHECK(h->reserve(probe.off));
-  Carver c(h->d_arena, h->arena_bytes);
-  take_all(c);
-  if (c.overrun) { set_error("matcher arena overrun"); return B200ORB_EINVAL; }
-  return B200ORB_OK;
-}
-
 int resolve_smem(int cmax, size_t* smem, const void* func) {
   *smem = (size_t)cmax * 5 + 16;
   if (*smem > 200 * 1024) { set_error("too many keypoints per frame for the matcher's shared memory"); return B200ORB_EINVAL; }
@@ -125,15 +98,14 @@ int orbm_create(int device, orbm_t** out) {
   *out = nullptr;
   B200_CHECK(check_device(device));
   DeviceGuard g(device);
-  orbm* h = new (std::nothrow) orbm();
+  std::unique_ptr<orbm> h(new (std::nothrow) orbm());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
   h->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { set_error("cudaStreamCreate: %s", cudaGetErrorString(e)); delete h; return B200ORB_ECUDA; }
-  *out = h;
+  B200_CHECK(h->stream.create());
+  *out = h.release();
   return B200ORB_OK;
 }
-void orbm_destroy(orbm_t* h) { delete h; }
+void orbm_destroy(orbm_t* h) { destroy_handle(h); }
 long long orbm_launch_count(const orbm_t* h) { return h ? h->launches : 0; }
 
 static int fill_cam(const OrbmFrame* f, float th, int mono, float nnratio, int check_ori, MatchCam* cam) {
@@ -206,7 +178,7 @@ int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLa
   LastView lv{};
   int *d_out, *d_nm, *d_acc;
   uint8_t* d_scratch;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     take_cur(c, cur, &cv);
     lv.xw = c.take<float>(nl * 3); lv.valid = c.take<uint8_t>(nl); lv.oct = c.take<int>(nl); lv.ang = c.take<float>(nl);
     lv.desc = c.take<uint8_t>(nl * 32); lv.obs = last->mp_obs ? c.take<int>(nl) : nullptr;
@@ -259,7 +231,7 @@ int orbm_search_by_projection_points(orbm_t* h, const OrbmFrame* f, const OrbmTr
   QueriesView qv{};
   ListView lsv;
   int *d_out, *d_nm;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     take_cur(c, f, &cv);
     qv.valid = c.take<uint8_t>(np); qv.u = c.take<float>(np); qv.v = c.take<float>(np); qv.radius = c.take<float>(np);
     qv.uright = c.take<float>(np); qv.min_level = c.take<int>(np); qv.max_level = c.take<int>(np);
@@ -313,7 +285,7 @@ int orbm_search_projected(orbm_t* h, const OrbmFrame* cur, const OrbmQueries* q,
   QueriesView qv{};
   ListView lsv;
   int *d_acc, *d_out, *d_nm;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     take_cur(c, cur, &cv);
     qv.valid = c.take<uint8_t>(nq); qv.u = c.take<float>(nq); qv.v = c.take<float>(nq); qv.radius = c.take<float>(nq);
     qv.min_level = c.take<int>(nq); qv.max_level = c.take<int>(nq); qv.uright = q->uright ? c.take<float>(nq) : nullptr;
@@ -364,7 +336,7 @@ int orbm_search_best(orbm_t* h, const OrbmFrame* kf, const OrbmQueries* q, int g
   QueriesView qv{};
   float* d_is2;
   int *d_bi, *d_bd;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     take_cur(c, &kf2, &cv);
     qv.valid = c.take<uint8_t>(nq); qv.u = c.take<float>(nq); qv.v = c.take<float>(nq); qv.radius = c.take<float>(nq);
     qv.min_level = c.take<int>(nq); qv.max_level = c.take<int>(nq); qv.uright = q->uright ? c.take<float>(nq) : nullptr;
@@ -406,7 +378,7 @@ int orbm_search_for_initialization(orbm_t* h, const OrbmFrame* f1, const OrbmFra
   CurView cv;
   InitView iv{};
   int *d_out, *d_nm;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     take_cur(c, &f2c, &cv);
     iv.oct1 = c.take<int>(n1); iv.ang1 = c.take<float>(n1); iv.desc1 = c.take<uint8_t>(n1 * 32);
     iv.prev_xy = c.take<float>(n1 * 2); iv.matched_dist = c.take<int>(n2); iv.match21 = c.take<int>(n2);
@@ -468,7 +440,7 @@ int orbm_search_for_triangulation(orbm_t* h, const OrbmTriKF* k1, const OrbmTriK
   TriView t;
   memset(&t, 0, sizeof(t));
   int *d_out, *d_nm;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     t.q_idx1 = c.take<int>(nq); t.f_beg = c.take<int>(nq); t.f_end = c.take<int>(nq); t.f_idx = c.take<unsigned>(nfi);
     t.desc1 = c.take<uint8_t>(n1 * 32); t.desc2 = c.take<uint8_t>(n2 * 32);
     t.x1 = c.take<float>(n1); t.y1 = c.take<float>(n1); t.ang1 = c.take<float>(n1); t.ur1 = c.take<float>(n1);
@@ -533,7 +505,7 @@ int orbm_is_in_frustum(orbm_t* h, const OrbmFrame* f, const OrbmFrustumPoints* p
   float *d_xw, *d_nrm, *d_mn, *d_mx, *d_px, *d_py, *d_pxr, *d_vc;
   uint8_t* d_in;
   int* d_lvl;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     d_xw = c.take<float>(n * 3); d_nrm = c.take<float>(n * 3); d_mn = c.take<float>(n); d_mx = c.take<float>(n);
     d_in = c.take<uint8_t>(n); d_px = c.take<float>(n); d_py = c.take<float>(n); d_pxr = c.take<float>(n);
     d_lvl = c.take<int>(n); d_vc = c.take<float>(n);
@@ -573,7 +545,7 @@ int orbm_undistort_keypoints(orbm_t* h, const float* xy_in, int n, const float K
   }
   DeviceGuard g(h->device);
   float *d_in, *d_out;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     d_in = c.take<float>((size_t)n * 2); d_out = c.take<float>((size_t)n * 2);
   }));
   UP(d_in, xy_in, (size_t)n * 2, float);
@@ -626,7 +598,7 @@ static int bow_impl(orbm_t* h, const OrbmBow* kf, const OrbmBow* f, float nnrati
   unsigned *d_fidx, *d_list;
   uint8_t *d_kd, *d_fd, *d_fvalid;
   float *d_ka, *d_fa;
-  B200_CHECK(carve_arena(h, [&](Carver& c) {
+  B200_CHECK(h->arena.reserve(h->stream, [&](Carver& c) {
     d_qkf = c.take<int>(nq); d_qb = c.take<int>(nq); d_qe = c.take<int>(nq); d_fidx = c.take<unsigned>(nfi);
     d_kd = c.take<uint8_t>((size_t)kf->n * 32); d_fd = c.take<uint8_t>((size_t)f->n * 32);
     d_ka = c.take<float>(kf->n); d_fa = c.take<float>(f->n);

@@ -4,12 +4,9 @@
 
 struct orbm {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  b200::Stream stream;
   long long launches = 0;
-  void* d_arena = nullptr;
-  size_t arena_bytes = 0;
-  ~orbm();
-  int reserve(size_t bytes);
+  b200::DeviceBlock arena;   // each entry carves its complete buffer list out of it
 };
 
 // Shared with the stream pipeline (orbs.cu): the LAST search of `npairs` (cur, last) pairs.  Frame pairs that fit in

@@ -1,6 +1,7 @@
 // orbs.cu -- batched stream pipeline (north_star's "batched many-frame mode"): per frame t of a batch the device
 // does what Tracking::GrabImageRGBD -> Frame::Frame(RGB-D) -> TrackWithMotionModel's SearchByProjection do on the
 // CPU (src/Tracking.cc:331-375,1324-1352; src/Frame.cc:176-240), with no host round trip between the stages.
+#include <memory>
 #include <new>
 
 #include "orbm_host.h"
@@ -115,50 +116,40 @@ constexpr int MAX_CHUNKS = 7;
 struct orbs {
   OrbsParams prm{};
   int device = 0;
-  orbx* ex = nullptr;
+  std::unique_ptr<orbx> ex;
   long long launches = 0;
   int rows = 0, cols = 0, maxF = 0, cap = 0, lastF = 0;
   // Geometry block, carved for (rows, cols, maxF, cap): the glue's SoA, the match results and the scratch of the
   // non-fused LAST search.
-  void* d_geom = nullptr;
+  DeviceBlock geom;
   float *d_x = nullptr, *d_y = nullptr, *d_ang = nullptr, *d_ur = nullptr, *d_dep = nullptr, *d_xw = nullptr;
   int* d_oct = nullptr;
   uint8_t* d_valid = nullptr;
   int *d_c2l = nullptr, *d_nm = nullptr, *d_acc = nullptr;
   void* d_match_scratch = nullptr;
   // Host-input block, carved by the first host-buffer call: the uploaded inputs and the depth under the keypoints.
-  void* d_in = nullptr;
-  int in_depth_bytes = 0;   // depth staging per pixel it holds: 4 for f32 input, 2 for pageable CV_16U, 0 for page-locked
+  DeviceBlock in;
+  int in_depth_bytes = -1;  // depth staging per pixel it holds: 4 for f32 input, 2 for pageable CV_16U, 0 for page-locked,
+                            // -1 while it holds no inputs of the current geometry
   uint8_t* d_gray = nullptr;
   float* d_T = nullptr;
   uint16_t* d_kpd16 = nullptr;    // [maxF][cap] CV_16U depth under the keypoints
   void* d_depth = nullptr;        // [maxF][rows][cols] uploaded depth, f32 or CV_16U
   const uint16_t* gather_src = nullptr;   // the CV_16U batch k_depth_prefetch reads during a call
   int chunk_frames = 128;   // frames per upload chunk of the host-buffer entries
-  cudaStream_t copy_stream = nullptr;
-  cudaStream_t gather_stream = nullptr;   // k_depth_prefetch, beside the extractor's stream
-  cudaEvent_t chunk_ev[MAX_CHUNKS] = {};
-  cudaEvent_t inputs_free_ev = nullptr;    // the previous call's kernels are done with the host-input block
-  cudaEvent_t sel_ev = nullptr, gather_ev = nullptr;
-  cudaEvent_t compute_done_ev = nullptr;   // recorded after the last kernel of a host-buffer batch (before its downloads)
+  Stream copy_stream;
+  Stream gather_stream;     // k_depth_prefetch, beside the extractor's stream
+  Event chunk_ev[MAX_CHUNKS];
+  Event inputs_free_ev;     // the previous call's kernels are done with the host-input block
+  Event sel_ev, gather_ev;
+  Event compute_done_ev;    // recorded after the last kernel of a host-buffer batch (before its downloads)
   orbs* chain_prev = nullptr;              // orbs_chain_after: the next batch's kernels wait for that handle's kernels
   bool have = false;
-  ~orbs() {
-    DeviceGuard g(device);
-    cudaFree(d_geom);
-    cudaFree(d_in);
-    if (copy_stream) cudaStreamDestroy(copy_stream);
-    if (gather_stream) cudaStreamDestroy(gather_stream);
-    for (cudaEvent_t e : chunk_ev) if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : {inputs_free_ev, sel_ev, gather_ev, compute_done_ev}) if (e) cudaEventDestroy(e);
-    delete ex;
-  }
   int create_streams() {
-    B200_CUDA(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
-    B200_CUDA(cudaStreamCreateWithFlags(&gather_stream, cudaStreamNonBlocking));
-    for (cudaEvent_t& e : chunk_ev) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (cudaEvent_t* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev})
-      B200_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    B200_CHECK(copy_stream.create());
+    B200_CHECK(gather_stream.create());
+    for (Event& e : chunk_ev) B200_CHECK(e.create());
+    for (Event* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev}) B200_CHECK(e->create());
     return B200ORB_OK;
   }
   // depth_bytes: depth staging per pixel a host-buffer call needs; -1 for the device entry, which needs no host-input
@@ -167,14 +158,11 @@ struct orbs {
   int ensure(int r, int c, int F, int depth_bytes) {
     B200_CHECK(ex->ensure_geometry(r, c, F));
     if (!(r == rows && c == cols && F <= maxF && ex->cap == cap)) {
-      B200_CUDA(cudaStreamSynchronize(ex->stream));
-      cudaFree(d_geom);
-      cudaFree(d_in);
-      d_geom = d_in = nullptr;
       rows = 0;   // no geometry until its block exists
+      in_depth_bytes = -1;   // the host-input block is sized for the old geometry
       const int nF = std::max(F, ex->maxF), ncap = ex->cap;
       const size_t n = (size_t)nF * ncap;
-      B200_CHECK(alloc_carved(&d_geom, [&](Carver& t) {
+      B200_CHECK(geom.carve(ex->stream, [&](Carver& t) {
         d_x = t.take<float>(n); d_y = t.take<float>(n); d_ang = t.take<float>(n); d_ur = t.take<float>(n);
         d_dep = t.take<float>(n); d_xw = t.take<float>(3 * n); d_oct = t.take<int>(n); d_valid = t.take<uint8_t>(n);
         d_c2l = t.take<int>(n); d_nm = t.take<int>(nF); d_acc = t.take<int>(n);
@@ -182,14 +170,10 @@ struct orbs {
       }));
       rows = r; cols = c; maxF = nF; cap = ncap;
     }
-    if (depth_bytes >= 0 && (!d_in || depth_bytes > in_depth_bytes)) {
-      if (d_in) {
-        B200_CUDA(cudaStreamSynchronize(ex->stream));
-        cudaFree(d_in);
-        d_in = nullptr;
-      }
+    if (depth_bytes > in_depth_bytes) {
+      in_depth_bytes = -1;
       const size_t px = (size_t)maxF * rows * cols;
-      B200_CHECK(alloc_carved(&d_in, [&](Carver& t) {
+      B200_CHECK(in.carve(ex->stream, [&](Carver& t) {
         d_gray = t.take<uint8_t>(px); d_T = t.take<float>((size_t)maxF * 16);
         d_kpd16 = t.take<uint16_t>((size_t)maxF * cap); d_depth = t.take<uint8_t>(px * depth_bytes);
       }));
@@ -243,18 +227,17 @@ int orbs_create(const OrbsParams* p, int device, orbs_t** out) {
   *out = nullptr;
   orbx_t* ex = nullptr;
   B200_CHECK(orbx_create(&p->orb, device, &ex));
-  orbs* h = new (std::nothrow) orbs();
-  if (!h) { orbx_destroy(ex); set_error("out of host memory"); return B200ORB_EINVAL; }
+  DeviceGuard g(device);
+  std::unique_ptr<orbs> h(new (std::nothrow) orbs());
+  if (!h) { delete ex; set_error("out of host memory"); return B200ORB_EINVAL; }
   h->prm = *p;
   h->device = device;
-  h->ex = ex;
-  DeviceGuard g(device);
-  const int rc = h->create_streams();
-  if (rc != B200ORB_OK) { delete h; return rc; }
-  *out = h;
+  h->ex.reset(ex);
+  B200_CHECK(h->create_streams());
+  *out = h.release();
   return B200ORB_OK;
 }
-void orbs_destroy(orbs_t* h) { delete h; }
+void orbs_destroy(orbs_t* h) { destroy_handle(h); }
 
 int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, int nframes,
                             int rows, int cols) {
@@ -296,7 +279,7 @@ int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, floa
 // under them on the side stream (the stream of the extractor goes on with blur and descriptors meanwhile)
 static int orbs_after_select(void* ctx, int f0, int F) {
   orbs* h = static_cast<orbs*>(ctx);
-  orbx* ex = h->ex;
+  orbx* ex = h->ex.get();
   B200_CUDA(cudaEventRecord(h->sel_ev, ex->stream));
   B200_CUDA(cudaStreamWaitEvent(h->gather_stream, h->sel_ev, 0));
   const long long items = (long long)F * h->cap;
@@ -428,8 +411,8 @@ int orbs_sync(orbs_t* h) {
   B200_CUDA(cudaStreamSynchronize(h->ex->stream));
   return B200ORB_OK;
 }
-void* orbs_stream(orbs_t* h) { return h ? (void*)h->ex->stream : nullptr; }
+void* orbs_stream(orbs_t* h) { return h ? (void*)(cudaStream_t)h->ex->stream : nullptr; }
 long long orbs_launch_count(const orbs_t* h) { return h ? h->launches + h->ex->launches : 0; }
-orbx_t* orbs_extractor(orbs_t* h) { return h ? h->ex : nullptr; }
+orbx_t* orbs_extractor(orbs_t* h) { return h ? h->ex.get() : nullptr; }
 
 }  // extern "C"

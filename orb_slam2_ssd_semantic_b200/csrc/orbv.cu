@@ -7,6 +7,7 @@
 // the first frames.  Outputs per descriptor: word id, word weight, id of the ancestor `levelsup` levels above the leaves --
 // the BowVector / FeatureVector maps are assembled from them in feature order by the caller (their double accumulation
 // order is part of the result).
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -61,19 +62,22 @@ using namespace b200;
 
 struct orbv {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   long long launches = 0;
   int k = 0, L = 0, n_nodes = 0, n_words = 0;
-  uint4* d_desc = nullptr;
-  int *d_first = nullptr, *d_nch = nullptr, *d_orig = nullptr, *d_word = nullptr;
-  double* d_weight = nullptr;
-  void* d_io = nullptr;
-  size_t io_bytes = 0;
-  ~orbv() {
-    DeviceGuard g(device);
-    auto F = [](void* p) { if (p) cudaFree(p); };
-    F(d_desc); F(d_first); F(d_nch); F(d_orig); F(d_word); F(d_weight); F(d_io);
-    if (stream) cudaStreamDestroy(stream);
+  DeviceBlock tree;   // the renumbered vocabulary tree, uploaded once by orbv_create
+  VocView v{};
+  DeviceBlock io;     // orbv_transform's inputs and outputs
+};
+
+// The tree's arrays in the layout of the device block; orbv_create fills a host copy of the same layout.
+struct TreeArrays {
+  uint8_t* desc;
+  int *first, *nch, *orig, *word;
+  double* weight;
+  void take(Carver& t, int n) {
+    desc = t.take<uint8_t>((size_t)n * 32); first = t.take<int>(n); nch = t.take<int>(n); orig = t.take<int>(n);
+    word = t.take<int>(n); weight = t.take<double>(n);
   }
 };
 
@@ -93,10 +97,16 @@ int orbv_create(int device, int k, int L, int n_nodes, const int32_t* parent, co
   std::vector<int> order;   // new index -> DBoW2 id
   order.reserve(n_nodes);
   order.push_back(0);
-  std::vector<int> first(n_nodes, -1), nch(n_nodes, 0);
+  TreeArrays ht, dt;
+  Carver probe;
+  ht.take(probe, n_nodes);
+  std::vector<char> staging(probe.off);
+  Carver hc(staging.data(), staging.size());
+  ht.take(hc, n_nodes);
   for (size_t q = 0; q < order.size(); ++q) {
     const int id = order[q];
-    if (!ch[id].empty()) { first[q] = (int)order.size(); nch[q] = (int)ch[id].size(); }
+    ht.first[q] = ch[id].empty() ? -1 : (int)order.size();
+    ht.nch[q] = (int)ch[id].size();
     for (int c : ch[id]) order.push_back(c);
   }
   if ((int)order.size() != n_nodes) { set_error("the parent array is not a tree rooted at node 0"); return B200ORB_EINVAL; }
@@ -105,37 +115,23 @@ int orbv_create(int device, int k, int L, int n_nodes, const int32_t* parent, co
   int nw = 0;
   for (int id = 1; id < n_nodes; ++id)
     if (ch[id].empty()) { word_of[id] = word_id ? word_id[id] : nw; ++nw; }
-  std::vector<uint8_t> hdesc((size_t)n_nodes * 32);
-  std::vector<int> horig(n_nodes), hword(n_nodes);
-  std::vector<double> hw(n_nodes);
   for (int q = 0; q < n_nodes; ++q) {
     const int id = order[q];
-    memcpy(&hdesc[(size_t)q * 32], desc + (size_t)id * 32, 32);
-    horig[q] = id; hword[q] = word_of[id] < 0 ? 0 : word_of[id]; hw[q] = weight[id];
+    memcpy(ht.desc + (size_t)q * 32, desc + (size_t)id * 32, 32);
+    ht.orig[q] = id; ht.word[q] = word_of[id] < 0 ? 0 : word_of[id]; ht.weight[q] = weight[id];
   }
-  orbv* h = new (std::nothrow) orbv();
+  std::unique_ptr<orbv> h(new (std::nothrow) orbv());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
   h->device = device; h->k = k; h->L = L; h->n_nodes = n_nodes; h->n_words = nw;
-  auto fail = [&](cudaError_t e) { set_error("orbv_create: %s", cudaGetErrorString(e)); delete h; return B200ORB_ECUDA; };
-  cudaError_t e;
-  if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_desc, (size_t)n_nodes * 32)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_first, 4 * (size_t)n_nodes)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_nch, 4 * (size_t)n_nodes)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_orig, 4 * (size_t)n_nodes)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_word, 4 * (size_t)n_nodes)) != cudaSuccess) return fail(e);
-  if ((e = cudaMalloc(&h->d_weight, 8 * (size_t)n_nodes)) != cudaSuccess) return fail(e);
-  cudaMemcpyAsync(h->d_desc, hdesc.data(), (size_t)n_nodes * 32, cudaMemcpyHostToDevice, h->stream);
-  cudaMemcpyAsync(h->d_first, first.data(), 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, h->stream);
-  cudaMemcpyAsync(h->d_nch, nch.data(), 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, h->stream);
-  cudaMemcpyAsync(h->d_orig, horig.data(), 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, h->stream);
-  cudaMemcpyAsync(h->d_word, hword.data(), 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, h->stream);
-  cudaMemcpyAsync(h->d_weight, hw.data(), 8 * (size_t)n_nodes, cudaMemcpyHostToDevice, h->stream);
-  if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return fail(e);
-  *out = h;
+  B200_CHECK(h->stream.create());
+  B200_CHECK(h->tree.carve(h->stream, [&](Carver& t) { dt.take(t, n_nodes); }));
+  B200_CUDA(cudaMemcpyAsync(h->tree.p, staging.data(), staging.size(), cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  h->v = VocView{(const uint4*)dt.desc, dt.first, dt.nch, dt.orig, dt.word, dt.weight, L};
+  *out = h.release();
   return B200ORB_OK;
 }
-void orbv_destroy(orbv_t* h) { delete h; }
+void orbv_destroy(orbv_t* h) { destroy_handle(h); }
 int orbv_num_words(const orbv_t* h) { return h ? h->n_words : 0; }
 long long orbv_launch_count(const orbv_t* h) { return h ? h->launches : 0; }
 
@@ -144,20 +140,14 @@ int orbv_transform(orbv_t* h, const uint8_t* desc, int n, int levelsup, uint32_t
   if (!h || n < 0 || (n > 0 && (!desc || !word_id || !word_weight || !node_id))) { set_error("bad argument"); return B200ORB_EINVAL; }
   if (n == 0) return B200ORB_OK;
   DeviceGuard g(h->device);
-  const size_t need = (size_t)n * (32 + 4 + 8 + 4) + 1024;
-  if (need > h->io_bytes) {
-    if (h->d_io) { cudaStreamSynchronize(h->stream); cudaFree(h->d_io); h->d_io = nullptr; h->io_bytes = 0; }
-    B200_CUDA(cudaMalloc(&h->d_io, need * 2));
-    h->io_bytes = need * 2;
-  }
-  char* p = (char*)h->d_io;
-  double* d_w = (double*)p; p += align_up_sz((size_t)n * 8, 256);
-  uint8_t* d_d = (uint8_t*)p; p += align_up_sz((size_t)n * 32, 256);
-  unsigned* d_word = (unsigned*)p; p += align_up_sz((size_t)n * 4, 256);
-  unsigned* d_node = (unsigned*)p;
+  double* d_w;
+  uint8_t* d_d;
+  unsigned *d_word, *d_node;
+  B200_CHECK(h->io.reserve(h->stream, [&](Carver& t) {
+    d_w = t.take<double>(n); d_d = t.take<uint8_t>((size_t)n * 32); d_word = t.take<unsigned>(n); d_node = t.take<unsigned>(n);
+  }));
   B200_CUDA(cudaMemcpyAsync(d_d, desc, (size_t)n * 32, cudaMemcpyHostToDevice, h->stream));
-  VocView v{h->d_desc, h->d_first, h->d_nch, h->d_orig, h->d_word, h->d_weight, h->L};
-  k_bow_transform<<<(n + 7) / 8, 256, 0, h->stream>>>(v, d_d, n, levelsup, d_word, d_w, d_node);
+  k_bow_transform<<<(n + 7) / 8, 256, 0, h->stream>>>(h->v, d_d, n, levelsup, d_word, d_w, d_node);
   ++h->launches;
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(word_id, d_word, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));

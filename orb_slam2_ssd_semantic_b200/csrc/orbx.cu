@@ -3,6 +3,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdlib>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -57,8 +58,6 @@ using namespace b200;
 // =====================================================================================================
 // handle
 // =====================================================================================================
-orbx::orbx() {}
-
 int orbx::init(const OrbxParams& p, int dev) {
   prm = p;
   device = dev;
@@ -90,35 +89,15 @@ int orbx::init(const OrbxParams& p, int dev) {
     otab.umax[v] = v0;
     ++v0;
   }
-  B200_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  B200_CHECK(stream.create());
   for (v = 1; v <= HALF_PATCH_SIZE; ++v)   // k_orient_desc tests the circular mask as v <= vmax(|u|)
     if (otab.umax[v] > otab.umax[v - 1]) { set_error("umax table is not non-increasing"); return B200ORB_EINVAL; }
-  float patf[1024];
-  for (int i = 0; i < 1024; ++i) patf[i] = (float)kPatternHost[i];
-  B200_CUDA(cudaMalloc(&d_patf, sizeof(patf)));
-  B200_CUDA(cudaMemcpyAsync(d_patf, patf, sizeof(patf), cudaMemcpyHostToDevice, stream));
+  float pat[1024];
+  for (int i = 0; i < 1024; ++i) pat[i] = (float)kPatternHost[i];
+  B200_CHECK(patf.carve(stream, [&](Carver& t) { d_patf = t.take<float4>(256); }));
+  B200_CUDA(cudaMemcpyAsync(d_patf, pat, sizeof(pat), cudaMemcpyHostToDevice, stream));
   B200_CUDA(cudaStreamSynchronize(stream));
   return B200ORB_OK;
-}
-
-void orbx::free_geometry() {
-  auto F = [](void* p) { if (p) cudaFree(p); };
-  F(d_raw); F(d_blur); F(d_cells); F(d_cand); F(d_cellcnt); F(d_qkp); F(d_qnode); F(d_sel); F(d_selcnt);
-  F(d_candcnt); F(d_kps); F(d_desc); F(d_n); F(d_xt); F(d_yt); F(d_xg); F(d_tmp); F(d_blur_tiles); F(d_blur_edges);
-  d_blur_tiles = nullptr; d_blur_edges = nullptr;
-  d_raw = d_blur = nullptr; d_cells = nullptr; d_cand = nullptr; d_cellcnt = nullptr; d_qkp = nullptr;
-  d_qnode = nullptr; d_sel = nullptr; d_selcnt = nullptr; d_candcnt = nullptr; d_kps = nullptr; d_desc = nullptr;
-  d_n = nullptr; d_xt = d_yt = nullptr; d_xg = nullptr; d_tmp = nullptr; tmp_bytes = 0;
-  if (h_stage) cudaFreeHost(h_stage);
-  h_stage = nullptr; stage_bytes = 0;
-  rows = cols = maxF = 0;
-}
-
-orbx::~orbx() {
-  DeviceGuard g(device);
-  free_geometry();
-  if (d_patf) cudaFree(d_patf);
-  if (stream) cudaStreamDestroy(stream);
 }
 
 // (re)build every geometry-dependent table and buffer for F frames of rows x cols
@@ -126,8 +105,8 @@ int orbx::ensure_geometry(int r, int c, int F) {
   if (r == rows && c == cols && F <= maxF) return B200ORB_OK;
   if (r > 4095 || c > 4095) { set_error("image %dx%d exceeds the 4095-px packing limit", c, r); return B200ORB_EINVAL; }
   const int keepF = (r == rows && c == cols) ? std::max(F, maxF) : F;
-  B200_CUDA(cudaStreamSynchronize(stream));
-  free_geometry();
+  rows = cols = maxF = 0;   // no geometry until its block exists
+  have_results = false;
   const int nl = prm.nlevels;
   // level sizes (:1121-1122)
   size_t off = 0;
@@ -261,47 +240,37 @@ int orbx::ensure_geometry(int r, int c, int F) {
   if (qt_smem > 100 * 1024) { set_error("nfeatures too large for the quad-tree kernel's shared memory"); return B200ORB_EINVAL; }
   B200_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qt_smem));
 
-  rows = r; cols = c; maxF = keepF;
-  const size_t Fz = (size_t)maxF;
-  B200_CUDA(cudaMalloc(&d_raw, frame_bytes * Fz));
-  B200_CUDA(cudaMalloc(&d_blur, frame_bytes * Fz));
-  B200_CUDA(cudaMalloc(&d_cells, sizeof(CellDesc) * ncells));
-  B200_CUDA(cudaMalloc(&d_cand, sizeof(unsigned) * slots_per_frame * Fz));
-  B200_CUDA(cudaMalloc(&d_cellcnt, sizeof(int) * ncells * Fz));
-  B200_CUDA(cudaMalloc(&d_qkp, sizeof(unsigned) * slots_per_frame * Fz));
-  B200_CUDA(cudaMalloc(&d_qnode, sizeof(int) * slots_per_frame * Fz));
-  B200_CUDA(cudaMalloc(&d_sel, sizeof(unsigned) * sel_per_frame * Fz));
-  B200_CUDA(cudaMalloc(&d_selcnt, sizeof(int) * nl * Fz));
-  B200_CUDA(cudaMalloc(&d_candcnt, sizeof(int) * nl * Fz));
-  B200_CUDA(cudaMalloc(&d_kps, sizeof(OrbxKeyPoint) * cap * Fz));
-  B200_CUDA(cudaMalloc(&d_desc, (size_t)32 * cap * Fz));
-  B200_CUDA(cudaMalloc(&d_n, sizeof(int) * Fz));
-  B200_CUDA(cudaMalloc(&d_xt, sizeof(int2) * std::max<size_t>(xt.size(), 1)));
-  B200_CUDA(cudaMalloc(&d_yt, sizeof(int2) * std::max<size_t>(yt.size(), 1)));
-  B200_CUDA(cudaMalloc(&d_xg, sizeof(int4) * std::max<size_t>(xg.size(), 1)));
-  {
-    std::vector<BlurTile> bt;
-    for (int l = 0; l < nl; ++l)
-      for (int y = 0; y < lh[l]; y += BLS_ROWS)
-        for (int x = 0; x < lw[l]; x += 128) bt.push_back(BlurTile{(short)l, (short)x, (short)y, 0});
-    n_blur_tiles = (int)bt.size();
-    std::vector<BlurEdge> be;
-    for (int l = 0; l < nl; ++l)
-      for (int x = 0; x < lw[l]; x += 4)
-        if (x < 4 || x + 8 > lw[l])
-          for (int y = 0; y < lh[l]; y += BLS_ROWS) be.push_back(BlurEdge{(short)l, (short)x, (short)y, 0});
-    n_blur_edges = (int)be.size();
-    B200_CUDA(cudaMalloc(&d_blur_edges, sizeof(BlurEdge) * be.size()));
-    B200_CUDA(cudaMemcpyAsync(d_blur_edges, be.data(), sizeof(BlurEdge) * be.size(), cudaMemcpyHostToDevice, stream));
-    B200_CUDA(cudaMalloc(&d_blur_tiles, sizeof(BlurTile) * bt.size()));
-    B200_CUDA(cudaMemcpyAsync(d_blur_tiles, bt.data(), sizeof(BlurTile) * bt.size(), cudaMemcpyHostToDevice, stream));
-    B200_CUDA(cudaStreamSynchronize(stream));   // bt is a local
-  }
+  std::vector<BlurTile> bt;
+  for (int l = 0; l < nl; ++l)
+    for (int y = 0; y < lh[l]; y += BLS_ROWS)
+      for (int x = 0; x < lw[l]; x += 128) bt.push_back(BlurTile{(short)l, (short)x, (short)y, 0});
+  n_blur_tiles = (int)bt.size();
+  std::vector<BlurEdge> be;
+  for (int l = 0; l < nl; ++l)
+    for (int x = 0; x < lw[l]; x += 4)
+      if (x < 4 || x + 8 > lw[l])
+        for (int y = 0; y < lh[l]; y += BLS_ROWS) be.push_back(BlurEdge{(short)l, (short)x, (short)y, 0});
+  n_blur_edges = (int)be.size();
+
+  const size_t Fz = (size_t)keepF;
+  B200_CHECK(geom.carve(stream, [&](Carver& t) {
+    d_raw = t.take<uint8_t>(frame_bytes * Fz); d_blur = t.take<uint8_t>(frame_bytes * Fz);
+    d_cells = t.take<CellDesc>(ncells); d_cand = t.take<unsigned>(slots_per_frame * Fz);
+    d_cellcnt = t.take<int>(ncells * Fz); d_qkp = t.take<unsigned>(slots_per_frame * Fz);
+    d_qnode = t.take<int>(slots_per_frame * Fz); d_sel = t.take<unsigned>(sel_per_frame * Fz);
+    d_selcnt = t.take<int>(nl * Fz); d_candcnt = t.take<int>(nl * Fz);
+    d_kps = t.take<OrbxKeyPoint>(cap * Fz); d_desc = t.take<uint8_t>(32 * cap * Fz); d_n = t.take<int>(Fz);
+    d_xt = t.take<int2>(xt.size()); d_yt = t.take<int2>(yt.size()); d_xg = t.take<int4>(xg.size());
+    d_blur_tiles = t.take<BlurTile>(bt.size()); d_blur_edges = t.take<BlurEdge>(be.size());
+  }));
+  B200_CUDA(cudaMemcpyAsync(d_blur_edges, be.data(), sizeof(BlurEdge) * be.size(), cudaMemcpyHostToDevice, stream));
+  B200_CUDA(cudaMemcpyAsync(d_blur_tiles, bt.data(), sizeof(BlurTile) * bt.size(), cudaMemcpyHostToDevice, stream));
   B200_CUDA(cudaMemcpyAsync(d_cells, cells.data(), sizeof(CellDesc) * ncells, cudaMemcpyHostToDevice, stream));
   if (!xt.empty()) B200_CUDA(cudaMemcpyAsync(d_xt, xt.data(), sizeof(int2) * xt.size(), cudaMemcpyHostToDevice, stream));
   if (!yt.empty()) B200_CUDA(cudaMemcpyAsync(d_yt, yt.data(), sizeof(int2) * yt.size(), cudaMemcpyHostToDevice, stream));
   if (!xg.empty()) B200_CUDA(cudaMemcpyAsync(d_xg, xg.data(), sizeof(int4) * xg.size(), cudaMemcpyHostToDevice, stream));
-  B200_CUDA(cudaStreamSynchronize(stream));
+  B200_CUDA(cudaStreamSynchronize(stream));   // the tables are locals
+  rows = r; cols = c; maxF = keepF;
   // blurred pyramid view never changes; raw view's level 0 may alias the caller's buffer per call
   for (int l = 0; l < nl; ++l) {
     blurv.p[l] = d_blur + loff[l]; blurv.fstride[l] = frame_bytes; blurv.pitch[l] = lpitch[l];
@@ -309,7 +278,6 @@ int orbx::ensure_geometry(int r, int c, int F) {
     rawv.p[l] = d_raw + loff[l]; rawv.fstride[l] = frame_bytes; rawv.pitch[l] = lpitch[l];
     rawv.w[l] = lw[l]; rawv.h[l] = lh[l];
   }
-  have_results = false;
   return B200ORB_OK;
 }
 
@@ -396,37 +364,16 @@ int orbx::run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0) {
 
 int orbx::prof_begin(int frames) {
   if (!profile) return B200ORB_OK;
-  StageEvents se;
-  memset(&se, 0, sizeof(se));
-  se.frames = frames;
-  prof_runs.push_back(se);
+  prof_runs.emplace_back();
+  prof_runs.back().frames = frames;
   return prof_mark(0);
 }
 
 int orbx::prof_mark(int boundary) {
   if (!profile || prof_runs.empty()) return B200ORB_OK;
   StageEvents& se = prof_runs.back();
-  B200_CUDA(cudaEventCreate(&se.ev[boundary]));
+  B200_CHECK(se.ev[boundary].create(/*timing=*/1));
   B200_CUDA(cudaEventRecord(se.ev[boundary], stream));
-  se.used[boundary] = true;
-  return B200ORB_OK;
-}
-
-int orbx::ensure_stage(size_t bytes) {
-  if (bytes <= stage_bytes) return B200ORB_OK;
-  if (h_stage) cudaFreeHost(h_stage);
-  h_stage = nullptr; stage_bytes = 0;
-  B200_CUDA(cudaHostAlloc(&h_stage, bytes, cudaHostAllocDefault));
-  stage_bytes = bytes;
-  return B200ORB_OK;
-}
-
-int orbx::ensure_tmp(size_t bytes) {
-  if (bytes <= tmp_bytes) return B200ORB_OK;
-  if (d_tmp) cudaFree(d_tmp);
-  d_tmp = nullptr; tmp_bytes = 0;
-  B200_CUDA(cudaMalloc(&d_tmp, bytes));
-  tmp_bytes = bytes;
   return B200ORB_OK;
 }
 
@@ -460,15 +407,14 @@ int orbx_create(const OrbxParams* p, int device, orbx_t** out) {
   }
   B200_CHECK(check_device(device));
   DeviceGuard g(device);
-  orbx* h = new (std::nothrow) orbx();
+  std::unique_ptr<orbx> h(new (std::nothrow) orbx());
   if (!h) { set_error("out of host memory"); return B200ORB_EINVAL; }
-  int rc = h->init(*p, device);
-  if (rc != B200ORB_OK) { delete h; return rc; }
-  *out = h;
+  B200_CHECK(h->init(*p, device));
+  *out = h.release();
   return B200ORB_OK;
 }
 
-void orbx_destroy(orbx_t* h) { delete h; }
+void orbx_destroy(orbx_t* h) { destroy_handle(h); }
 
 int orbx_max_keypoints(const orbx_t* h) {
   if (!h) return 0;
@@ -509,15 +455,16 @@ int orbx_extract_batch(orbx_t* h, const uint8_t* gray, int nframes, int rows, in
   if (!kps || !desc || cap <= 0) { set_error("null/empty output buffers"); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
   B200_CHECK(extract_common(h, gray, false, nframes, rows, cols, stride, frame_stride));
-  const size_t kb = sizeof(OrbxKeyPoint) * h->cap, db = (size_t)32 * h->cap;
-  B200_CHECK(h->ensure_stage((kb + db) * nframes + sizeof(int) * nframes));
-  char* hs = (char*)h->h_stage;
-  OrbxKeyPoint* hk = (OrbxKeyPoint*)hs;
-  uint8_t* hd = (uint8_t*)(hs + kb * nframes);
-  int* hn = (int*)(hs + (kb + db) * nframes);
+  const size_t kn = (size_t)h->cap * nframes;
+  OrbxKeyPoint* hk;
+  uint8_t* hd;
+  int* hn;
+  B200_CHECK(h->stage.reserve(h->stream, [&](Carver& t) {
+    hk = t.take<OrbxKeyPoint>(kn); hd = t.take<uint8_t>(32 * kn); hn = t.take<int>(nframes);
+  }));
   B200_CUDA(cudaMemcpyAsync(hn, h->d_n, sizeof(int) * nframes, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaMemcpyAsync(hk, h->d_kps, kb * nframes, cudaMemcpyDeviceToHost, h->stream));
-  B200_CUDA(cudaMemcpyAsync(hd, h->d_desc, db * nframes, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(hk, h->d_kps, sizeof(OrbxKeyPoint) * kn, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(hd, h->d_desc, 32 * kn, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   int rc = B200ORB_OK;
   for (int f = 0; f < nframes; ++f) {
@@ -560,7 +507,7 @@ int orbx_sync(orbx_t* h) {
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
 }
-void* orbx_stream(orbx_t* h) { return h ? (void*)h->stream : nullptr; }
+void* orbx_stream(orbx_t* h) { return h ? (void*)(cudaStream_t)h->stream : nullptr; }
 
 int orbx_level_dims(const orbx_t* h, int level, int* rows, int* cols) {
   if (!h || level < 0 || level >= h->prm.nlevels || h->rows == 0) { set_error("bad level / no geometry yet"); return B200ORB_EINVAL; }
@@ -585,11 +532,12 @@ int orbx_get_level(orbx_t* h, int frame, int level, int bordered, uint8_t* dst, 
   }
   const int B = EDGE_THRESHOLD, bw = w + 2 * B, bh = hh + 2 * B;
   if (dst_stride < (size_t)bw) { set_error("dst_stride too small"); return B200ORB_EINVAL; }
-  B200_CHECK(h->ensure_tmp((size_t)bw * bh));
+  uint8_t* d_tmp;
+  B200_CHECK(h->tmp.reserve(h->stream, [&](Carver& t) { d_tmp = t.take<uint8_t>((size_t)bw * bh); }));
   dim3 blk(32, 8), grd((bw + 31) / 32, (bh + 7) / 8);
-  k_border_copy<<<grd, blk, 0, h->stream>>>(src, h->rawv.pitch[level], w, hh, (uint8_t*)h->d_tmp, bw, B);
+  k_border_copy<<<grd, blk, 0, h->stream>>>(src, h->rawv.pitch[level], w, hh, d_tmp, bw, B);
   ++h->launches;
-  B200_CUDA(cudaMemcpy2DAsync(dst, dst_stride, h->d_tmp, bw, bw, bh, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpy2DAsync(dst, dst_stride, d_tmp, bw, bw, bh, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
 }
@@ -635,13 +583,12 @@ int orbx_profile_read(orbx_t* h, float* ms /*B200ORB_NUM_STAGES*/, long long* fr
     fr += se.frames;
     int prev = 0;
     for (int b = 1; b <= ST_COUNT; ++b) {
-      if (!se.used[b]) continue;
+      if (!se.ev[b]) continue;
       float t = 0.f;
-      if (se.used[prev]) cudaEventElapsedTime(&t, se.ev[prev], se.ev[b]);
+      if (se.ev[prev]) cudaEventElapsedTime(&t, se.ev[prev], se.ev[b]);
       ms[b - 1] += t;
       prev = b;
     }
-    for (int b = 0; b <= ST_COUNT; ++b) if (se.used[b]) cudaEventDestroy(se.ev[b]);
   }
   if (frames) *frames = fr;
   if (runs) *runs = (int)h->prof_runs.size();

@@ -7,16 +7,15 @@
 namespace b200 {
 enum { ST_RESIZE = 0, ST_FAST, ST_QUADTREE, ST_BLUR, ST_ORIENT_DESC, ST_GLUE, ST_MATCH, ST_COUNT };
 struct StageEvents {
-  cudaEvent_t ev[ST_COUNT + 1];
-  bool used[ST_COUNT + 1];
-  int frames;
+  Event ev[ST_COUNT + 1];   // null: the boundary was not recorded
+  int frames = 0;
 };
 }  // namespace b200
 
 struct orbx {
   OrbxParams prm{};
   int device = 0;
-  cudaStream_t stream = nullptr;
+  b200::Stream stream;
   long long launches = 0;
   // optional hook, called by run() right after the keypoint selection of frames [f0, f0 + F) has been enqueued
   // (the batch tracker uses it to start fetching the depth under the selected keypoints while blur / descriptors run)
@@ -26,6 +25,7 @@ struct orbx {
   float sf[b200::MAX_LEVELS], invsf[b200::MAX_LEVELS], sigma2[b200::MAX_LEVELS], invsigma2[b200::MAX_LEVELS];
   int nfeat[b200::MAX_LEVELS];
   b200::OrientTab otab{};
+  b200::DeviceBlock patf;
   float4* d_patf = nullptr;   // the 256 tests as float4 (x0, y0, x1, y1), for k_orient_desc
   // geometry-dependent state
   int rows = 0, cols = 0, maxF = 0, lastF = 0;
@@ -35,6 +35,7 @@ struct orbx {
   int xt_off[b200::MAX_LEVELS], yt_off[b200::MAX_LEVELS], xg_off[b200::MAX_LEVELS];
   b200::LevelTab ltab{};
   b200::PyrView rawv{}, blurv{};
+  b200::DeviceBlock geom;   // carved for (rows, cols, maxF): every d_ array below
   int ncells = 0, slots_per_frame = 0, sel_per_frame = 0, cap = 0, qt_cap = 0;
   size_t qt_smem = 0;
   int fast_tp = 0, fast_rows_max = 0, fast_clist_cap = 0;
@@ -56,23 +57,16 @@ struct orbx {
   b200::BlurTile* d_blur_tiles = nullptr;
   b200::BlurEdge* d_blur_edges = nullptr;
   int n_blur_tiles = 0, n_blur_edges = 0;
-  void* d_tmp = nullptr;
-  size_t tmp_bytes = 0;
-  void* h_stage = nullptr;
-  size_t stage_bytes = 0;
+  b200::DeviceBlock tmp;    // orbx_get_level's bordered copy
+  b200::HostBlock stage;    // orbx_extract_batch's downloads
   bool have_results = false;
   // optional per-stage CUDA-event timing (bench.py's roofline leg): one event set per run(), read lazily
   bool profile = false;
   std::vector<b200::StageEvents> prof_runs;
 
-  orbx();
-  ~orbx();
   int init(const OrbxParams& p, int dev);
-  void free_geometry();
   int ensure_geometry(int r, int c, int F);
   int run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0 = 0);
-  int ensure_stage(size_t bytes);
-  int ensure_tmp(size_t bytes);
   int prof_mark(int boundary);   // record event `boundary` of the current run (no-op unless profiling)
   int prof_begin(int frames);
 };
