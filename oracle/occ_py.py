@@ -49,7 +49,10 @@ class PyOccupancy:
                 y = F32(F32(F32(m) - cy) * z) / fy
                 if y < -self.y_max or y > self.y_max:
                     continue
-                key = (int(math.floor(F32(z * inv_leaf))), int(math.floor(F32(y * inv_leaf))), int(math.floor(F32(x * inv_leaf))))
+                if math.isfinite(x) and math.isfinite(y) and math.isfinite(z):
+                    key = (int(math.floor(F32(z * inv_leaf))), int(math.floor(F32(y * inv_leaf))), int(math.floor(F32(x * inv_leaf))))
+                else:                                    # NaN depth passes both gates: one cell of its own, emitted last
+                    key = (math.inf, math.inf, math.inf)
                 acc = cells.setdefault(key, [F32(0), F32(0), F32(0), 0, 0 if label is None else int(label[m, n])])
                 acc[0] = F32(acc[0] + x); acc[1] = F32(acc[1] + y); acc[2] = F32(acc[2] + z)   # row-major pixel order
                 acc[3] += 1
@@ -71,6 +74,8 @@ class PyOccupancy:
 
     # ---- octomap -------------------------------------------------------------------------------------------------
     def coord_to_key(self, c) -> int | None:
+        if not math.isfinite(c):      # a non-finite coordinate never makes a key
+            return None
         k = int(math.floor(self.res_factor * float(c))) + 32768
         return k if 0 <= k < 65536 else None
 

@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <thread>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -48,10 +49,15 @@ struct OccMap {
     cmax = logodds(q.clamp_max);
   }
   static uint64_t pack(const uint16_t k[3]) { return (uint64_t)k[0] | ((uint64_t)k[1] << 16) | ((uint64_t)k[2] << 32); }
-  bool coord_to_key(double c, uint16_t& k) const {   // coordToKeyChecked, tree_max_val = 32768
-    const int s = ((int)std::floor(res_factor * c)) + 32768;
-    if (s >= 0 && (unsigned)s < 65536u) { k = (uint16_t)s; return true; }
-    return false;
+  // coordToKeyChecked, tree_max_val = 32768.  A non-finite coordinate never makes a key: octomap gets there on x86 only
+  // through the undefined int conversion of NaN (INT_MIN); here the rule is explicit, and the range test is made before
+  // the conversion.
+  bool coord_to_key(double c, uint16_t& k) const {
+    if (!std::isfinite(c)) return false;
+    const double f = std::floor(res_factor * c);
+    if (!(f >= -32768.0 && f < 32768.0)) return false;
+    k = (uint16_t)((int)f + 32768);
+    return true;
   }
   bool point_to_key(const float* pt, uint16_t k[3]) const {
     return coord_to_key((double)pt[0], k[0]) && coord_to_key((double)pt[1], k[1]) && coord_to_key((double)pt[2], k[2]);
@@ -117,6 +123,9 @@ struct OccMap {
                 float cx, float cy, const uint8_t* label) {
     struct Acc { float sx = 0, sy = 0, sz = 0, sr = 0, sg = 0, sb = 0; int n = 0; uint8_t label = 0; };
     std::map<std::tuple<int, int, int>, Acc> vox;   // ordered by (iz, iy, ix): PCL's ascending linear index
+    // NaN depth passes both gates (:655); those pixels form one cell of their own (emitted last) rather than one whose
+    // index comes from an undefined int conversion.  Its centroid is NaN, so it never makes an octree key.
+    Acc nonfinite;
     std::vector<float> raw;
     std::vector<uint8_t> raw_rgb, raw_label;
     const bool filter = p.leaf > 0;
@@ -137,14 +146,17 @@ struct OccMap {
           raw_label.push_back(lab);
           continue;
         }
-        const int ix = (int)std::floor(x * inv_leaf), iy = (int)std::floor(y * inv_leaf), iz = (int)std::floor(z * inv_leaf);
-        Acc& a = vox[std::make_tuple(iz, iy, ix)];
+        const bool finite = std::isfinite(x) && std::isfinite(y) && std::isfinite(z);
+        const int ix = finite ? (int)std::floor(x * inv_leaf) : 0, iy = finite ? (int)std::floor(y * inv_leaf) : 0,
+                  iz = finite ? (int)std::floor(z * inv_leaf) : 0;
+        Acc& a = finite ? vox[std::make_tuple(iz, iy, ix)] : nonfinite;
         if (a.n == 0) a.label = lab;
         a.sx += x; a.sy += y; a.sz += z;
         a.sr += (float)c[2]; a.sg += (float)c[1]; a.sb += (float)c[0];
         a.n++;
       }
     if (filter) {
+      if (nonfinite.n) vox.emplace(std::make_tuple(INT_MAX, INT_MAX, INT_MAX), nonfinite);   // sorts last
       for (auto& kv : vox) {
         const Acc& a = kv.second;
         const float fn = (float)a.n;

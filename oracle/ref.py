@@ -341,6 +341,9 @@ class RefOccupancy:
         e = np.ascontiguousarray(end, np.float32)
         keys = np.zeros((4096, 3), np.uint16)
         n = self.L.occ_ref_ray(self.h, _p(o), _p(e), _p(keys), 4096)
+        if n > len(keys):        # a long ray: ask again with room for all of it
+            keys = np.zeros((n, 3), np.uint16)
+            n = self.L.occ_ref_ray(self.h, _p(o), _p(e), _p(keys), n)
         return None if n < 0 else keys[:n].copy()
 
 

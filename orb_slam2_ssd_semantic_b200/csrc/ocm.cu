@@ -181,7 +181,13 @@ __device__ __forceinline__ bool backproject(const OcmConst& c, const float* __re
   return true;
 }
 
+// VoxelGrid cell of a gated point: 21 bits per axis (ocm_insert_* refuse gates and intrinsics that would let
+// |coord / leaf| reach 2^20, where cells would alias).  NaN depth passes both gates (MapDrawer.cc:655 keeps it); those
+// pixels share one cell of their own, NONFINITE_CELL (bit 63: no real cell has it, and it is not a sentinel of k_ocm_bin),
+// instead of the cell that cvt's NaN -> 0 would give them.  Their centroid is NaN, so they never reach the map.
+constexpr unsigned long long NONFINITE_CELL = 1ull << 63;
 __device__ __forceinline__ unsigned long long leaf_key(const OcmConst& c, float x, float y, float z) {
+  if (!(isfinite(x) && isfinite(y) && isfinite(z))) return NONFINITE_CELL;
   const long long ix = (long long)floorf(x * c.inv_leaf) + (1 << 20);
   const long long iy = (long long)floorf(y * c.inv_leaf) + (1 << 20);
   const long long iz = (long long)floorf(z * c.inv_leaf) + (1 << 20);
@@ -337,10 +343,12 @@ __global__ void k_ocm_points_nofilter(const KfJob* __restrict__ jobs) {
   pts_label[v] = label ? label[pix] : 0;
 }
 
-__device__ __forceinline__ bool coord_to_key(const OcmConst& c, float coord, int& k) {   // coordToKeyChecked
-  const int s = (int)floor(c.res_factor * (double)coord) + 32768;
-  k = s;
-  return s >= 0 && s < 65536;
+// coordToKeyChecked.  The range test is made on the double, before the conversion: a non-finite coordinate never makes a
+// key (cvt turns NaN into 0, which would be the in-range key 32768, and +-inf into INT_MAX / INT_MIN).
+__device__ __forceinline__ bool coord_to_key(const OcmConst& c, float coord, int& k) {
+  const double f = floor(c.res_factor * (double)coord);
+  k = (int)f + 32768;
+  return f >= -32768.0 && f < 32768.0;
 }
 __device__ __forceinline__ unsigned long long pack_key(int kx, int ky, int kz) {
   return (unsigned long long)kx | ((unsigned long long)ky << 16) | ((unsigned long long)kz << 32);
@@ -701,10 +709,33 @@ int ocm::check_err() {
   return B200ORB_OK;
 }
 
+// The VoxelGrid cell key holds 21 bits per axis (leaf_key): distinct cells alias once |coord / leaf| reaches 2^20, so
+// gates and intrinsics that allow it are refused.  Float rounding is monotonic, so the largest |coord * inv_leaf| a gated
+// pixel can produce is the one of the outermost pixel column / row at the largest |depth|, computed here with the same
+// float operations as backproject() and leaf_key().  (A NaN gate lets every depth through: refused as well.)
+static int check_leaf_range(const OcmParams& p, int rows, int cols, float fx, float fy, float cx, float cy) {
+  if (!(p.leaf > 0)) return B200ORB_OK;   // no VoxelGrid
+  const float inv_leaf = 1.0f / p.leaf;
+  const float z = std::isnan(p.depth_min) || std::isnan(p.depth_max) ? INFINITY
+                                                                     : std::max(std::fabs(p.depth_min), std::fabs(p.depth_max));
+  auto reach = [z](int last, float c, float f) {   // max over pixel index 0..last of |(n - c) * z / f|
+    return std::max(std::fabs((0.f - c) * z / f), std::fabs(((float)last - c) * z / f));
+  };
+  const float b[3] = {reach(cols - 1, cx, fx) * inv_leaf, std::min(reach(rows - 1, cy, fy), std::fabs(p.y_max)) * inv_leaf,
+                      z * inv_leaf};
+  if (!(b[0] < 1048576.f && b[1] < 1048576.f && b[2] < 1048576.f)) {
+    set_error("occupancy insert: |coord / leaf| can reach (%g, %g, %g); the VoxelGrid cell key needs it below 2^20 "
+              "(lower depth_max / y_max or raise leaf)", b[0], b[1], b[2]);
+    return B200ORB_EINVAL;
+  }
+  return B200ORB_OK;
+}
+
 // n keyframes (insertion order = array order), up to MAX_SLOTS per round of launches: every stage is one launch for
 // the whole round, including the map update (per-voxel replay of the round's observations in keyframe order).
 int ocm::insert_batch(int n, const float* const* dd, const uint8_t* const* drgb, const uint8_t* const* dlabel, int r, int c,
                       const float* Tcw_all, float fx, float fy, float cx, float cy) {
+  B200_CHECK(check_leaf_range(prm, r, c, fx, fy, cx, cy));
   B200_CHECK(ensure_scratch(r, c, n));
   const int npix = r * c;
   for (int b0 = 0; b0 < n; b0 += (int)slots.size()) {
@@ -924,9 +955,10 @@ int ocm_query(ocm_t* h, const float xyz[3], float* logodds, int* found) {
   DeviceGuard g(h->device);
   int k[3];
   const double rf = 1.0 / h->prm.resolution;
-  for (int i = 0; i < 3; ++i) {
-    k[i] = (int)floor(rf * (double)xyz[i]) + 32768;
-    if (k[i] < 0 || k[i] >= 65536) { *found = 0; *logodds = 0; return B200ORB_OK; }
+  for (int i = 0; i < 3; ++i) {   // coord_to_key's rule: a non-finite coordinate has no key
+    const double f = floor(rf * (double)xyz[i]);
+    if (!(f >= -32768.0 && f < 32768.0)) { *found = 0; *logodds = 0; return B200ORB_OK; }
+    k[i] = (int)f + 32768;
   }
   const unsigned long long key = (unsigned long long)k[0] | ((unsigned long long)k[1] << 16) | ((unsigned long long)k[2] << 32);
   k_ocm_query<<<1, 1, 0, h->stream>>>(h->map, key, h->d_query_val, h->d_query_found);

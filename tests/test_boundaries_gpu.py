@@ -553,7 +553,7 @@ def test_map_at_high_load_matches_oracle(loaded_scene):
     kg, lg, _ = pcm.export_leaves()
     pk_g, lo_g = _leaves(kg, lg)
     assert len(pk_g) == n and (pk_g == pk_r).all()
-    assert np.abs(lo_g - lo_r).max() <= 1e-5
+    assert (lo_g.view(np.uint32) == lo_r.view(np.uint32)).all()
     assert (lo_r < 0).sum() > 1000 and (lo_r > 0).sum() > 1000
     # every leaf through the find-only probe
     res = 0.05

@@ -22,7 +22,7 @@ def _leaf_dict(keys, lo):
 def _same_leaves(gpu, ref):
     (pg, lg), (pr, lr) = _leaf_dict(*gpu.export_leaves()[:2]), _leaf_dict(*ref.export_leaves())
     assert len(pr) > 500 and len(pg) == len(pr) and (pg == pr).all()
-    assert np.abs(lg - lr).max() <= 1e-5
+    assert (lg.view(np.uint32) == lr.view(np.uint32)).all()
 
 
 def test_extractor_geometry_and_batch_changes():
@@ -139,7 +139,8 @@ def test_occupancy_scratch_staging_export_and_merge(oracle):
         ref.insert_keyframe(T, depth, rgb, *cam)
         pg, pr = gpu.last_points()[0], ref.last_points()[0]
         assert len(pg) == len(pr) > 100
-        assert np.abs(np.sort(pg, axis=0) - np.sort(pr, axis=0)).max() <= 1e-5
+        rows = lambda p: p.view(np.uint32)[np.lexsort(p.view(np.uint32).T[::-1])]   # noqa: E731
+        assert (rows(pg) == rows(pr)).all()
 
     def insert_u16(ts):
         factor = np.float32(1 / 5000.0)
@@ -169,7 +170,7 @@ def test_occupancy_scratch_staging_export_and_merge(oracle):
     assert L.ocm_export_leaves(gpu.handle, ptr(keys), ptr(lo), ptr(col), n, C.byref(cnt)) == 0 and cnt.value == n
     pg, lg = _leaf_dict(keys, lo)
     pr, lr = _leaf_dict(*ref.export_leaves())
-    assert (pg == pr).all() and np.abs(lg - lr).max() <= 1e-5
+    assert (pg == pr).all() and (lg.view(np.uint32) == lr.view(np.uint32)).all()
 
     for t in (5, 6):
         insert_f32(*frames[t][1:])

@@ -200,7 +200,7 @@ def test_full_size_bench_workload_against_reference_sources(oracle):
     camera), ORBextractor(2000, ...), SearchByProjection(th = 15) -- per-frame keypoint and match counts of the whole batch
     against the reference's OWN tracking sources (oracle/_ref: Frame constructor + ORBmatcher of /root/reference), three
     frames keypoint by keypoint against the oracle, and the occupancy map of the batch's 22 keyframes with the GT floor as
-    ground label (free-space rays) against the sequential occupancy oracle: same leaf set, log-odds within 1e-5."""
+    ground label (free-space rays) against the sequential occupancy oracle: same leaf set, log-odds bit-equal."""
     import os
     from orb_slam2_ssd_semantic_b200 import PointCloudMapping, StreamTracker
     F, KF, NF = 256, 12, 2000
@@ -234,5 +234,5 @@ def test_full_size_bench_workload_against_reference_sources(oracle):
     pk = lambda k: k.astype(np.uint64)[:, 0] | (k.astype(np.uint64)[:, 1] << np.uint64(16)) | (k.astype(np.uint64)[:, 2] << np.uint64(32))
     og, orr = np.argsort(pk(kg)), np.argsort(pk(kr))
     assert len(kg) == len(kr) and (pk(kg)[og] == pk(kr)[orr]).all()
-    assert np.abs(lg[og] - lr[orr]).max() <= 1e-5
+    assert (lg[og].view(np.uint32) == lr[orr].view(np.uint32)).all()
     assert (lr < 0).sum() > 5000 and (lr > 0).sum() > 5000
