@@ -395,6 +395,35 @@ int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d
  * world point Frame::UnprojectStereo gives per keypoint under that frame's pose (:879-899) and whether the keypoint has
  * depth; host arrays of at least the handle's keypoint capacity (NULL = skip). */
 int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, float* xw, uint8_t* valid, int cap);
+/* Masked batches: the `perfect` variant's live path per frame (perfect/src/Tracking.cc:703-719).  Between extraction and the
+ * frame glue, one kernel per batch does Flow::ComputeMask after calcOpticalFlowFarneback (perfect/src/Flow.cc:14-53: pyrUp
+ * of the flow, mask = 0 where x*x + y*y >= max(binary_threshold, 40), erode, erode, dilate with the 21 x 21 ellipse) and
+ * the keypoint loop of the masked RGB-D Frame constructor (perfect/src/Frame.cc:328-427, :356-377: when the mask's sum is
+ * above 65 % of the pixels, keypoints whose pixel is not 1 are dropped with their descriptors, order kept).  Frame t is
+ * then tracked against the filtered frame t-1 with SearchByProjection(cur, last) (perfect/src/Tracking.cc:1933), and
+ * orbs_read_dynamic_mask returns the mask FrameDrawer receives (perfect/src/FrameDrawer.cc:262).
+ * flow[n][rows/2][cols/2][2] f32 is what calcOpticalFlowFarneback returns for the pyrDown'ed previous and current gray
+ * images (CV_32FC2, continuous); mask pixels beyond the 2 (rows/2) x 2 (cols/2) it covers stay 1.  A frame without a
+ * previous image (the sequence's first) takes a zero flow field: its mask is all ones and it keeps every keypoint, the
+ * reference's `mask = ones` case.  Outputs keep the layout of the unmasked entries and describe the FILTERED frames
+ * (nkp, kps, desc, cur2last against frame t-1's filtered keypoints), as do orbs_device_results and orbs_read_frame_glue.
+ * Geometry: a frame's mask is held as two bit planes in one CTA's shared memory, 8 * rows * ceil(cols / 32) + 132 bytes;
+ * on an H100 (232448 bytes per CTA) rows * ceil(cols / 32) <= 29039: 1280 x 720 and 1241 x 376 fit, 1280 x 725 is the
+ * largest 1280-wide image.  Larger images and flow fields under 2 x 2 return B200ORB_EINVAL before anything is enqueued.
+ * A masked batch launches one kernel more than the same unmasked batch; orbx_profile_read counts its time in stage 5. */
+int orbs_track_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                                const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                                uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
+/* Streaming form (as orbs_submit_batch_u16): flow is page-locked too and goes up chunk by chunk next to the gray images. */
+int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                                 const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                                 uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
+/* Device-resident form (as orbs_track_batch_device), d_flow in HBM. */
+int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,
+                                   float binary_threshold, int nframes, int rows, int cols);
+/* Frame `frame` of the last batch, which must have been masked: mask[rows][cols] 0 / 1 (the Flow::ComputeMask result,
+ * FrameDrawer's mDynMask), *filtered = whether the 65 % rule dropped keypoints of this frame (NULL = skip either). */
+int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered);
 int orbs_sync(orbs_t* h);
 void* orbs_stream(orbs_t* h);
 long long orbs_launch_count(const orbs_t* h);

@@ -30,6 +30,7 @@ EXPORTS = [
     "orbm_hamming", "orbm_create", "orbm_destroy", "orbm_launch_count", "orbm_search_by_projection_last",
     "orbm_search_by_projection_points", "orbm_search_by_bow", "orbm_search_by_bow_kf", "orbm_search_projected", "orbm_search_best", "orbm_search_for_initialization", "orbm_search_for_triangulation", "orbm_is_in_frustum", "orbm_undistort_keypoints", "orbv_create", "orbv_destroy", "orbv_num_words", "orbv_launch_count", "orbv_transform",
     "orbs_create", "orbs_destroy", "orbs_track_batch", "orbs_track_batch_u16", "orbs_submit_batch_u16", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_track_batch_device", "orbs_device_results", "orbs_read_frame_glue", "orbs_sync",
+    "orbs_track_batch_u16_masked", "orbs_submit_batch_u16_masked", "orbs_track_batch_masked_device", "orbs_read_dynamic_mask",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
     "ocm_default_params", "ocm_create", "ocm_destroy", "ocm_insert_keyframe", "ocm_insert_keyframe_device",
@@ -128,6 +129,10 @@ def lib() -> C.CDLL:
     L.orbs_track_batch_device.argtypes = [vp, vp, vp, vp, i, i, i]
     L.orbs_device_results.argtypes = [vp] + [C.POINTER(vp)] * 5 + [C.POINTER(i)]
     L.orbs_read_frame_glue.argtypes = [vp, i, vp, vp, vp, vp, i]
+    L.orbs_track_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
+    L.orbs_submit_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
+    L.orbs_track_batch_masked_device.argtypes = [vp, vp, vp, vp, vp, C.c_float, i, i, i]
+    L.orbs_read_dynamic_mask.argtypes = [vp, i, vp, C.POINTER(i)]
     L.orbs_sync.argtypes = [vp]
     L.orbs_stream.argtypes = [vp]
     L.orbs_stream.restype = vp

@@ -14,7 +14,7 @@
 #include <memory>
 #include <new>
 
-#include "common.cuh"
+#include "dynm_plane.cuh"   // pyrup_at, dynm_check_geometry
 
 namespace b200 {
 
@@ -22,34 +22,6 @@ constexpr int DYNM_R = 10;                 // dilation_size, perfect/src/Flow.cc
 constexpr int DYNM_K = 2 * DYNM_R + 1;     // 21 x 21 element
 
 struct EllipseTab { int hw[DYNM_K]; };     // half width of the element's row dy + DYNM_R
-
-// One row-pass value of cv::pyrUp (pyrUp_<FltCast<float,6>>) at output column X of a source row; `row` points at the
-// channel's first element, consecutive pixels are `cn` floats apart.  w >= 2.
-__device__ __forceinline__ float pyrup_row(const float* __restrict__ row, int X, int w, int cn) {
-  const int x = X >> 1;
-  const float x0 = row[(size_t)x * cn];
-  if ((X & 1) == 0) {
-    if (x == 0) return __fadd_rn(__fmul_rn(x0, 6.f), __fmul_rn(row[cn], 2.f));
-    if (x == w - 1) return __fadd_rn(row[(size_t)(x - 1) * cn], __fmul_rn(x0, 7.f));
-    return __fadd_rn(__fadd_rn(__fmul_rn(x0, 6.f), row[(size_t)(x - 1) * cn]), row[(size_t)(x + 1) * cn]);
-  }
-  if (x == w - 1) return __fmul_rn(x0, 8.f);
-  return __fmul_rn(__fadd_rn(x0, row[(size_t)(x + 1) * cn]), 4.f);
-}
-
-__device__ __forceinline__ float pyrup_at(const float* __restrict__ src, int X, int Y, int w, int h, int cn, int c) {
-  const int y = Y >> 1;
-  const size_t rs = (size_t)w * cn;
-  const int yn = (y + 1 < h) ? y + 1 : h - 1;   // borderInterpolate(2 (y+1), 2 h, REFLECT_101) / 2
-  const float r1 = pyrup_row(src + (size_t)y * rs + c, X, w, cn);
-  const float r2 = pyrup_row(src + (size_t)yn * rs + c, X, w, cn);
-  if ((Y & 1) == 0) {
-    const int yp = (y > 0) ? y - 1 : 1;
-    const float r0 = pyrup_row(src + (size_t)yp * rs + c, X, w, cn);
-    return __fmul_rn(__fadd_rn(__fadd_rn(__fmul_rn(r1, 6.f), r0), r2), 0.015625f);
-  }
-  return __fmul_rn(__fmul_rn(__fadd_rn(r1, r2), 4.f), 0.015625f);
-}
 
 // pyrUp(flow) + the threshold loop of Flow::ComputeMask (:31-41): mask = 1, 0 where x*x + y*y >= thr (NaN -> 0)
 // The mask has the gray image's size H x W (2h <= H <= 2h + 1, same for W): pixels beyond flow2 keep the initial 1 (:25).
@@ -228,16 +200,6 @@ int dynm_element(const dynm_t* h, uint8_t* element /* 21 x 21 */) {
   if (!h || !element) { set_error("bad argument"); return B200ORB_EINVAL; }
   for (int i = 0; i < DYNM_K; ++i)
     for (int j = 0; j < DYNM_K; ++j) element[i * DYNM_K + j] = (j >= DYNM_R - h->tab.hw[i] && j <= DYNM_R + h->tab.hw[i]) ? 1 : 0;
-  return B200ORB_OK;
-}
-
-static int dynm_check_geometry(int rows, int cols, int mask_rows, int mask_cols) {
-  if (rows < 2 || cols < 2) { set_error("flow field smaller than 2x2"); return B200ORB_EINVAL; }
-  if (mask_rows < 2 * rows || mask_rows > 2 * rows + 1 || mask_cols < 2 * cols || mask_cols > 2 * cols + 1) {
-    set_error("mask %dx%d does not belong to a %dx%d flow field (the gray image is 2 rows (+1) x 2 cols (+1))", mask_cols,
-              mask_rows, cols, rows);
-    return B200ORB_EINVAL;
-  }
   return B200ORB_OK;
 }
 

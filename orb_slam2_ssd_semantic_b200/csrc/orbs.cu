@@ -4,6 +4,7 @@
 #include <memory>
 #include <new>
 
+#include "dynm_plane.cuh"
 #include "orbm_host.h"
 #include "orbx_host.h"
 
@@ -144,6 +145,14 @@ struct orbs {
   Event sel_ev, gather_ev;
   Event compute_done_ev;    // recorded after the last kernel of a host-buffer batch (before its downloads)
   orbs* chain_prev = nullptr;              // orbs_chain_after: the next batch's kernels wait for that handle's kernels
+  // Dynamic-mask block, reserved by the first masked call: the final bit plane and mask sum per frame, and the flow the
+  // host-buffer entries upload.
+  DeviceBlock dyn;
+  uint32_t* d_plane = nullptr;   // [maxF][rows][ceil(cols / 32)]
+  unsigned* d_msum = nullptr;    // [maxF]
+  float* d_flow = nullptr;       // [maxF][rows / 2][cols / 2][2]
+  bool masked = false;           // the running batch went through mask_filter
+  int mask_F = 0;                // frames of the last batch that carry a dynamic mask (0: it was not masked)
   bool have = false;
   int create_streams() {
     B200_CHECK(copy_stream.create());
@@ -159,6 +168,7 @@ struct orbs {
     B200_CHECK(ex->ensure_geometry(r, c, F));
     if (!(r == rows && c == cols && F <= maxF && ex->cap == cap)) {
       rows = 0;   // no geometry until its block exists
+      mask_F = 0;   // the dynamic masks of the last batch belong to the old geometry
       in_depth_bytes = -1;   // the host-input block is sized for the old geometry
       const int nF = std::max(F, ex->maxF), ncap = ex->cap;
       const size_t n = (size_t)nF * ncap;
@@ -179,6 +189,40 @@ struct orbs {
       }));
       in_depth_bytes = depth_bytes;
     }
+    return B200ORB_OK;
+  }
+  // Masked entries, before they touch any state: the flow field is at least 2 x 2 and both bit planes of a frame fit one
+  // CTA's shared memory (on an H100, 232448 bytes: rows * ceil(cols / 32) <= 29039, e.g. 1280 x 725).
+  int check_masked(int r, int c) const {
+    B200_CHECK(dynm_check_geometry(r / 2, c / 2, r, c));
+    int optin = 0;
+    B200_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    if (dynp_smem_bytes(r, c) > (size_t)optin) {
+      set_error("masked tracking of %dx%d images needs %zu bytes of shared memory per CTA (two bit planes of the mask); the "
+                "device allows %d: rows * ceil(cols / 32) must be at most %d", c, r, dynp_smem_bytes(r, c), optin,
+                (optin / 4 - 33) / 2);
+      return B200ORB_EINVAL;
+    }
+    return B200ORB_OK;
+  }
+  int ensure_dyn(bool host_flow) {
+    const size_t planes = (size_t)maxF * rows * dynp_words(cols), flow = host_flow ? (size_t)maxF * (rows / 2) * (cols / 2) * 2 : 0;
+    return dyn.reserve(ex->stream, [&](Carver& t) {
+      d_plane = t.take<uint32_t>(planes); d_msum = t.take<unsigned>(maxF); d_flow = t.take<float>(flow);
+    });
+  }
+  // Flow::ComputeMask + the masked Frame constructor's keypoint filter (perfect/src/Flow.cc:24-47, perfect/src/Frame.cc:
+  // 356-377) on the F frames the extractor has just run, in place; kpd16 (the CV_16U depth under the keypoints) moves with
+  // them.  dflow: [F][rows / 2][cols / 2][2] f32.
+  int mask_filter(const float* dflow, float thr, uint16_t* kpd16, int F) {
+    if (thr < 40.0f) thr = 40.0f;   // perfect/src/Flow.cc:24
+    const size_t smem = dynp_smem_bytes(rows, cols);
+    B200_CUDA(cudaFuncSetAttribute(k_dynm_plane_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_dynm_plane_filter<<<F, DYNP_THREADS, smem, ex->stream>>>(dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum,
+                                                               ex->d_kps, ex->d_desc, kpd16, ex->d_n, cap);
+    ++launches;
+    B200_CUDA(cudaGetLastError());
+    masked = true;
     return B200ORB_OK;
   }
   // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  Depth is the gathered CV_16U
@@ -215,6 +259,8 @@ struct orbs {
     }
     B200_CHECK(ex->prof_mark(ST_MATCH + 1));
     lastF = F;
+    mask_F = masked ? F : 0;
+    masked = false;
     have = true;
     return B200ORB_OK;
   }
@@ -293,12 +339,14 @@ static int orbs_after_select(void* ctx, int f0, int F) {
 
 static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, const uint16_t* depth16, float factor,
                             const float* Tcw, int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc,
-                            int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap, bool wait = true) {
+                            int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap, bool wait = true,
+                            const float* flow = nullptr, float thr = 0.f) {
   if (!h || !gray || (!depth && !depth16) || !Tcw || !kps || !desc || !nkp || !cur2last || !nmatch || nframes <= 0 ||
       rows <= 0 || cols <= 0) {
     set_error("bad argument");
     return B200ORB_EINVAL;
   }
+  if (flow) B200_CHECK(h->check_masked(rows, cols));
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
@@ -318,8 +366,9 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
   const char* depth_up = depth ? (const char*)depth : (const char*)depth16;
   B200_CHECK(h->ensure(rows, cols, nframes, depth_bytes));
   if (cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", cap, h->cap); return B200ORB_ECAP; }
+  if (flow) B200_CHECK(h->ensure_dyn(true));
   cudaStream_t st = h->ex->stream;
-  const size_t px = (size_t)rows * cols, F = nframes;
+  const size_t px = (size_t)rows * cols, F = nframes, fpx = (size_t)(rows / 2) * (cols / 2) * 2;
   // the inputs go up in chunks on a copy stream while the extractor already works on the chunks that have arrived
   // (PCIe and SMs overlap); everything after extraction runs on the whole batch.
   const int nchunk = (int)std::min<size_t>(MAX_CHUNKS, (F + h->chunk_frames - 1) / h->chunk_frames);   // >= 64-frame chunks keep each launch wide enough
@@ -340,6 +389,9 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
       if (depth_bytes)
         B200_CUDA(cudaMemcpyAsync((char*)h->d_depth + o, depth_up + o, px * (f1 - f0) * depth_bytes, cudaMemcpyHostToDevice,
                                   h->copy_stream));
+      if (flow)
+        B200_CUDA(cudaMemcpyAsync(h->d_flow + fpx * f0, flow + fpx * f0, fpx * (f1 - f0) * 4, cudaMemcpyHostToDevice,
+                                  h->copy_stream));
       B200_CUDA(cudaEventRecord(h->chunk_ev[c], h->copy_stream));
       B200_CUDA(cudaStreamWaitEvent(st, h->chunk_ev[c], 0));
       B200_CHECK(h->ex->run(h->d_gray + px * f0, cols, px, (int)(f1 - f0), (int)f0));
@@ -347,6 +399,7 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
   }
   h->ex->after_select = nullptr;
   if (depth16) B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
+  if (flow) B200_CHECK(h->mask_filter(h->d_flow, thr, depth16 ? h->d_kpd16 : nullptr, nframes));
   B200_CUDA(cudaMemcpyAsync(h->d_T, Tcw, F * 64, cudaMemcpyHostToDevice, st));
   B200_CHECK(h->run(depth ? static_cast<const float*>(h->d_depth) : nullptr, depth16 ? h->d_kpd16 : nullptr, factor, h->d_T,
                     nframes));
@@ -386,6 +439,59 @@ int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_
                           int32_t* cur2last, int32_t* nmatch, int cap) {
   return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
                           nmatch, cap, /*wait=*/false);
+}
+
+int orbs_track_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                                const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                                uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
+  if (!flow) { set_error("bad argument"); return B200ORB_EINVAL; }
+  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
+                          nmatch, cap, /*wait=*/true, flow, binary_threshold);
+}
+
+int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                                 const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                                 uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
+  if (!flow) { set_error("bad argument"); return B200ORB_EINVAL; }
+  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
+                          nmatch, cap, /*wait=*/false, flow, binary_threshold);
+}
+
+int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,
+                                   float binary_threshold, int nframes, int rows, int cols) {
+  if (!h || !d_gray || !d_depth || !d_Tcw || !d_flow || nframes <= 0 || rows <= 0 || cols <= 0) {
+    set_error("bad argument");
+    return B200ORB_EINVAL;
+  }
+  B200_CHECK(h->check_masked(rows, cols));
+  DeviceGuard g(h->device);
+  B200_CHECK(h->ensure(rows, cols, nframes, -1));
+  B200_CHECK(h->ensure_dyn(false));
+  B200_CHECK(h->ex->run(d_gray, cols, (size_t)rows * cols, nframes));
+  B200_CHECK(h->mask_filter(d_flow, binary_threshold, nullptr, nframes));
+  return h->run(d_depth, nullptr, 0.f, d_Tcw, nframes);
+}
+
+// The dynamic mask of frame `frame` of the last batch, if that batch was masked: FrameDrawer's mDynMask
+// (perfect/src/FrameDrawer.cc:262), unpacked to one byte per pixel, and whether the 65 % rule filtered the frame.
+int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered) {
+  if (!h || frame < 0 || frame >= h->mask_F) {
+    set_error(h && !h->mask_F ? "the last batch was not masked" : "bad argument");
+    return B200ORB_EINVAL;
+  }
+  DeviceGuard g(h->device);
+  const int rows = h->rows, cols = h->cols, nw = dynp_words(cols);
+  std::vector<uint32_t> words((size_t)rows * nw);
+  unsigned sum = 0;
+  cudaStream_t st = h->ex->stream;
+  B200_CUDA(cudaMemcpyAsync(words.data(), h->d_plane + (size_t)frame * rows * nw, words.size() * 4, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(&sum, h->d_msum + frame, 4, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  if (mask)
+    for (int y = 0; y < rows; ++y)
+      for (int x = 0; x < cols; ++x) mask[(size_t)y * cols + x] = (words[(size_t)y * nw + (x >> 5)] >> (x & 31)) & 1u;
+  if (filtered) *filtered = (double)sum > (double)(rows * cols) * 0.65;
+  return B200ORB_OK;
 }
 
 // frames per upload chunk of the host-buffer entries (default 128; at most MAX_CHUNKS per call): smaller chunks start the

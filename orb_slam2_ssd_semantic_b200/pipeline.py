@@ -86,6 +86,66 @@ class StreamTracker:
                                                  F, rows, cols, ptr(kps), ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
         return out
 
+    @staticmethod
+    def _check_flow(flow: np.ndarray, F: int, rows: int, cols: int):
+        if flow.shape != (F, rows // 2, cols // 2, 2):
+            raise ValueError("flow must be [nframes][rows/2][cols/2][2] float32, got %s" % (flow.shape,))
+
+    def track_batch_u16_masked(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                               flow: np.ndarray, binary_threshold: float = 40.0, out=None):
+        """The `perfect` variant's masked frames (perfect/src/Tracking.cc:703-719): like track_batch_u16, with the dynamic
+        mask of each frame computed on the device from its half-resolution optical flow (flow[n][rows/2][cols/2][2],
+        calcOpticalFlowFarneback's output; a zero field for a frame without a predecessor) and the keypoints outside the
+        mask dropped before tracking.  The outputs describe the filtered frames; dynamic_mask(frame) returns the masks."""
+        gray = np.ascontiguousarray(gray, np.uint8)
+        depth_u16 = np.ascontiguousarray(depth_u16, np.uint16)
+        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
+        flow = np.ascontiguousarray(flow, np.float32)
+        F, rows, cols = gray.shape
+        assert depth_u16.shape == gray.shape and Tcw.shape[0] == F
+        self._check_flow(flow, F, rows, cols)
+        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
+        _lib.check(self._L.orbs_track_batch_u16_masked(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
+                                                       ptr(Tcw), ptr(flow), float(binary_threshold), F, rows, cols, ptr(kps),
+                                                       ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
+        return kps, desc, nkp, c2l, nm
+
+    def submit_batch_u16_masked(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                                flow: np.ndarray, binary_threshold: float, out):
+        """Asynchronous track_batch_u16_masked (as submit_batch_u16): every input, the flow included, must be page-locked,
+        C-contiguous and untouched until sync()."""
+        for a, dt in ((gray, np.uint8), (depth_u16, np.uint16), (Tcw, np.float32), (flow, np.float32)):
+            if a.dtype != dt or not a.flags.c_contiguous:
+                raise ValueError("submit_batch_u16_masked takes C-contiguous %s arrays (no hidden copies)" % np.dtype(dt).name)
+        F, rows, cols = gray.shape
+        assert depth_u16.shape == gray.shape and Tcw.size == F * 16
+        self._check_flow(flow, F, rows, cols)
+        kps, desc, nkp, c2l, nm = out
+        _lib.check(self._L.orbs_submit_batch_u16_masked(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
+                                                        ptr(Tcw), ptr(flow), float(binary_threshold), F, rows, cols, ptr(kps),
+                                                        ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
+        return out
+
+    def track_batch_masked_device(self, d_gray: int, d_depth: int, d_Tcw: int, d_flow: int, binary_threshold: float,
+                                  nframes: int, rows: int, cols: int):
+        """track_batch_device with the dynamic mask; d_flow = [nframes][rows/2][cols/2][2] f32 in HBM. Asynchronous."""
+        _lib.check(self._L.orbs_track_batch_masked_device(self._h, C.c_void_p(d_gray), C.c_void_p(d_depth), C.c_void_p(d_Tcw),
+                                                          C.c_void_p(d_flow), float(binary_threshold), nframes, rows, cols))
+
+    def dynamic_mask(self, frame: int):
+        """-> (mask rows x cols uint8 0 / 1, filtered) of `frame` of the last batch, which must have been masked:
+        FrameDrawer's mDynMask and whether the 65 % rule dropped keypoints of that frame."""
+        rows, cols = self._mask_shape()
+        mask = np.zeros((rows, cols), np.uint8)
+        filtered = C.c_int(0)
+        _lib.check(self._L.orbs_read_dynamic_mask(self._h, int(frame), ptr(mask), C.byref(filtered)))
+        return mask, bool(filtered.value)
+
+    def _mask_shape(self):
+        r, c = C.c_int(0), C.c_int(0)
+        _lib.check(self._L.orbx_level_dims(self._L.orbs_extractor(self._h), 0, C.byref(r), C.byref(c)))
+        return r.value, c.value
+
     def set_chunk_frames(self, frames: int):
         """Frames per upload chunk of the host-buffer calls (default 128)."""
         _lib.check(self._L.orbs_set_chunk_frames(self._h, int(frames)))
