@@ -18,7 +18,8 @@ dis = subprocess.run(["nvdisasm", "-c", os.path.join(tmp, cubin)], capture_outpu
 kernels = [("k_fast_cells<48>", "k_fast_cellsILi48E"), ("k_orient_desc", "k_orient_descENS"),
            ("k_quadtree", "10k_quadtreeENS"), ("k_match_last_fused", "k_match_last_fused"),
            ("k_blur7_strip", "k_blur7_strip"), ("k_resize_g", "k_resize_g"), ("k_ocm_scan_keys", "k_ocm_scan_keys"),
-           ("k_ocm_bin", "k_ocm_binE"), ("k_dynm_morph<true>", "k_dynm_morphILb1"), ("k_dynm_flow_mask", "k_dynm_flow_mask")]
+           ("k_ocm_bin", "k_ocm_binE"), ("k_dynm_plane_filter", "k_dynm_plane_filter"),
+           ("k_dynm_erode<true>", "k_dynm_erodeILb1")]
 out = ["# SASS of libb200orb.so (sm_90a): `cuobjdump -xelf all` + `nvdisasm -c` of the library built from this tree by",
        "# csrc/Makefile (nvcc 12.9, -O3 --fmad=false -lineinfo).  Static instruction counts and opcode mix per hot kernel, excerpts."]
 tot = collections.Counter()
