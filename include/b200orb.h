@@ -504,6 +504,35 @@ int ocm_nccl_comm_destroy(void* nccl_comm);
  * survived gates + leaf filter, summed over the round's keyframes); voxel_updates = CUMULATIVE number of (voxel, keyframe)
  * log-odds updates since the map was created (U summed over every keyframe so far). */
 int ocm_last_batch_stats(ocm_t* h, int64_t* points, int64_t* voxel_updates);
+/* The map as octomap's pruned ColorOcTree, and back (`.ot` files: what octovis reads, what MapDrawer saves and loads).
+ *   ocm_tree_build   InsertScan's m_octree->prune() (perfect/src/MapDrawer.cc:1024) and the walk of the tree's write():
+ *                    builds, in device memory of the handle, the pruned tree of the map as it stands after everything
+ *                    enqueued so far -- the 8-byte nodes octomap writes, in pre-order (inner value = max child, inner
+ *                    colour white, 8 equal childless children collapse into their parent, cascading) -- and its leaves.
+ *                    The tree is a snapshot: the three readers below return the last build until the next one.
+ *   ocm_write_ot     the file's bytes, header (`id ColorOcTree`, `size` = nodes, `res` as an ostream prints a double) and
+ *                    nodes; buf == NULL: *n = size only.  An empty map writes the header with `size 0`.
+ *   ocm_tree_leaves  the pruned leaves in file order: key of the min corner (3 x u16), depth (16 = one cell; a leaf of
+ *                    depth d covers (2^(16-d))^3 cells), log-odds, colour -- the cells MapDrawer::DrawOctoMap walks
+ *                    (:406-416).  Any output may be NULL; all NULL: *n only.
+ *   ocm_save_ot      MapDrawer::SaveOctoMap (:1103-1111): ocm_tree_build + ocm_write_ot into `path`; *n_nodes (NULL = skip).
+ *   ocm_read_ot      MapDrawer::LoadOctoMap (:1113-1117), from memory: REPLACES the map's contents by the file's leaves,
+ *                    pruned leaves expanded to their depth-16 cells, inner nodes ignored.  Afterwards the handle is a map
+ *                    that was just merged: inserts, ocm_merge_nccl, ocm_query and ocm_export_leaves continue from it.
+ *                    Refused with the map untouched: an id other than ColorOcTree, a `res` other than the handle's,
+ *                    a `size` that disagrees with the bytes or the child masks, a tree deeper than 16 (B200ORB_EINVAL);
+ *                    more cells than the map's capacity (B200ORB_ECAP).
+ *   ocm_load_ot      the same from a file.
+ *   ocm_ot_leaves    the parser alone, on the host (no handle, no GPU): the leaves of `.ot` bytes in file order, as
+ *                    ocm_tree_leaves returns them.  cap too small: B200ORB_ECAP, *n_out = leaves; nothing else written. */
+int ocm_tree_build(ocm_t* h, int64_t* n_nodes, int64_t* n_leaves);
+int ocm_write_ot(ocm_t* h, uint8_t* buf, int64_t cap, int64_t* n);
+int ocm_tree_leaves(ocm_t* h, uint16_t* keys, uint8_t* depth, float* logodds, uint8_t* rgb, int64_t cap, int64_t* n);
+int ocm_save_ot(ocm_t* h, const char* path, int64_t* n_nodes);
+int ocm_read_ot(ocm_t* h, const uint8_t* bytes, int64_t n);
+int ocm_load_ot(ocm_t* h, const char* path);
+int ocm_ot_leaves(const uint8_t* bytes, int64_t n, double* res, uint16_t* keys, uint8_t* depth, float* logodds,
+                  uint8_t* rgb, int64_t cap, int64_t* n_out);
 int ocm_sync(ocm_t* h);
 void* ocm_stream(ocm_t* h);
 long long ocm_launch_count(const ocm_t* h);

@@ -37,6 +37,7 @@ EXPORTS = [
     "ocm_last_points", "ocm_num_leaves", "ocm_export_leaves", "ocm_query", "ocm_sync", "ocm_stream", "ocm_launch_count",
     "ocm_insert_keyframes_labeled_device", "ocm_insert_keyframes_u16_labeled", "ocm_merge_nccl", "ocm_nccl_unique_id",
     "ocm_nccl_comm_create", "ocm_nccl_comm_destroy", "ocm_last_batch_stats",
+    "ocm_tree_build", "ocm_write_ot", "ocm_tree_leaves", "ocm_save_ot", "ocm_read_ot", "ocm_load_ot", "ocm_ot_leaves",
     "dynm_create", "dynm_destroy", "dynm_launch_count", "dynm_stream", "dynm_sync", "dynm_element", "dynm_mask_from_flow",
     "dynm_mask_from_flow_batch_device", "dynm_filter_keypoints", "dynm_filter_keypoints_batch_device",
 ]
@@ -170,6 +171,14 @@ def lib() -> C.CDLL:
     L.ocm_num_leaves.restype = C.c_int64
     L.ocm_export_leaves.argtypes = [vp, vp, vp, vp, C.c_int64, C.POINTER(C.c_int64)]
     L.ocm_query.argtypes = [vp, vp, C.POINTER(f), C.POINTER(i)]
+    i64p = C.POINTER(C.c_int64)
+    L.ocm_tree_build.argtypes = [vp, i64p, i64p]
+    L.ocm_write_ot.argtypes = [vp, vp, C.c_int64, i64p]
+    L.ocm_tree_leaves.argtypes = [vp, vp, vp, vp, vp, C.c_int64, i64p]
+    L.ocm_save_ot.argtypes = [vp, C.c_char_p, i64p]
+    L.ocm_read_ot.argtypes = [vp, vp, C.c_int64]
+    L.ocm_load_ot.argtypes = [vp, C.c_char_p]
+    L.ocm_ot_leaves.argtypes = [vp, C.c_int64, C.POINTER(C.c_double), vp, vp, vp, vp, C.c_int64, i64p]
     L.ocm_sync.argtypes = [vp]
     L.ocm_stream.argtypes = [vp]
     L.ocm_stream.restype = vp

@@ -14,6 +14,8 @@
 //                word = keyframe j of the running batch observed the voxel occupied / free.  The scan of ALL keyframes
 //                of a batch only ORs bits (order-free, one launch); one more launch replays each touched voxel's bits in
 //                keyframe order, which reproduces the sequential clamped updates exactly.
+//   tree         on demand (ocm_tree_build, ocm_tree.cuh): the map as octomap's pruned ColorOcTree, 8-byte nodes in
+//                pre-order plus the pruned leaves -- what an `.ot` file holds; ocm_read_ot goes the other way.
 #include <algorithm>
 #include <memory>
 #include <new>
@@ -582,6 +584,8 @@ __global__ void k_depth_u16_to_f32(const ushort4* __restrict__ src, float4* __re
 
 }  // namespace b200
 
+#include "ocm_tree.cuh"
+
 using namespace b200;
 
 struct ocm {
@@ -627,6 +631,12 @@ struct ocm {
   HostBlock mg_counts_h;
   DeviceBlock mg;
   Event mg_ev[2];                     // orders the merge after the caller's stream, and the caller's stream after it
+  // ocm_tree_build: per-cell workspace, and the tree of the last build (tree_nodes < 0: none yet)
+  DeviceBlock tree_ws, tree_res;
+  TreeWork tw{};
+  TreeOut tree{};
+  long long tree_nodes = -1, tree_leaves = 0;
+  DeviceBlock load;                   // ocm_read_ot's leaves
 
   // Every array 256-byte aligned by the Carver (k_ocm_apply reads bm in 16-byte words).
   void take_block(Carver& c) {
@@ -652,6 +662,10 @@ struct ocm {
     return insert_batch(1, &dd, &drgb, &dlabel, r, c, Tcw, fx, fy, cx, cy);
   }
   int check_err();
+  int clear_map();
+  int scan(unsigned long long* data, int n);
+  int build_tree();
+  int read_ot(const uint8_t* bytes, int64_t n);
 };
 
 static long long pow2_at_least(long long v) {
@@ -706,6 +720,15 @@ int ocm::check_err() {
               e == ERR_LEAF_TABLE_FULL ? "VoxelGrid table full" : "map full (raise OcmParams.map_capacity)");
     return B200ORB_ECAP;
   }
+  return B200ORB_OK;
+}
+
+// The empty map: no voxel, every clamp-add summary at the identity, no batch mask, the handle's device words zero.
+int ocm::clear_map() {
+  const long long C = map_cap;
+  B200_CUDA(cudaMemsetAsync(block.p, 0, block.bytes, stream));
+  fill(map.keys, EMPTY_KEY, C); fill(map.lo, -INFINITY, C); fill(map.hi, INFINITY, C);
+  B200_CUDA(cudaMemsetAsync(map.rgb, 0xff, 4 * C, stream));
   return B200ORB_OK;
 }
 
@@ -790,6 +813,124 @@ int ocm::insert_batch(int n, const float* const* dd, const uint8_t* const* drgb,
   return B200ORB_OK;
 }
 
+// Exclusive scan of n 64-bit words in place; the total lands in tw.total.
+int ocm::scan(unsigned long long* data, int n) {
+  const int tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
+  k_ocm_tree_scan_tiles<<<tiles, SCAN_THREADS, 0, stream>>>(data, n, tw.sums);
+  k_ocm_tree_scan_sums<<<1, SCAN_THREADS, 0, stream>>>(tw.sums, tiles, tw.total);
+  k_ocm_tree_scan_apply<<<tiles, SCAN_THREADS, 0, stream>>>(data, n, tw.sums);
+  launches += 3;
+  B200_CUDA(cudaGetLastError());
+  return B200ORB_OK;
+}
+
+// Hash -> pruned tree (ocm_tree.cuh), on the map's stream after everything enqueued there.  The host reads two counts,
+// the cells and then the nodes and leaves, to size the buffers; no cell and no node passes through it.
+int ocm::build_tree() {
+  tree_nodes = -1;
+  int n = 0;
+  B200_CUDA(cudaMemcpyAsync(&n, map.nleaves, 4, cudaMemcpyDeviceToHost, stream));
+  B200_CUDA(cudaStreamSynchronize(stream));
+  B200_CHECK(check_err());   // a map that overflowed is not written
+  if (n == 0) { tree_nodes = tree_leaves = 0; return B200ORB_OK; }
+  size_t sort_bytes = 0;
+  B200_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr,
+                                            (unsigned long long*)nullptr, (const unsigned*)nullptr, (unsigned*)nullptr, n, 0,
+                                            48, (cudaStream_t)stream));
+  B200_CHECK(tree_ws.reserve(stream, [&](Carver& t) {
+    tw.code_in = t.take<unsigned long long>(n); tw.code = t.take<unsigned long long>(n);
+    tw.slot_in = t.take<unsigned>(n); tw.slot = t.take<unsigned>(n);
+    tw.val = t.take<float>(n); tw.rgb = t.take<unsigned>(n);
+    tw.run = t.take<unsigned long long>(n); tw.off = t.take<unsigned long long>(n);
+    tw.lcp = t.take<signed char>(n); tw.top = t.take<signed char>(n);
+    tw.sums = t.take<unsigned long long>((n + SCAN_TILE - 1) / SCAN_TILE); tw.total = t.take<unsigned long long>(1);
+    tw.count = t.take<int>(1); tw.sort_tmp = t.take<char>(sort_bytes);
+  }));
+  const unsigned cells = (unsigned)((n + 255) / 256);
+  B200_CUDA(cudaMemsetAsync(tw.count, 0, 4, stream));
+  k_ocm_tree_gather<<<(unsigned)((map_cap + 255) / 256), 256, 0, stream>>>(map, n, tw.code_in, tw.slot_in, tw.count);
+  B200_CUDA(cub::DeviceRadixSort::SortPairs(tw.sort_tmp, sort_bytes, (const unsigned long long*)tw.code_in, tw.code,
+                                            (const unsigned*)tw.slot_in, tw.slot, n, 0, 48, (cudaStream_t)stream));
+  k_ocm_tree_cells<<<cells, 256, 0, stream>>>(map, n, tw.slot, tw.val, tw.rgb, tw.run);
+  launches += 2;
+  B200_CHECK(scan(tw.run, n));
+  k_ocm_tree_classify<<<cells, 256, 0, stream>>>(n, tw.code, tw.run, tw.lcp, tw.top, tw.off);
+  ++launches;
+  B200_CHECK(scan(tw.off, n));
+  unsigned long long total = 0;
+  B200_CUDA(cudaMemcpyAsync(&total, tw.total, 8, cudaMemcpyDeviceToHost, stream));
+  B200_CUDA(cudaStreamSynchronize(stream));
+  const long long nn = (long long)(total & 0xffffffffull), nl = (long long)(total >> 32);
+  B200_CHECK(tree_res.reserve(stream, [&](Carver& t) {
+    tree.nodes = t.take<uint2>(nn); tree.keys = t.take<unsigned short>(3 * nl); tree.depth = t.take<unsigned char>(nl);
+    tree.val = t.take<float>(nl); tree.rgb = t.take<unsigned char>(3 * nl);
+  }));
+  k_ocm_tree_leaves<<<cells, 256, 0, stream>>>(n, tw.code, tw.val, tw.rgb, tw.lcp, tw.top, tw.off, tree);
+  for (int d = 15; d >= 0; --d)
+    k_ocm_tree_inner<<<cells, 256, 0, stream>>>(n, d, tw.code, tw.val, tw.lcp, tw.top, tw.off, tree.nodes);
+  launches += 17;
+  B200_CUDA(cudaGetLastError());
+  tree_nodes = nn; tree_leaves = nl;
+  return B200ORB_OK;
+}
+
+// Replace the map by the leaves of an `.ot` file.  Everything that can be refused is refused before the table is touched.
+int ocm::read_ot(const uint8_t* bytes, int64_t n) {
+  double res = 0;
+  std::vector<OtLeaf> leaves;
+  B200_CHECK(parse_ot(bytes, n, &res, &leaves));
+  char mine[32];
+  snprintf(mine, sizeof(mine), "%g", prm.resolution);   // the resolution as a file carries it
+  if (res != strtod(mine, nullptr)) {
+    set_error(".ot: res %g, this map has %s", res, mine);
+    return B200ORB_EINVAL;
+  }
+  const size_t nl = leaves.size();
+  std::vector<long long> first(nl + 1, 0);
+  for (size_t i = 0; i < nl; ++i) {
+    first[i + 1] = first[i] + (1ll << (3 * (16 - leaves[i].depth)));
+    if (first[i + 1] > map_cap) {
+      set_error(".ot: more than %lld cells, the map holds %lld (raise OcmParams.map_capacity)", first[i], map_cap);
+      return B200ORB_ECAP;
+    }
+  }
+  unsigned long long* key = nullptr;
+  float* val = nullptr;
+  unsigned* rgb = nullptr;
+  unsigned char* depth = nullptr;
+  long long* d_first = nullptr;
+  B200_CHECK(load.reserve(stream, [&](Carver& t) {
+    key = t.take<unsigned long long>(nl); d_first = t.take<long long>(nl); val = t.take<float>(nl);
+    rgb = t.take<unsigned>(nl); depth = t.take<unsigned char>(nl);
+  }));
+  B200_CHECK(clear_map());
+  if (nl > 0) {
+    std::vector<unsigned long long> hk(nl);
+    std::vector<float> hv(nl);
+    std::vector<unsigned> hc(nl);
+    std::vector<unsigned char> hd(nl);
+    for (size_t i = 0; i < nl; ++i) {
+      const OtLeaf& l = leaves[i];
+      hk[i] = (unsigned long long)l.key[0] | (unsigned long long)l.key[1] << 16 | (unsigned long long)l.key[2] << 32;
+      hv[i] = l.val;
+      hc[i] = (unsigned)l.rgb[0] | (unsigned)l.rgb[1] << 8 | (unsigned)l.rgb[2] << 16;
+      hd[i] = l.depth;
+    }
+    B200_CUDA(cudaMemcpyAsync(key, hk.data(), 8 * nl, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(d_first, first.data(), 8 * nl, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(val, hv.data(), 4 * nl, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(rgb, hc.data(), 4 * nl, cudaMemcpyHostToDevice, stream));
+    B200_CUDA(cudaMemcpyAsync(depth, hd.data(), nl, cudaMemcpyHostToDevice, stream));
+    const long long cells = first[nl];
+    k_ocm_tree_expand<<<(unsigned)((cells + 255) / 256), 256, 0, stream>>>(map, (int)nl, cells, key, depth, val, rgb, d_first,
+                                                                          d_err);
+    ++launches;
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaStreamSynchronize(stream));   // the staging vectors go out of scope
+  }
+  return check_err();
+}
+
 extern "C" {
 
 void ocm_default_params(OcmParams* p) {
@@ -825,12 +966,9 @@ int ocm_create(const OcmParams* p, int device, ocm_t** out) {
   B200_CHECK(h->stream.create(hi_p));
   for (Event& e : h->job_ev) B200_CHECK(e.create());
   for (Event& e : h->mg_ev) B200_CHECK(e.create());
-  const long long C = h->map_cap;
-  h->map.mask = C - 1;
+  h->map.mask = h->map_cap - 1;
   B200_CHECK(h->block.carve(h->stream, [&](Carver& t) { h->take_block(t); }));
-  B200_CUDA(cudaMemsetAsync(h->block.p, 0, h->block.bytes, h->stream));
-  h->fill(h->map.keys, EMPTY_KEY, C); h->fill(h->map.lo, -INFINITY, C); h->fill(h->map.hi, INFINITY, C);
-  B200_CUDA(cudaMemsetAsync(h->map.rgb, 0xff, 4 * C, h->stream));
+  B200_CHECK(h->clear_map());
   B200_CUDA(cudaStreamSynchronize(h->stream));
   *out = h.release();
   return B200ORB_OK;
@@ -1137,6 +1275,112 @@ int ocm_last_batch_stats(ocm_t* h, int64_t* points, int64_t* voxels_touched) {
   for (int j = 0; j <= h->last_slot && j < ocm::MAX_SLOTS; ++j) p += c[4 * j + 1];
   if (points) *points = p;
   if (voxels_touched) *voxels_touched = (int64_t)nt;
+  return B200ORB_OK;
+}
+
+int ocm_tree_build(ocm_t* h, int64_t* n_nodes, int64_t* n_leaves) {
+  if (!h) { set_error("null argument"); return B200ORB_EINVAL; }
+  DeviceGuard g(h->device);
+  B200_CHECK(h->build_tree());
+  if (n_nodes) *n_nodes = h->tree_nodes;
+  if (n_leaves) *n_leaves = h->tree_leaves;
+  return B200ORB_OK;
+}
+
+int ocm_write_ot(ocm_t* h, uint8_t* buf, int64_t cap, int64_t* n) {
+  if (!h || (buf && cap < 0)) { set_error("bad argument"); return B200ORB_EINVAL; }
+  if (h->tree_nodes < 0) { set_error("no tree: call ocm_tree_build first"); return B200ORB_EINVAL; }
+  const std::string hdr = ot_header(h->tree_nodes, h->prm.resolution);
+  const int64_t need = (int64_t)hdr.size() + 8 * h->tree_nodes;
+  if (n) *n = need;
+  if (!buf) return B200ORB_OK;
+  if (cap < need) { set_error(".ot buffer of %lld bytes < %lld", (long long)cap, (long long)need); return B200ORB_ECAP; }
+  DeviceGuard g(h->device);
+  memcpy(buf, hdr.data(), hdr.size());
+  if (h->tree_nodes > 0) {
+    B200_CUDA(cudaMemcpyAsync(buf + hdr.size(), h->tree.nodes, 8 * h->tree_nodes, cudaMemcpyDeviceToHost, h->stream));
+    B200_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return B200ORB_OK;
+}
+
+int ocm_tree_leaves(ocm_t* h, uint16_t* keys, uint8_t* depth, float* logodds, uint8_t* rgb, int64_t cap, int64_t* n) {
+  if (!h || cap < 0) { set_error("bad argument"); return B200ORB_EINVAL; }
+  if (h->tree_nodes < 0) { set_error("no tree: call ocm_tree_build first"); return B200ORB_EINVAL; }
+  const long long nl = h->tree_leaves;
+  if (n) *n = nl;
+  if (!keys && !depth && !logodds && !rgb) return B200ORB_OK;
+  if (cap < nl) { set_error("cap %lld < %lld pruned leaves", (long long)cap, nl); return B200ORB_ECAP; }
+  if (nl == 0) return B200ORB_OK;
+  DeviceGuard g(h->device);
+  if (keys) B200_CUDA(cudaMemcpyAsync(keys, h->tree.keys, 6 * nl, cudaMemcpyDeviceToHost, h->stream));
+  if (depth) B200_CUDA(cudaMemcpyAsync(depth, h->tree.depth, nl, cudaMemcpyDeviceToHost, h->stream));
+  if (logodds) B200_CUDA(cudaMemcpyAsync(logodds, h->tree.val, 4 * nl, cudaMemcpyDeviceToHost, h->stream));
+  if (rgb) B200_CUDA(cudaMemcpyAsync(rgb, h->tree.rgb, 3 * nl, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200ORB_OK;
+}
+
+int ocm_save_ot(ocm_t* h, const char* path, int64_t* n_nodes) {
+  if (!h || !path) { set_error("null argument"); return B200ORB_EINVAL; }
+  B200_CHECK(ocm_tree_build(h, n_nodes, nullptr));
+  int64_t bytes = 0;
+  B200_CHECK(ocm_write_ot(h, nullptr, 0, &bytes));
+  std::vector<uint8_t> buf((size_t)bytes);
+  B200_CHECK(ocm_write_ot(h, buf.data(), bytes, nullptr));
+  FILE* f = fopen(path, "wb");
+  const bool ok = f && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
+  if ((f && fclose(f) != 0) || !ok) { set_error("cannot write %s", path); return B200ORB_EINVAL; }
+  return B200ORB_OK;
+}
+
+int ocm_read_ot(ocm_t* h, const uint8_t* bytes, int64_t n) {
+  if (!h || n < 0 || (!bytes && n > 0)) { set_error("bad argument"); return B200ORB_EINVAL; }
+  DeviceGuard g(h->device);
+  return h->read_ot(bytes, n);
+}
+
+// a whole file; false (with the error set) when it cannot be read
+static bool read_file(const char* path, std::vector<uint8_t>* out) {
+  FILE* f = fopen(path, "rb");
+  if (!f) { set_error("cannot open %s", path); return false; }
+  uint8_t chunk[1 << 16];
+  size_t got;
+  while ((got = fread(chunk, 1, sizeof(chunk), f)) > 0) out->insert(out->end(), chunk, chunk + got);
+  const bool ok = !ferror(f);
+  fclose(f);
+  if (!ok) set_error("cannot read %s", path);
+  return ok;
+}
+
+int ocm_load_ot(ocm_t* h, const char* path) {
+  if (!h || !path) { set_error("null argument"); return B200ORB_EINVAL; }
+  std::vector<uint8_t> bytes;
+  if (!read_file(path, &bytes)) return B200ORB_EINVAL;
+  return ocm_read_ot(h, bytes.data(), (int64_t)bytes.size());
+}
+
+int ocm_ot_leaves(const uint8_t* bytes, int64_t n, double* res, uint16_t* keys, uint8_t* depth, float* logodds, uint8_t* rgb,
+                  int64_t cap, int64_t* n_out) {
+  if (n < 0 || (!bytes && n > 0) || cap < 0) { set_error("bad argument"); return B200ORB_EINVAL; }
+  double r = 0;
+  std::vector<OtLeaf> leaves;
+  B200_CHECK(parse_ot(bytes, n, &r, &leaves));
+  const int64_t nl = (int64_t)leaves.size();
+  if ((keys || depth || logodds || rgb) && cap < nl) {
+    if (n_out) *n_out = nl;
+    set_error("cap %lld < %lld leaves", (long long)cap, (long long)nl);
+    return B200ORB_ECAP;
+  }
+  if (n_out) *n_out = nl;
+  if (res) *res = r;
+  for (int64_t i = 0; i < nl; ++i) {
+    const OtLeaf& l = leaves[i];
+    if (keys) memcpy(keys + 3 * i, l.key, 6);
+    if (depth) depth[i] = l.depth;
+    if (logodds) logodds[i] = l.val;
+    if (rgb) memcpy(rgb + 3 * i, l.rgb, 3);
+  }
   return B200ORB_OK;
 }
 

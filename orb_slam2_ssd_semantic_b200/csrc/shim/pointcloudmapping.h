@@ -60,6 +60,17 @@ class PointCloudMapping {
       lastKeyframeSize = N - 1;
     }
   }
+  // MapDrawer::SaveOctoMap / LoadOctoMap (perfect/src/MapDrawer.cc:1103-1117): the map as a pruned ColorOcTree `.ot`
+  // file.  Loading replaces the map, as the reference replaces m_octree; keyframes inserted afterwards continue from it.
+  void SaveOctoMap(const char* filename) {
+    if (ocm_save_ot(h_, filename, nullptr) != B200ORB_OK)
+      throw std::runtime_error(std::string("PointCloudMapping(B200): ") + b200orb_last_error());
+  }
+  void LoadOctoMap() { LoadOctoMap("octomap.ot"); }   // the reference's fixed name (:1115)
+  void LoadOctoMap(const std::string& filename) {
+    if (ocm_load_ot(h_, filename.c_str()) != B200ORB_OK)
+      throw std::runtime_error(std::string("PointCloudMapping(B200): ") + b200orb_last_error());
+  }
   void shutdown() { ocm_sync(h_); }     // src/pointcloudmapping.cc:104-113 joins the viewer thread
   void update() {}                      // T variant's map refresh hook: nothing to do, the map lives in HBM
   long long numLeaves() { return (long long)ocm_num_leaves(h_); }

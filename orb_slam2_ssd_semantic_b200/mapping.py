@@ -4,6 +4,7 @@ insertKeyFrame() pushes one RGB-D keyframe through MapDrawer::GeneratePointCloud
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -149,10 +150,46 @@ class PointCloudMapping:
         return (v.value if f.value else None)
 
     def SaveOctoMap(self, name: str):
-        """MapDrawer::SaveOctoMap (perfect/src/MapDrawer.cc:1103-1111): writes a pruned ColorOcTree `.ot` file
-        (octovis-readable) from the GPU leaf map.  Returns (leaves, nodes)."""
-        from . import octree_io
-        return octree_io.save_octomap(self, name)
+        """MapDrawer::SaveOctoMap (perfect/src/MapDrawer.cc:1103-1111): writes the map as a pruned ColorOcTree `.ot` file
+        (octovis-readable), the tree built on the device (ocm_save_ot).  Returns (depth-16 cells in the map, nodes)."""
+        nodes = C.c_int64(0)
+        _lib.check(self._L.ocm_save_ot(self._h, os.fsencode(name), C.byref(nodes)))
+        return self.num_leaves(), nodes.value
+
+    def LoadOctoMap(self, name: str = "octomap.ot"):
+        """MapDrawer::LoadOctoMap (:1113-1117): replaces the map by the leaves of an `.ot` file; inserts and merges
+        continue from it."""
+        _lib.check(self._L.ocm_load_ot(self._h, os.fsencode(name)))
+
+    def read_ot(self, data: bytes):
+        """LoadOctoMap from the bytes of an `.ot` file."""
+        buf = np.frombuffer(data, np.uint8)
+        _lib.check(self._L.ocm_read_ot(self._h, ptr(buf) if len(buf) else None, len(buf)))
+
+    def tree_build(self):
+        """ocm_tree_build: the pruned ColorOcTree of the map as it stands, kept on the device.  -> (nodes, leaves)."""
+        nn, nl = C.c_int64(0), C.c_int64(0)
+        _lib.check(self._L.ocm_tree_build(self._h, C.byref(nn), C.byref(nl)))
+        return nn.value, nl.value
+
+    def write_ot(self) -> bytes:
+        """The `.ot` bytes of the last tree_build()."""
+        n = C.c_int64(0)
+        _lib.check(self._L.ocm_write_ot(self._h, None, 0, C.byref(n)))
+        buf = np.zeros(n.value, np.uint8)
+        _lib.check(self._L.ocm_write_ot(self._h, ptr(buf), n.value, C.byref(n)))
+        return buf.tobytes()
+
+    def tree_leaves(self):
+        """The pruned leaves of the last tree_build() in file order -> (keys[n,3] u16 of the min corner, depth[n] u8,
+        log-odds[n], rgb[n,3])."""
+        n = C.c_int64(0)
+        _lib.check(self._L.ocm_tree_leaves(self._h, None, None, None, None, 0, C.byref(n)))
+        m = max(n.value, 1)
+        keys, depth = np.zeros((m, 3), np.uint16), np.zeros(m, np.uint8)
+        lo, rgb = np.zeros(m, np.float32), np.zeros((m, 3), np.uint8)
+        _lib.check(self._L.ocm_tree_leaves(self._h, ptr(keys), ptr(depth), ptr(lo), ptr(rgb), n.value, C.byref(n)))
+        return keys[:n.value], depth[:n.value], lo[:n.value], rgb[:n.value]
 
     def sync(self):
         _lib.check(self._L.ocm_sync(self._h))
