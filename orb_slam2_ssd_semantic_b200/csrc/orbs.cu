@@ -379,8 +379,14 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
     B200_CUDA(cudaEventRecord(h->inputs_free_ev, st));
     B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->inputs_free_ev, 0));
     // orbs_chain_after: this batch's kernels start when the other handle's kernels are done -- the uploads enqueued
-    // below (copy stream) and that handle's downloads run meanwhile, and kernels of two batches never share the SMs
-    if (h->chain_prev) B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
+    // below (copy stream) and that handle's downloads run meanwhile, and kernels of two batches never share the SMs.
+    // The uploads start only once that handle's in-place depth reads (k_depth_prefetch) are done: both cross the host
+    // link toward the device, the reads are latency-bound and its matcher waits for them, while these uploads are
+    // needed only when this batch's kernels start.
+    if (h->chain_prev) {
+      B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
+      B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->chain_prev->gather_ev, 0));
+    }
     h->chain_prev = nullptr;
     for (int c = 0; c < nchunk; ++c) {
       const size_t f0 = F * c / nchunk, f1 = F * (c + 1) / nchunk;
@@ -503,7 +509,7 @@ int orbs_set_chunk_frames(orbs_t* h, int frames) {
 }
 
 // The next host-buffer batch submitted to `h` starts its kernels only when the kernels of `prev`'s last submitted batch
-// are done (its uploads are not held back).  Two handles submitted alternately with this form a 3-stage pipeline:
+// are done, and its uploads only when `prev`'s in-place depth reads are done.  Two handles submitted alternately with this form a 3-stage pipeline:
 // upload of batch k+1 | kernels of batch k | download of batch k-1.
 int orbs_chain_after(orbs_t* h, orbs_t* prev) {
   if (!h || !prev || h == prev || h->device != prev->device) { set_error("bad argument"); return B200ORB_EINVAL; }

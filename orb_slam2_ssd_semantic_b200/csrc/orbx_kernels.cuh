@@ -354,6 +354,7 @@ __global__ void __launch_bounds__(FAST_THREADS, 4) k_fast_cells(PyrView pyr, con
 //     (:752-759) is an atomicMax over (response << 24 | ~index).
 // ---------------------------------------------------------------------------------------------------
 constexpr int QT_THREADS = 512;
+constexpr int QT_WARPS = QT_THREADS / 32;
 constexpr int QT_UNTOUCHED = 0x40000000;   // flag in QtSmem::cpos: the node keeps its box this round
 
 struct QtScratchView {
@@ -361,19 +362,31 @@ struct QtScratchView {
   int* qnode;       // [F][slots_per_frame] list index of each candidate's node
 };
 
-struct QtSmem {   // carved from dynamic shared memory, cap entries each
-  short4* box[2];
-  int* cnt[2];
-  int* cc;        // [cap][4] child counts (per quadrant) of every node of the current list
-  int* cc2;       // [cap][4] the same for the list being built (filled while the keypoints are re-homed)
-  int* cpos;      // [cap][4] new list index of each child
-  int* rk;        // processing rank or -1
-  int* npos;      // new list index of untouched nodes
-  int* byrank;    // node index by processing rank
-  int* pre;       // inclusive prefix of child counts by rank
+// Dynamic shared memory, cap entries per array.  Every array sits at an offset from the one base that depends on cap
+// only: a table of array pointers picked at run time would live in local memory.  The list read in a round has parity
+// `cur`, the list built from it `cur ^ 1`; box, cnt and the child populations cc are double-buffered by that parity.
+struct QtSmem {
+  unsigned char* base;
+  int cap;
+  __device__ short4* box(int par) const { return (short4*)base + par * cap; }
+  // [cap][4] keypoints per quadrant of every node: the child populations, counted while the keypoints are re-homed
+  __device__ int* cc(int par) const { return (int*)(base + 16 * cap) + par * 4 * cap; }
+  __device__ int* cpos() const { return (int*)(base + 48 * cap); }   // [cap][4] new list index of each child
+  // the largest-first rank's sort keys, two per entry, over cpos (written only after the sort)
+  __device__ unsigned long long* key() const { return (unsigned long long*)(base + 48 * cap); }
+  __device__ int* cnt(int par) const { return (int*)(base + 64 * cap) + par * cap; }
+  __device__ int* rk() const { return (int*)(base + 72 * cap); }       // processing rank or -1 (largest-first)
+  __device__ int* npos() const { return (int*)(base + 76 * cap); }     // new list index of untouched nodes
+  __device__ int* byrank() const { return (int*)(base + 80 * cap); }   // node index by processing rank
+  __device__ int* pre() const { return (int*)(base + 84 * cap); }      // inclusive prefix of child counts by rank
 };
 
 __host__ __device__ inline size_t qt_smem_bytes(int cap) { return (size_t)cap * (2 * 8 + 2 * 4 + 16 + 16 + 16 + 4 * 4); }
+
+// orbx.cu refuses qt_smem_bytes(qt_cap) > 100 KiB, so a list never holds more nodes than this.  A sweep round's scan
+// sums (candidate flag | non-empty children << 16) over the list: both fields must stay below their 16 bits.
+constexpr int QT_CAP_MAX = 100 * 1024 / 88;
+static_assert(QT_CAP_MAX < (1 << 16) && 4 * QT_CAP_MAX < (1 << 15), "quad-tree scan fields overflow");
 
 __device__ __forceinline__ int qt_quadrant(short4 b, unsigned kp) {
   // DivideNode's assignment (:509-523); node boxes are relative to (minBorderX, minBorderY) = (16,16)
@@ -395,14 +408,28 @@ __device__ __forceinline__ void qt_count(int* ctr, int idx, bool active) {
   }
 }
 
-// in-place exclusive scan of a[0..n) (shared memory); returns the total. All threads must call.
+// Exclusive scan of one int per thread across the CTA with a single barrier: every warp scans the QT_WARPS warp totals
+// itself.  Returns the exclusive prefix; *total = CTA sum.  All threads must call, and a barrier must separate this
+// call from the last read of `ws` (>= QT_WARPS ints) by the scan before it.
+__device__ __forceinline__ int qt_block_scan(int v, int* ws, int* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int inc = warp_incl_scan(v, lane);
+  if (lane == 31) ws[wid] = inc;
+  __syncthreads();
+  const int w = (lane < QT_WARPS) ? ws[lane] : 0;
+  const int winc = warp_incl_scan(w, lane);
+  *total = __shfl_sync(0xffffffffu, winc, 31);
+  return __shfl_sync(0xffffffffu, winc - w, wid) + inc - v;
+}
+
+// in-place exclusive scan of a[0..n) (shared memory); returns the total. All threads must call; ends with a barrier.
 __device__ int qt_scan_array(int* a, int n, int* ws) {
   const int per = (n + QT_THREADS - 1) / QT_THREADS;   // launch contract: blockDim.x == QT_THREADS (a shift, not a division)
   const int beg = min(n, (int)threadIdx.x * per), end = min(n, beg + per);
   int s = 0;
   for (int i = beg; i < end; ++i) s += a[i];
   int total;
-  int run = block_excl_scan(s, ws, &total);
+  int run = qt_block_scan(s, ws, &total);
   for (int i = beg; i < end; ++i) {
     const int v = a[i];
     a[i] = run;
@@ -412,12 +439,62 @@ __device__ int qt_scan_array(int* a, int n, int* ws) {
   return total;
 }
 
-// Register budget: 4 CTAs per SM (the compiler's own choice is 52 registers on sm_90a, i.e. 2 CTAs per SM; the cap
-// spills a little).  The kernel is latency-bound (barriers + L2 round trips per round), so resident CTAs are what hides
-// it.  Measured on an H100 SXM (80 GB HBM3, 400 W power limit), per 96-frame batch of 2000 features alone the stage
-// takes 0.34 ms at 2 CTAs per SM and 0.42 / 0.47 ms capped for 3 / 4.  But in bench.py, with two batches and the mapper
-// in flight, 2 CTAs per SM gave 46.7 k `value` / 38.4-40.2 k `e2e` frames/s against 44.5-44.6 k / 41.4-41.8 k for 4
-// (3: 45.0-45.1 k / 40.9-41.3 k): 4 is the one budget that slows neither number.
+__device__ __forceinline__ int qt_nonempty(const int* c) { return (c[0] > 0) + (c[1] > 0) + (c[2] > 0) + (c[3] > 0); }
+
+// A node holding cnt keypoints with child populations c[0..3], as one scan value: candidate flag | non-empty children << 16
+__device__ __forceinline__ int qt_split(int cnt, const int* c) { return cnt > 1 ? 1 | (qt_nonempty(c) << 16) : 0; }
+
+// DivideNode (:478-534) of node i of the list of parity cur: its non-empty children n4, n3, n2, n1 take positions
+// p, p+1, ... of the list being built.  Returns how many of them hold more than one keypoint.
+__device__ __forceinline__ int qt_divide(const QtSmem& S, int cur, int i, int p) {
+  const short4 b = S.box(cur)[i];
+  const int* c = S.cc(cur) + i * 4;
+  const int mx = b.x + ((b.z - b.x + 1) >> 1), my = b.y + ((b.w - b.y + 1) >> 1);
+  int exp = 0;
+#pragma unroll
+  for (int q = 3; q >= 0; --q) {
+    const int cq = c[q];
+    if (cq > 0) {
+      S.cpos()[i * 4 + q] = p;
+      short4 nb;
+      nb.x = (q & 1) ? mx : b.x;
+      nb.z = (q & 1) ? b.z : mx;
+      nb.y = (q & 2) ? my : b.y;
+      nb.w = (q & 2) ? b.w : my;
+      S.box(cur ^ 1)[p] = nb;
+      S.cnt(cur ^ 1)[p] = cq;
+      exp += (cq > 1);
+      ++p;
+    }
+  }
+  return exp;
+}
+
+// Bitonic sort of key[0..P) into descending order, P a power of two.  All threads must call; ends with a barrier.
+__device__ void qt_sort_desc(unsigned long long* key, int P) {
+  for (int k = 2; k <= P; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+#pragma unroll 1
+      for (int q = threadIdx.x; q < (P >> 1); q += QT_THREADS) {
+        const int i = ((q & ~(j - 1)) << 1) | (q & (j - 1)), l = i | j;   // the pair (i, i + j) of this stage
+        const unsigned long long a = key[i], b = key[l];
+        if (((i & k) == 0) == (a < b)) {   // descending where bit k of i is clear, ascending where it is set
+          key[i] = b;
+          key[l] = a;
+        }
+      }
+      __syncthreads();
+    }
+}
+
+// Register budget: 4 CTAs per SM, 32 registers on sm_90a and no stack frame (at a budget of 2 CTAs per SM the compiler
+// takes 46 registers, at 3 it takes 39).  A sweep round costs three barriers (its one scan, and one on each side of the
+// re-homing pass), and the budget hardly moves the stage any more.  Measured in bench.py on an H100 SXM (80 GB HBM3,
+// 700 W power limit), back to back: the stage takes 7.77 / 7.24 / 7.32-7.41 ms per 4240-frame step at 2 / 3 / 4 CTAs per
+// SM (one run each for 2 and 3, three for 4), `value` 52.9 k / 53.9 k / 53.7-54.0 k and `e2e` 37.3 k / 35.6 k /
+// 34.5-36.4 k frames/s, all before chained batches ordered their uploads after the other batch's depth reads (orbs.cu):
+// the slower stage at 2 CTAs per SM had started those reads later.  With that ordering, 4 CTAs per SM keeps `e2e` at the
+// previous kernel's level (34.6-35.4 k against 34.2-35.0 k, alternated), so the budget stays where it was.
 constexpr int QT_MIN_CTAS = 4;
 __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab lt, const CellDesc* __restrict__ cells,
                                                             const unsigned* __restrict__ cand,
@@ -432,21 +509,7 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
   const int l = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, nthr = blockDim.x;
   const int nlev = lt.nlevels;
   const int N = lt.nfeat[l];
-  QtSmem S;
-  {
-    unsigned char* p = smem_raw;
-    S.box[0] = (short4*)p; p += (size_t)qt_cap * 8;
-    S.box[1] = (short4*)p; p += (size_t)qt_cap * 8;
-    S.cnt[0] = (int*)p; p += (size_t)qt_cap * 4;
-    S.cnt[1] = (int*)p; p += (size_t)qt_cap * 4;
-    S.cc = (int*)p; p += (size_t)qt_cap * 16;
-    S.cc2 = (int*)p; p += (size_t)qt_cap * 16;
-    S.cpos = (int*)p; p += (size_t)qt_cap * 16;
-    S.rk = (int*)p; p += (size_t)qt_cap * 4;
-    S.npos = (int*)p; p += (size_t)qt_cap * 4;
-    S.byrank = (int*)p; p += (size_t)qt_cap * 4;
-    S.pre = (int*)p;
-  }
+  const QtSmem S{smem_raw, qt_cap};
   const unsigned* fcand = cand + (size_t)f * slots_per_frame;
   const int* fcnt = cellcnt + (size_t)f * ncells;
   // Per-candidate arrays (packed keypoint + node id) stay in the L2-resident global scratch: staging them in shared
@@ -485,7 +548,7 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
   const float hX = lt.hx[l];
   const int boxH = lt.box_h[l];
   int cur = 0;
-  int* icnt = S.cc;   // nIni counters
+  int* icnt = S.cc(1);   // nIni counters
   for (int i = tid; i < nIni; i += nthr) icnt[i] = 0;
   __syncthreads();
   for (int k = tid; k < K; k += nthr) {
@@ -496,143 +559,131 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
     atomicAdd(&icnt[ii], 1);
   }
   __syncthreads();
-  for (int i = tid; i < nIni; i += nthr) S.npos[i] = (icnt[i] > 0) ? 1 : 0;
+  for (int i = tid; i < nIni; i += nthr) S.npos()[i] = (icnt[i] > 0) ? 1 : 0;
   __syncthreads();
-  int n = qt_scan_array(S.npos, nIni, ws);
+  int n = qt_scan_array(S.npos(), nIni, ws);
   for (int i = tid; i < nIni; i += nthr) {
     if (icnt[i] > 0) {
-      const int p = S.npos[i];
-      S.box[0][p] = make_short4((short)(int)__fmul_rn(hX, (float)i), 0, (short)(int)__fmul_rn(hX, (float)(i + 1)),
+      const int p = S.npos()[i];
+      S.box(0)[p] = make_short4((short)(int)__fmul_rn(hX, (float)i), 0, (short)(int)__fmul_rn(hX, (float)(i + 1)),
                                 (short)boxH);
-      S.cnt[0][p] = icnt[i];
+      S.cnt(0)[p] = icnt[i];
     }
   }
-  for (int i = tid; i < nIni * 4; i += nthr) S.cc2[i] = 0;
+  for (int i = tid; i < nIni * 4; i += nthr) S.cc(0)[i] = 0;
   __syncthreads();
   // compact the node ids and count, per node, the keypoints of each quadrant (the child populations of round 0)
   for (int k = tid; k < K; k += nthr) {
-    const int p = S.npos[qnode[k]];
+    const int p = S.npos()[qnode[k]];
     qnode[k] = p;
-    atomicAdd(&S.cc2[p * 4 + qt_quadrant(S.box[0][p], qkp[k])], 1);
+    atomicAdd(&S.cc(0)[p * 4 + qt_quadrant(S.box(0)[p], qkp[k])], 1);
   }
   __syncthreads();
-  { int* t = S.cc; S.cc = S.cc2; S.cc2 = t; }   // S.cc aliased icnt until here
 
   // ---- rounds -------------------------------------------------------------------------------------------
-  bool largest = false, finish = false;
-  while (!finish) {
-    const int prevSize = n;
-    short4* box = S.box[cur];
-    int* cnt = S.cnt[cur];
-    short4* nbox = S.box[cur ^ 1];
-    int* ncnt = S.cnt[cur ^ 1];
-    // (1) processing rank of every node holding more than one keypoint
-    int m;   // number of candidates
+  // A thread owns the contiguous list range [beg, end) in the round's scan and in the sweep's writes.  The loops over
+  // that range and the sort's pair loop stay rolled: unrolled, they push the per-round state out of the 32 registers.
+  for (bool largest = false;;) {
+    const short4* box = S.box(cur);
+    const int* cnt = S.cnt(cur);
+    const int* cc = S.cc(cur);
+    if (tid == 0) s_expand = 0;   // last read before the previous round's final barrier
+    // (1) one scan of (candidate flag | non-empty children << 16) over the list.  The child populations cc were counted
+    //     while the keypoints were re-homed last round.
+    const int per = (n + QT_THREADS - 1) / QT_THREADS;
+    const int beg = min(n, tid * per), end = min(n, beg + per);
+    int run = 0;
+    for (int i = beg; i < end; ++i) run += qt_split(cnt[i], cc + i * 4);
+    int tot;
+    run = qt_block_scan(run, ws, &tot);
+    const int m = tot & 0xffff;   // candidates: nodes holding more than one keypoint
+    int TC, nUn, myexp = 0;       // children created this round, nodes left untouched
     if (!largest) {
-      for (int i = tid; i < n; i += nthr) S.rk[i] = (cnt[i] > 1) ? 1 : 0;
-      __syncthreads();
-      m = qt_scan_array(S.rk, n, ws);
-      for (int i = tid; i < n; i += nthr) {
-        if (cnt[i] > 1) S.byrank[S.rk[i]] = i;
-        else S.rk[i] = -1;
+      // (2) sweep round (:608-667): every candidate splits, in list order, so node i's exclusive sums place it.  Its
+      //     rank is the number of candidates before it; children of rank r fill [TC - pre[r], TC - pre[r-1]) with pre the
+      //     inclusive prefix of non-empty children; an untouched node keeps its order behind all TC children.
+      TC = tot >> 16;
+      nUn = n - m;
+#pragma unroll 1
+      for (int i = beg; i < end; ++i) {
+        const int v = qt_split(cnt[i], cc + i * 4);
+        if (v) {
+          myexp += qt_divide(S, cur, i, TC - (run >> 16) - (v >> 16));
+        } else {
+          const int p = TC + i - (run & 0xffff);
+          S.box(cur ^ 1)[p] = box[i];
+          S.cnt(cur ^ 1)[p] = cnt[i];
+          int* cp = S.cpos() + i * 4;
+          cp[0] = cp[1] = cp[2] = cp[3] = p | QT_UNTOUCHED;
+        }
+        run += v;
       }
     } else {
-      for (int i = tid; i < n; i += nthr) S.npos[i] = (cnt[i] > 1) ? 1 : 0;
-      __syncthreads();
-      m = qt_scan_array(S.npos, n, ws);   // only the total is needed
-      for (int i = tid; i < n; i += nthr) {
-        const int ci = cnt[i];
-        if (ci > 1) {
-          int r = 0;
-          for (int j = 0; j < n; ++j) {
-            const int cj = cnt[j];
-            r += (cj > ci) || (cj == ci && j < i);   // (size desc, list index asc); cj>ci>1 implies candidate
-          }
-          S.rk[i] = r;
-          S.byrank[r] = i;
-        } else {
-          S.rk[i] = -1;
-        }
+      // (2) largest-first round (:678-739): candidates in (size desc, list index asc) order, i.e. the 64-bit keys
+      //     size << 32 | ~index sorted descending; the scan's flag prefix is each candidate's slot in the key array.
+      unsigned long long* key = S.key();
+      for (int i = beg; i < end; ++i) {
+        const int v = qt_split(cnt[i], cc + i * 4);
+        if (v) key[run & 0xffff] = ((unsigned long long)cnt[i] << 32) | (unsigned)~i;
+        else S.rk()[i] = -1;
+        run += v;
       }
-    }
-    __syncthreads();
-    // (2) the child populations S.cc[node][quadrant] were counted while the keypoints were re-homed last round
-    // (3) inclusive prefix over processing order of the number of non-empty children
-    for (int r = tid; r < m; r += nthr) {
-      const int* c = &S.cc[S.byrank[r] * 4];
-      S.pre[r] = (c[0] > 0) + (c[1] > 0) + (c[2] > 0) + (c[3] > 0);
-    }
-    if (tid == 0) { s_rstar = m - 1; s_expand = 0; }
-    __syncthreads();
-    {
-      const int tot = qt_scan_array(S.pre, m, ws);   // exclusive in place ...
-      (void)tot;
-      for (int r = tid; r < m; r += nthr) {          // ... turn into inclusive
-        const int* c = &S.cc[S.byrank[r] * 4];
-        S.pre[r] += (c[0] > 0) + (c[1] > 0) + (c[2] > 0) + (c[3] > 0);
-      }
+      const int P = (m > 1) ? 1 << (32 - __clz(m - 1)) : m;   // m rounded up to a power of two, <= 2 * cap keys
+      for (int r = m + tid; r < P; r += nthr) key[r] = 0;      // below every candidate's key
       __syncthreads();
-    }
-    if (largest) {   // :732 stop right after the split that reaches N
+      qt_sort_desc(key, P);
       for (int r = tid; r < m; r += nthr) {
-        const bool now = (n + S.pre[r] - (r + 1)) >= N;
-        const bool before = (r > 0) && ((n + S.pre[r - 1] - r) >= N);
+        const int i = ~(unsigned)key[r];
+        S.rk()[i] = r;
+        S.byrank()[r] = i;
+        S.pre()[r] = qt_nonempty(cc + i * 4);
+      }
+      if (tid == 0) s_rstar = m - 1;
+      __syncthreads();
+      // inclusive prefix over processing order of the number of non-empty children
+      qt_scan_array(S.pre(), m, ws);   // exclusive in place ...
+      for (int r = tid; r < m; r += nthr) S.pre()[r] += qt_nonempty(cc + S.byrank()[r] * 4);   // ... inclusive
+      __syncthreads();
+      // :732 stop right after the split that reaches N
+      for (int r = tid; r < m; r += nthr) {
+        const bool now = (n + S.pre()[r] - (r + 1)) >= N;
+        const bool before = (r > 0) && ((n + S.pre()[r - 1] - r) >= N);
         if (now && !before) s_rstar = r;
       }
       __syncthreads();
-    }
-    const int rstar = s_rstar;
-    const int TC = (m > 0) ? S.pre[rstar] : 0;   // children created this round
-    // (4) new list index of untouched nodes
-    for (int i = tid; i < n; i += nthr) {
-      const int r = S.rk[i];
-      S.npos[i] = (r < 0 || r > rstar) ? 1 : 0;
-    }
-    __syncthreads();
-    const int nUn = qt_scan_array(S.npos, n, ws);
-    for (int i = tid; i < n; i += nthr) {
-      const int r = S.rk[i];
-      if (r < 0 || r > rstar) {
-        const int p = TC + S.npos[i];
-        S.npos[i] = p;
-        nbox[p] = box[i];
-        ncnt[p] = cnt[i];
-        S.rk[i] = -1;
-        S.cpos[i * 4 + 0] = S.cpos[i * 4 + 1] = S.cpos[i * 4 + 2] = S.cpos[i * 4 + 3] = p | QT_UNTOUCHED;
+      const int rstar = s_rstar;
+      TC = (m > 0) ? S.pre()[rstar] : 0;
+      // new list index of untouched nodes
+      for (int i = tid; i < n; i += nthr) {
+        const int r = S.rk()[i];
+        S.npos()[i] = (r < 0 || r > rstar) ? 1 : 0;
       }
-    }
-    // (5) children: block of rank r starts at TC - pre[r]; inside the block n4,n3,n2,n1 (non-empty only)
-    int myexp = 0;
-    for (int r = tid; r <= rstar && r < m; r += nthr) {
-      const int i = S.byrank[r];
-      const short4 b = box[i];
-      const int* c = &S.cc[i * 4];
-      const int mx = b.x + ((b.z - b.x + 1) >> 1), my = b.y + ((b.w - b.y + 1) >> 1);
-      int p = TC - S.pre[r];
-#pragma unroll
-      for (int q = 3; q >= 0; --q) {
-        if (c[q] > 0) {
-          S.cpos[i * 4 + q] = p;
-          short4 nb;
-          nb.x = (q & 1) ? mx : b.x;
-          nb.z = (q & 1) ? b.z : mx;
-          nb.y = (q & 2) ? my : b.y;
-          nb.w = (q & 2) ? b.w : my;
-          nbox[p] = nb;
-          ncnt[p] = c[q];
-          myexp += (c[q] > 1);
-          ++p;
+      __syncthreads();
+      nUn = qt_scan_array(S.npos(), n, ws);
+      for (int i = tid; i < n; i += nthr) {
+        const int r = S.rk()[i];
+        if (r < 0 || r > rstar) {
+          const int p = TC + S.npos()[i];
+          S.box(cur ^ 1)[p] = box[i];
+          S.cnt(cur ^ 1)[p] = cnt[i];
+          int* cp = S.cpos() + i * 4;
+          cp[0] = cp[1] = cp[2] = cp[3] = p | QT_UNTOUCHED;
         }
       }
+      // children: block of rank r starts at TC - pre[r]
+      for (int r = tid; r <= rstar && r < m; r += nthr) myexp += qt_divide(S, cur, S.byrank()[r], TC - S.pre()[r]);
     }
     if (myexp) atomicAdd(&s_expand, myexp);
-    for (int i = tid; i < (TC + nUn) * 4; i += nthr) S.cc2[i] = 0;
+    int* ncc = S.cc(cur ^ 1);
+    for (int i = tid; i < (TC + nUn) * 4; i += nthr) ncc[i] = 0;
     __syncthreads();
-    // (6) re-home the keypoints; the same pass counts the quadrant populations inside the NEW nodes, i.e. the child
+    const int nToExpand = s_expand;
+    // (3) re-home the keypoints; the same pass counts the quadrant populations inside the NEW nodes, i.e. the child
     //     populations the next round needs (one pass over the keypoints per round instead of two)
     // cpos[p][q] holds the new list index for quadrant q of node p -- for untouched nodes the node's own new index in
     // all four entries, flagged -- so the loop needs no branch on the node state and one box load: the child's box, and
     // with it the quadrant the keypoint will fall into NEXT round, follows from the parent's box and q.
+    const int* cpos = S.cpos();
     for (int k = tid; k < K; k += nthr) {
       const int p = qnode[k];
       const unsigned kp = qkp[k];
@@ -641,7 +692,7 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
       const int mx = b.x + ((b.z - b.x + 1) >> 1), my = b.y + ((b.w - b.y + 1) >> 1);
       const int qx = (x < mx) ? 0 : 1, qy = (y < my) ? 0 : 1;
       const int q = qx | (qy << 1);
-      const int v = S.cpos[p * 4 + q];
+      const int v = cpos[p * 4 + q];
       const int np = v & 0x3fffffff;
       int q2 = q;
       if (!(v & QT_UNTOUCHED)) {   // the node was split: quadrant inside child q (DivideNode :478-534 of the child)
@@ -650,20 +701,19 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
         q2 = ((x < cmx) ? 0 : 1) | ((y < cmy) ? 0 : 2);
       }
       qnode[k] = np;
-      atomicAdd(&S.cc2[np * 4 + q2], 1);
+      atomicAdd(&ncc[np * 4 + q2], 1);
     }
-    { int* t = S.cc; S.cc = S.cc2; S.cc2 = t; }
+    const bool grew = (TC + nUn != n);
     n = TC + nUn;
-    const int nToExpand = s_expand;
     cur ^= 1;
-    // (7) termination logic (:671-675, :736-737)
-    if (n >= N || n == prevSize) finish = true;
-    else if (!largest && (n + nToExpand * 3) > N) largest = true;
     __syncthreads();
+    // (4) termination logic (:671-675, :736-737)
+    if (n >= N || !grew) break;
+    if ((n + nToExpand * 3) > N) largest = true;
   }
 
   // ---- best keypoint of every node (:746-762), output in list order --------------------------------------
-  unsigned* best = (unsigned*)S.cc;
+  unsigned* best = (unsigned*)S.cc(cur);
   for (int i = tid; i < n; i += nthr) best[i] = 0;
   __syncthreads();
   for (int k = tid; k < K; k += nthr)
