@@ -92,6 +92,16 @@ int orbx::init(const OrbxParams& p, int dev) {
   B200_CHECK(stream.create());
   for (v = 1; v <= HALF_PATCH_SIZE; ++v)   // k_orient_desc tests the circular mask as v <= vmax(|u|)
     if (otab.umax[v] > otab.umax[v - 1]) { set_error("umax table is not non-increasing"); return B200ORB_EINVAL; }
+  // k_orient_desc reads the descriptor's tests from a tile of reach OD_BR.  A point (px, py) lands at
+  // round(px*cos - py*sin), round(px*sin + py*cos): both terms are at most |(px, py)| in magnitude, up to the relative
+  // error of glibc's cosf / sinf and of three rounded float ops (< 1e-6; 2^-16 leaves room), so the rounded offset is
+  // at most floor(|(px, py)| * (1 + 2^-16) + 0.5) at every angle.  ORB's pattern: 18, from (-13, -13) at 45 degrees.
+  int reach = 0;
+  for (int i = 0; i < 512; ++i) {
+    const double r = std::hypot((double)kPatternHost[2 * i], (double)kPatternHost[2 * i + 1]);
+    reach = std::max(reach, (int)std::floor(r * (1.0 + 1.0 / 65536) + 0.5));
+  }
+  if (reach > OD_BR) { set_error("descriptor pattern reaches %d px, beyond the %d-px patch tile", reach, OD_BR); return B200ORB_EINVAL; }
   float pat[1024];
   for (int i = 0; i < 1024; ++i) pat[i] = (float)kPatternHost[i];
   B200_CHECK(patf.carve(stream, [&](Carver& t) { d_patf = t.take<float4>(256); }));
@@ -195,6 +205,13 @@ int orbx::ensure_geometry(int r, int c, int F) {
         cd.pad = 0;
         cd.slot_off = slots;
         if (cd.rw > FAST_MAX_ROI - 2 || cd.rh > FAST_MAX_ROI) { set_error("FAST cell larger than %d px", FAST_MAX_ROI); return B200ORB_EGEOM; }
+        // k_orient_desc's patch tiles reach EDGE_THRESHOLD px around a keypoint: the detection range [x0+3, x0+rw-3)
+        // x [y0+3, y0+rh-3) must keep that far from every side of the level
+        if (cd.x0 + 3 < EDGE_THRESHOLD || cd.y0 + 3 < EDGE_THRESHOLD || cd.x0 + cd.rw - 4 + EDGE_THRESHOLD > lw[l] - 1 ||
+            cd.y0 + cd.rh - 4 + EDGE_THRESHOLD > lh[l] - 1) {
+          set_error("FAST cell of level %d reaches within %d px of its side", l, EDGE_THRESHOLD);
+          return B200ORB_EGEOM;
+        }
         const int iw = cd.rw - 6, ih = cd.rh - 6;
         if (iw > 0 && ih > 0) slots += ((iw + 1) / 2) * ((ih + 1) / 2);
         cells.push_back(cd);
