@@ -572,7 +572,9 @@ __global__ void __launch_bounds__(32) k_resolve_generic(CurView cv, QueriesView 
   if (lane == 0) nmatch[p] = n_acc - pruned;
 }
 
-// K9 (POINTS): best and second best among unclaimed candidates, level-aware ratio test (:98-152)
+// K9 (POINTS): best and second best among unclaimed candidates, level-aware ratio test (:98-152).  The reference's
+// `dist < bestDist` / `dist < bestDist2` chain starts both at 256, so a candidate at distance 256 is never recorded:
+// it must not become the runner-up, whose level decides whether the ratio test applies at all.
 __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, QueriesView qv, MatchCam cam, ListView in, int* f2pt,
                                                        int* nmatch, int cmax) {
   extern __shared__ __align__(16) unsigned char rsm[];
@@ -593,7 +595,9 @@ __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, QueriesView q
     if (cn == 0) continue;
     int bestIdx = -1, bestDist = 256, bestDist2 = 256, bestLevel = -1, bestLevel2 = -1;
     if (cn > 0) {
-      const unsigned v0 = in.list[(size_t)i * LCAP + lane], v1 = in.list[(size_t)i * LCAP + lane + 32];
+      unsigned v0 = in.list[(size_t)i * LCAP + lane], v1 = in.list[(size_t)i * LCAP + lane + 32];
+      if ((v0 >> 20) >= 256u) v0 = KEY_INF;
+      if ((v1 >> 20) >= 256u) v1 = KEY_INF;
       const Pick p1 = pick_min(v0, v1, cn, taken, -1, lane);
       if (p1.idx >= 0) {
         bestIdx = p1.idx; bestDist = p1.dist; bestLevel = cv.oct[p1.idx];
@@ -607,7 +611,7 @@ __global__ void __launch_bounds__(32) k_resolve_points(CurView cv, QueriesView q
         const uint4 d0 = __ldg(reinterpret_cast<const uint4*>(d)), d1 = __ldg(reinterpret_cast<const uint4*>(d) + 1);
         unsigned long long b1 = ~0ull, b2 = ~0ull;   // two smallest keys per lane
         warp_walk(g, q, d0, d1, [&](int ord, int idx, int dist) {
-          if (!taken[idx]) {
+          if (!taken[idx] && dist < 256) {
             const unsigned long long k = key64(dist, ord, idx);
             if (k < b1) { b2 = b1; b1 = k; } else if (k < b2) b2 = k;
           }
