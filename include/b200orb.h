@@ -304,6 +304,63 @@ int orbv_transform(orbv_t* h, const uint8_t* desc, int n, int levelsup, uint32_t
                    uint32_t* node_id);
 
 /* ------------------------------------------------------------------------------------------------
+ * Key-frame database -- KeyFrameDatabase (src/KeyFrameDatabase.cc): the inverted file of add / erase / clear (:39-73) and
+ * the walk, the common-word counts and the L1 scores of DetectLoopCandidates (:76-139) and
+ * DetectRelocalizationCandidates (:199-253).  The covisibility accumulation and the 0.75f * bestAccScore filter that follow
+ * (:141-196, :255-308) read GetBestCovisibilityKeyFrames(10) of the caller's objects and stay with the caller
+ * (shim/KeyFrameDatabase.h).
+ *
+ * A slot is the caller's handle of one keyframe (0 <= slot < 2^24).  The database keeps per slot its BowVector (ascending
+ * word ids < n_words, L1-scoring weights) and a mirror of the six KeyFrame members the database writes (OrbvDbMembers).
+ *   orbv_db_add    KeyFrameDatabase::add (:39-45).  A slot added k times without an erase is in each of its lists k times
+ *                  and counted k times.  `members`: the keyframe's current values (NULL keeps the mirror; a slot never
+ *                  added before starts at zero).  A slot already in the database keeps the BowVector it was added with.
+ *   orbv_db_erase  KeyFrameDatabase::erase (:47-67) with the BowVector the slot was added with: removes the slot's earliest
+ *                  add from every list; a slot not in the database is left as it is (the reference's loops find nothing).
+ *   orbv_db_clear  KeyFrameDatabase::clear (:69-73): every list empty; the mirrors stay (they are the objects' members).
+ *   orbv_db_query  the walk and the scores of one query: kind ORBV_DB_RELOC (query_id = Frame::mnId) or ORBV_DB_LOOP
+ *                  (query_id = KeyFrame::mnId, connected = GetConnectedKeyFrames() as slots; unknown keyframes may be left
+ *                  out).  words / weights: the query's BowVector.  out[0 .. *n_appended) are lKFsSharingWords in list
+ *                  order (flag ORBV_DB_SCORED when words > minCommonWords: score = (float)TemplatedVocabulary::score);
+ *                  out[*n_appended .. *n_met) are the other slots the walk met.  Every record carries the slot's new
+ *                  query / words / score of `kind`; slots the walk did not meet are unchanged.  The loop filter si >=
+ *                  minScore is the caller's.  cap >= orbv_db_state's *n_live (else B200ORB_ECAP, nothing changes).
+ *   orbv_db_state  one slot's mirror and how many times it is in the database (NULL outputs are skipped; slot -1: only
+ *                  *n_live, the number of slots in the database).
+ * B200ORB_EINVAL: a word id >= n_words, word ids not strictly ascending, a slot out of range, an unknown slot for
+ * orbv_db_erase / orbv_db_state.  One host sync per query (the result copy).
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct orbv_db orbv_db_t;
+typedef struct {
+  uint64_t loop_query;   /* mnLoopQuery */
+  int32_t loop_words;    /* mnLoopWords */
+  float loop_score;      /* mLoopScore */
+  uint64_t reloc_query;  /* mnRelocQuery */
+  int32_t reloc_words;   /* mnRelocWords */
+  float reloc_score;     /* mRelocScore */
+} OrbvDbMembers;
+typedef struct {
+  int32_t slot;
+  int32_t words;         /* mnRelocWords / mnLoopWords after the walk */
+  uint64_t query;        /* mnRelocQuery / mnLoopQuery after the walk */
+  float score;           /* mRelocScore / mLoopScore after the query */
+  int32_t flags;         /* ORBV_DB_APPENDED | ORBV_DB_SCORED */
+} OrbvDbHit;
+#define ORBV_DB_RELOC 0
+#define ORBV_DB_LOOP 1
+#define ORBV_DB_APPENDED 1
+#define ORBV_DB_SCORED 2
+int orbv_db_create(int device, int n_words, orbv_db_t** out);
+void orbv_db_destroy(orbv_db_t* h);
+int orbv_db_add(orbv_db_t* h, int slot, const uint32_t* words, const double* weights, int n, const OrbvDbMembers* members);
+int orbv_db_erase(orbv_db_t* h, int slot);
+int orbv_db_clear(orbv_db_t* h);
+int orbv_db_query(orbv_db_t* h, int kind, uint64_t query_id, const uint32_t* words, const double* weights, int n,
+                  const int32_t* connected, int n_connected, OrbvDbHit* out, int cap, int* n_appended, int* n_met);
+int orbv_db_state(orbv_db_t* h, int slot, OrbvDbMembers* members, int* count, int* n_live);
+long long orbv_db_launch_count(const orbv_db_t* h);
+
+/* ------------------------------------------------------------------------------------------------
  * Dynamic-mask stages of the `perfect` variant (SURVEY 8(f4), the image-arithmetic parts):
  *   FlowSLAM::Flow::ComputeMask (perfect/include/Flow.h:24-27, perfect/src/Flow.cc:17-52) after the call of
  *   cv::calcOpticalFlowFarneback -- which stays on the host side: OpenCV's own float code -- i.e. pyrUp of the half-

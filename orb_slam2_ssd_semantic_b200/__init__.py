@@ -10,5 +10,6 @@ from .matcher import ORBmatcher, FrameView, LastView, TrackPointsView, BowView, 
 from .pipeline import StreamTracker  # noqa: F401
 from .mapping import GlobalCloudMapping, PointCloudMapping  # noqa: F401
 from .vocabulary import ORBVocabulary  # noqa: F401
+from .keyframedb import KeyFrameDatabase  # noqa: F401
 
 __all__ = ["ORBextractor", "KP_DTYPE", "B200OrbError", "lib", "library_path"]

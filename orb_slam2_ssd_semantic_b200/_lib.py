@@ -29,6 +29,8 @@ EXPORTS = [
     "orbx_profile_enable", "orbx_profile_read",
     "orbm_hamming", "orbm_create", "orbm_destroy", "orbm_launch_count", "orbm_search_by_projection_last",
     "orbm_search_by_projection_points", "orbm_search_by_bow", "orbm_search_by_bow_kf", "orbm_search_projected", "orbm_search_best", "orbm_search_for_initialization", "orbm_search_for_triangulation", "orbm_is_in_frustum", "orbm_undistort_keypoints", "orbv_create", "orbv_destroy", "orbv_num_words", "orbv_launch_count", "orbv_transform",
+    "orbv_db_create", "orbv_db_destroy", "orbv_db_add", "orbv_db_erase", "orbv_db_clear", "orbv_db_query", "orbv_db_state",
+    "orbv_db_launch_count",
     "orbs_create", "orbs_destroy", "orbs_track_batch", "orbs_track_batch_u16", "orbs_submit_batch_u16", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_track_batch_device", "orbs_device_results", "orbs_read_frame_glue", "orbs_sync",
     "orbs_track_batch_u16_masked", "orbs_submit_batch_u16_masked", "orbs_track_batch_masked_device", "orbs_read_dynamic_mask",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
@@ -106,6 +108,16 @@ def lib() -> C.CDLL:
     L.orbv_launch_count.argtypes = [vp]
     L.orbv_launch_count.restype = C.c_longlong
     L.orbv_transform.argtypes = [vp, vp, i, i, vp, vp, vp]
+    L.orbv_db_create.argtypes = [i, i, C.POINTER(vp)]
+    L.orbv_db_destroy.argtypes = [vp]
+    L.orbv_db_destroy.restype = None
+    L.orbv_db_add.argtypes = [vp, i, vp, vp, i, vp]
+    L.orbv_db_erase.argtypes = [vp, i]
+    L.orbv_db_clear.argtypes = [vp]
+    L.orbv_db_query.argtypes = [vp, i, C.c_uint64, vp, vp, i, vp, i, vp, i, C.POINTER(i), C.POINTER(i)]
+    L.orbv_db_state.argtypes = [vp, i, vp, C.POINTER(i), C.POINTER(i)]
+    L.orbv_db_launch_count.argtypes = [vp]
+    L.orbv_db_launch_count.restype = C.c_longlong
     L.dynm_create.argtypes = [i, C.POINTER(vp)]
     L.dynm_destroy.argtypes = [vp]
     L.dynm_destroy.restype = None

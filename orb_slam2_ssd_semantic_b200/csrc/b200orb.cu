@@ -6,3 +6,4 @@
 #include "gcm.cu"
 #include "orbv.cu"
 #include "dynm.cu"
+#include "orbv_db.cu"

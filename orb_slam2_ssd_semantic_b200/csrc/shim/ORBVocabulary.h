@@ -27,6 +27,7 @@ class ORBVocabulary : public DBoW2::TemplatedVocabulary<DBoW2::FORB::TDescriptor
       : Base(k, L, weighting, scoring) {}
   ~ORBVocabulary() { orbv_destroy(h_); }
   void InvalidateDevice() { orbv_destroy(h_); h_ = nullptr; }
+  DBoW2::ScoringType getScoringType() const { return m_scoring; }   // DBoW2's accessor (shim/KeyFrameDatabase.h reads it)
 
   using Base::transform;   // the single-feature overloads stay DBoW2's
   void transform(const std::vector<DBoW2::FORB::TDescriptor>& features, DBoW2::BowVector& v, DBoW2::FeatureVector& fv,
