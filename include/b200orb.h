@@ -159,6 +159,17 @@ typedef struct {
 int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono,
                                    float nnratio, int check_ori, int32_t* cur2last, int* nmatches);
 
+/* The perfect tree's overload SearchByProjection(Frame &CurrentFrame, const Frame &LastFrame, th, bMono,
+ * vector<cv::Point2f>& points_last, vector<cv::Point2f>& points_current) (perfect/src/ORBmatcher.cc:1727-1880):
+ * the same search, plus the claim list it pushes the 2-D point pairs from (:1835-1836, inside `bestDist<=TH_HIGH`,
+ * BEFORE the rotation prune).  last2cur_accepted[last.n]: the current keypoint bestIdx2 that query i accepted, or -1;
+ * a pair the prune later drops stays listed, and a current keypoint whose MapPoint has no observations can appear
+ * twice.  The caller builds the pairs (mvKeys[i].pt, mvKeys[j].pt) in ascending i.  cur2last and *nmatches are those of
+ * orbm_search_by_projection_last; same kernels, same results.  Host buffers. */
+int orbm_search_by_projection_last_pairs(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono,
+                                         float nnratio, int check_ori, int32_t* cur2last, int32_t* last2cur_accepted,
+                                         int* nmatches);
+
 /* Local-map search: ORBmatcher::SearchByProjection(Frame &F, const vector<MapPoint*>&, th)
  * (src/ORBmatcher.cc:63-156); the per-MapPoint fields are those Frame::isInFrustum fills (src/Frame.cc:387-451). */
 typedef struct {

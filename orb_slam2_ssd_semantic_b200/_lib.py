@@ -28,6 +28,7 @@ EXPORTS = [
     "orbx_get_level", "orbx_scale_tables", "orbx_candidates_per_level", "orbx_launch_count",
     "orbx_profile_enable", "orbx_profile_read",
     "orbm_hamming", "orbm_create", "orbm_destroy", "orbm_launch_count", "orbm_search_by_projection_last",
+    "orbm_search_by_projection_last_pairs",
     "orbm_search_by_projection_points", "orbm_search_by_bow", "orbm_search_by_bow_kf", "orbm_search_projected", "orbm_search_best", "orbm_search_for_initialization", "orbm_search_for_triangulation", "orbm_is_in_frustum", "orbm_undistort_keypoints", "orbv_create", "orbv_destroy", "orbv_num_words", "orbv_launch_count", "orbv_transform",
     "orbv_db_create", "orbv_db_destroy", "orbv_db_add", "orbv_db_erase", "orbv_db_clear", "orbv_db_query", "orbv_db_state",
     "orbv_db_launch_count",
@@ -90,6 +91,8 @@ def lib() -> C.CDLL:
     L.orbm_launch_count.restype = C.c_longlong
     L.orbm_search_by_projection_last.argtypes = [vp, C.POINTER(OrbmFrame), C.POINTER(OrbmLast), C.c_float, i,
                                                  C.c_float, i, vp, C.POINTER(i)]
+    L.orbm_search_by_projection_last_pairs.argtypes = [vp, C.POINTER(OrbmFrame), C.POINTER(OrbmLast), C.c_float, i,
+                                                       C.c_float, i, vp, vp, C.POINTER(i)]
     L.orbm_search_by_projection_points.argtypes = [vp, C.POINTER(OrbmFrame), C.POINTER(OrbmTrackPoints), C.c_float,
                                                    C.c_float, vp, C.POINTER(i)]
     L.orbm_search_projected.argtypes = [vp, C.POINTER(OrbmFrame), C.POINTER(OrbmQueries), i, i, i, vp, C.POINTER(i)]

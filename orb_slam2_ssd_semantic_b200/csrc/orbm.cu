@@ -156,12 +156,15 @@ static int check_cur(const OrbmFrame* cur) {
   return B200ORB_OK;
 }
 
-int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono,
-                                   float nnratio, int check_ori, int32_t* cur2last, int* nmatches) {
+// both (cur, last) entries: last2cur_accepted == NULL is orbm_search_by_projection_last
+static int search_last(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono, float nnratio,
+                       int check_ori, int32_t* cur2last, int32_t* last2cur_accepted, int* nmatches) {
   if (!h || !cur || !last || !cur2last || !nmatches) { set_error("null argument"); return B200ORB_EINVAL; }
   B200_CHECK(check_cur(cur));
   if (last->n < 0) { set_error("bad keypoint count"); return B200ORB_EINVAL; }
   *nmatches = 0;
+  if (last2cur_accepted)
+    for (int i = 0; i < last->n; ++i) last2cur_accepted[i] = -1;
   if (cur->n == 0) return B200ORB_OK;
   if (last->n == 0) {
     for (int j = 0; j < cur->n; ++j) cur2last[j] = (cur->mp_obs && cur->mp_obs[j] >= 0) ? -2 : -1;
@@ -194,8 +197,22 @@ int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLa
   B200_CHECK(launch_match_last(cv, lv, cam, 1, d_scratch, d_acc, d_out, d_nm, h->stream, &h->launches));
   B200_CUDA(cudaMemcpyAsync(cur2last, d_out, sizeof(int) * nc, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaMemcpyAsync(nmatches, d_nm, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (last2cur_accepted)
+    B200_CUDA(cudaMemcpyAsync(last2cur_accepted, d_acc, sizeof(int) * nl, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
+}
+
+int orbm_search_by_projection_last(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono,
+                                   float nnratio, int check_ori, int32_t* cur2last, int* nmatches) {
+  return search_last(h, cur, last, th, mono, nnratio, check_ori, cur2last, nullptr, nmatches);
+}
+
+int orbm_search_by_projection_last_pairs(orbm_t* h, const OrbmFrame* cur, const OrbmLast* last, float th, int mono,
+                                         float nnratio, int check_ori, int32_t* cur2last, int32_t* last2cur_accepted,
+                                         int* nmatches) {
+  if (!last2cur_accepted) { set_error("null argument"); return B200ORB_EINVAL; }
+  return search_last(h, cur, last, th, mono, nnratio, check_ori, cur2last, last2cur_accepted, nmatches);
 }
 
 int orbm_search_by_projection_points(orbm_t* h, const OrbmFrame* f, const OrbmTrackPoints* pts, float th, float nnratio,

@@ -14,6 +14,7 @@
 
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <cstdlib>
@@ -45,6 +46,16 @@ class ORBextractor {
   ~ORBextractor() { orbx_destroy(h_); }
   ORBextractor(const ORBextractor&) = delete;
   ORBextractor& operator=(const ORBextractor&) = delete;
+  // takes over the handle: perfect/src/Map.cc:239 copy-initialises an extractor from a temporary, which before C++17
+  // needs a copy or move constructor
+  ORBextractor(ORBextractor&& o)
+      : mvImagePyramid(std::move(o.mvImagePyramid)), nfeatures(o.nfeatures), scaleFactor(o.scaleFactor), nlevels(o.nlevels),
+        iniThFAST(o.iniThFAST), minThFAST(o.minThFAST), mvScaleFactor(std::move(o.mvScaleFactor)),
+        mvInvScaleFactor(std::move(o.mvInvScaleFactor)), mvLevelSigma2(std::move(o.mvLevelSigma2)),
+        mvInvLevelSigma2(std::move(o.mvInvLevelSigma2)), h_(o.h_), kps_(std::move(o.kps_)), desc_(std::move(o.desc_)),
+        pyramid_valid_(o.pyramid_valid_) {
+    o.h_ = nullptr;
+  }
 
   // src/ORBextractor.cc:1052-1114.  `mask` is ignored exactly like the reference ignores it.
   void operator()(cv::InputArray _image, cv::InputArray /*mask*/, std::vector<cv::KeyPoint>& _keypoints,

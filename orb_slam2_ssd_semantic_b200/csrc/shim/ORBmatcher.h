@@ -3,6 +3,10 @@
 // Put this directory BEFORE the reference's include/ on the include path: Tracking.cc, LocalMapping.cc, LoopClosing.cc,
 // Frame.cc, KeyFrame.cc, MapPoint.cc, Sim3Solver.cc then compile unchanged (the GPU test suite does exactly that with the
 // reference's own Frame.cc / KeyFrame.cc / MapPoint.cc: oracle/Makefile, target `shim`).
+// The same header stands in for perfect/include/ORBmatcher.h, which declares one member more: the 2-D point-pair overload
+// of SearchByProjection(Frame&, const Frame&, ...) that the perfect tree's TrackHomo calls (perfect/include/ORBmatcher.h:
+// 64-68).  The T tree never calls it, so there the extra member does nothing (oracle/homo.mk builds the perfect
+// tree's Frame.cc / KeyFrame.cc / MapPoint.cc / Map.cc against this directory).
 //
 // The reference's searches walk and MUTATE the Frame / KeyFrame / MapPoint object graph.  Each member below
 //   1. flattens what the search reads into the array views of include/b200orb.h; the few scalar lines per MapPoint that
@@ -74,37 +78,21 @@ class ORBmatcher {
 
   // ---- src/ORBmatcher.cc:1578-1724 -----------------------------------------------------------------------------------
   int SearchByProjection(Frame& CurrentFrame, const Frame& LastFrame, const float th, const bool bMono) {
-    FlatFrame cur;
-    flatten(CurrentFrame, cur, true);
-    const int nl = LastFrame.N;
-    std::vector<float> xw((size_t)(nl > 0 ? nl : 1) * 3, 0.f), lang(nl);
-    std::vector<uint8_t> valid(nl, 0), ldesc((size_t)(nl > 0 ? nl : 1) * 32, 0);
-    std::vector<int32_t> loct(nl), lobs(nl, 0);
-    for (int i = 0; i < nl; ++i) {
-      MapPoint* pMP = LastFrame.mvpMapPoints[i];
-      loct[i] = LastFrame.mvKeys[i].octave;
-      lang[i] = LastFrame.mvKeysUn[i].angle;
-      if (pMP && !LastFrame.mvbOutlier[i]) {
-        valid[i] = 1;
-        cv::Mat p = pMP->GetWorldPos();
-        for (int k = 0; k < 3; ++k) xw[(size_t)i * 3 + k] = p.at<float>(k);
-        cv::Mat d = pMP->GetDescriptor();
-        std::memcpy(&ldesc[(size_t)i * 32], d.ptr(0), 32);
-        lobs[i] = pMP->Observations();
+    return search_last(CurrentFrame, LastFrame, th, bMono, NULL);
+  }
+
+  // ---- perfect/src/ORBmatcher.cc:1727-1880 (TrackHomo, perfect/src/Tracking.cc:1362,1371) ----------------------------
+  // The search above plus one point pair per accepted query, pushed before the rotation prune (:1835-1836): the prune
+  // leaves the pairs it unmatches in place.  Appends, never clears; the points are the distorted mvKeys.
+  int SearchByProjection(Frame& CurrentFrame, const Frame& LastFrame, const float th, const bool bMono,
+                         std::vector<cv::Point2f>& points_last, std::vector<cv::Point2f>& points_current) {
+    std::vector<int32_t> acc;
+    const int nmatches = search_last(CurrentFrame, LastFrame, th, bMono, &acc);
+    for (int i = 0; i < LastFrame.N; ++i)
+      if (acc[i] >= 0) {
+        points_last.push_back(LastFrame.mvKeys[i].pt);
+        points_current.push_back(CurrentFrame.mvKeys[acc[i]].pt);
       }
-    }
-    OrbmLast L;
-    L.n = nl; L.xw = xw.data(); L.valid = valid.data(); L.octave = loct.data(); L.angle = lang.data();
-    L.mp_desc = ldesc.data(); L.mp_obs = lobs.data();
-    copy_pose(LastFrame.mTcw, L.Tcw);
-    std::vector<int32_t> c2l(cur.n > 0 ? cur.n : 1, -1);
-    int nmatches = 0;
-    check(orbm_search_by_projection_last(h_, &cur.view, &L, th, bMono ? 1 : 0, mfNNratio, mbCheckOrientation ? 1 : 0, c2l.data(),
-                                         &nmatches));
-    for (int j = 0; j < cur.n; ++j) {      // the pointer state the reference leaves behind (:1680,:1716)
-      if (c2l[j] >= 0) CurrentFrame.mvpMapPoints[j] = LastFrame.mvpMapPoints[c2l[j]];
-      else if (c2l[j] == -1) CurrentFrame.mvpMapPoints[j] = static_cast<MapPoint*>(NULL);
-    }
     return nmatches;
   }
 
@@ -506,6 +494,48 @@ class ORBmatcher {
   static const int HISTO_LENGTH;
 
  protected:
+  // both (Frame&, const Frame&) overloads; acc != NULL: the per-query accepted current keypoint, or -1
+  int search_last(Frame& CurrentFrame, const Frame& LastFrame, const float th, const bool bMono, std::vector<int32_t>* acc) {
+    FlatFrame cur;
+    flatten(CurrentFrame, cur, true);
+    const int nl = LastFrame.N;
+    std::vector<float> xw((size_t)(nl > 0 ? nl : 1) * 3, 0.f), lang(nl);
+    std::vector<uint8_t> valid(nl, 0), ldesc((size_t)(nl > 0 ? nl : 1) * 32, 0);
+    std::vector<int32_t> loct(nl), lobs(nl, 0);
+    for (int i = 0; i < nl; ++i) {
+      MapPoint* pMP = LastFrame.mvpMapPoints[i];
+      loct[i] = LastFrame.mvKeys[i].octave;
+      lang[i] = LastFrame.mvKeysUn[i].angle;
+      if (pMP && !LastFrame.mvbOutlier[i]) {
+        valid[i] = 1;
+        cv::Mat p = pMP->GetWorldPos();
+        for (int k = 0; k < 3; ++k) xw[(size_t)i * 3 + k] = p.at<float>(k);
+        cv::Mat d = pMP->GetDescriptor();
+        std::memcpy(&ldesc[(size_t)i * 32], d.ptr(0), 32);
+        lobs[i] = pMP->Observations();
+      }
+    }
+    OrbmLast L;
+    L.n = nl; L.xw = xw.data(); L.valid = valid.data(); L.octave = loct.data(); L.angle = lang.data();
+    L.mp_desc = ldesc.data(); L.mp_obs = lobs.data();
+    copy_pose(LastFrame.mTcw, L.Tcw);
+    std::vector<int32_t> c2l(cur.n > 0 ? cur.n : 1, -1);
+    int nmatches = 0;
+    if (acc) {
+      acc->assign(nl > 0 ? nl : 1, -1);
+      check(orbm_search_by_projection_last_pairs(h_, &cur.view, &L, th, bMono ? 1 : 0, mfNNratio, mbCheckOrientation ? 1 : 0,
+                                                 c2l.data(), acc->data(), &nmatches));
+    } else {
+      check(orbm_search_by_projection_last(h_, &cur.view, &L, th, bMono ? 1 : 0, mfNNratio, mbCheckOrientation ? 1 : 0,
+                                           c2l.data(), &nmatches));
+    }
+    for (int j = 0; j < cur.n; ++j) {      // the pointer state the reference leaves behind (:1680,:1716)
+      if (c2l[j] >= 0) CurrentFrame.mvpMapPoints[j] = LastFrame.mvpMapPoints[c2l[j]];
+      else if (c2l[j] == -1) CurrentFrame.mvpMapPoints[j] = static_cast<MapPoint*>(NULL);
+    }
+    return nmatches;
+  }
+
   void open() {
     int dev = 0;
     if (const char* e = std::getenv("B200ORB_DEVICE")) dev = std::atoi(e);

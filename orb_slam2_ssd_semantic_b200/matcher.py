@@ -61,6 +61,22 @@ class ORBmatcher:
             raise TypeError("SearchByProjection: second argument must be a LastView or a TrackPointsView")
         return nm.value, out
 
+    def SearchByProjectionPairs(self, F: FrameView, last: LastView, th: float, bMono: bool = False):
+        """The perfect tree's (Frame&, const Frame& LastFrame, th, bMono, points_last, points_current)
+        (perfect/src/ORBmatcher.cc:1727-1880) -> (nmatches, cur2last, pairs).  nmatches and cur2last are those of
+        SearchByProjection(F, last, th, bMono); pairs is a k x 2 int32 array of (i, j): last keypoint i accepted current
+        keypoint j, in ascending i, taken before the rotation prune.  The reference pushes
+        (LastFrame.mvKeys[i].pt, CurrentFrame.mvKeys[j].pt) for each row: the distorted keypoints."""
+        out = np.full(F.n, -1, np.int32)
+        acc = np.full(max(last.n, 1), -1, np.int32)
+        nm = C.c_int(0)
+        fs, ls = F.struct(), last.struct()
+        _lib.check(self._L.orbm_search_by_projection_last_pairs(self._h, C.byref(fs), C.byref(ls), float(th), int(bMono),
+                                                                self.mfNNratio, int(self.mbCheckOrientation), ptr(out),
+                                                                ptr(acc), C.byref(nm)))
+        i = np.flatnonzero(acc[:last.n] >= 0).astype(np.int32)
+        return nm.value, out, np.stack([i, acc[i]], axis=1).reshape(-1, 2)
+
     def SearchProjected(self, F: FrameView, queries: QueriesView, max_dist: int, claim_rule: int = 1):
         """Shared tail of the projection overloads whose geometry the caller computes (relocalisation
         src/ORBmatcher.cc:1757-1899 -> claim_rule 1, max_dist = ORBdist; see include/b200orb.h)."""
