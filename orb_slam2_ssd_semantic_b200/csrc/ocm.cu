@@ -6,8 +6,10 @@
 //
 // HBM layout:
 //   leaf table   open-addressing hash of the 1-cm VoxelGrid cells of ONE keyframe (key = 3 x 21-bit cell index), one
-//                32-byte record per cell: key, count, first pixel, bucket offset.  Pixels of a cell are bucketed, sorted ascending and
-//                summed sequentially in float so the centroid equals the oracle's pixel-order sum bit for bit.
+//                16-byte record per cell: key, pixel count, position in the keyframe's cell list.  Per-cell state after
+//                binning (count, bucket offset) lives in dense arrays indexed by that position.  Pixels of a cell are
+//                bucketed, sorted ascending and summed sequentially in float so the centroid equals the oracle's
+//                pixel-order sum bit for bit.
 //   points       world-frame centroids of the last keyframe (xyz f32, rgb, ground label), unordered
 //   map          persistent open-addressing hash: key (3 x u16 OcTreeKey packed in u64) -> float log-odds, colour, the
 //                clamp-add summary (a, lo, hi) used by the multi-GPU merge, and the batch masks: bit j of the hit / miss
@@ -23,6 +25,8 @@
 
 #include <dlfcn.h>
 #include <nccl.h>
+
+#include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
 
@@ -90,21 +94,18 @@ struct OcmConst {
   int rows, cols;
 };
 
-// One 32-byte record (= one L2 sector) per VoxelGrid cell: an insert, the bucket bookkeeping and the reset all touch
-// the same sector instead of five arrays.
-struct __align__(32) LeafRec {
+// One 16-byte record per VoxelGrid cell.  k_ocm_bin inserts the key and adds the pixel counts; k_ocm_ranges moves the
+// count to the dense arrays, stores the cell's list position for k_ocm_scatter and empties the record for the next
+// keyframe in the same 16-byte store (the stale `cell` is never read before k_ocm_ranges writes it again).
+struct __align__(16) LeafRec {
   unsigned long long key;
   int count;
-  int first;     // smallest pixel index
-  int offset;
-  int pad[3];
+  int cell;      // position in the keyframe's cell list (valid from k_ocm_ranges to k_ocm_scatter)
 };
-static_assert(sizeof(LeafRec) == 32, "one L2 sector per leaf record");
-// An unused record: the initial fill of a leaf table, and what k_ocm_centroids leaves behind for the next keyframe.
+static_assert(sizeof(LeafRec) == 16, "one 16-byte record per leaf");
 __host__ __device__ __forceinline__ LeafRec empty_leaf() {
   LeafRec r{};
   r.key = EMPTY_KEY;
-  r.first = 0x7fffffff;
   return r;
 }
 struct LeafTable {
@@ -158,7 +159,9 @@ __device__ __forceinline__ bool map_touch(const MapView& m, unsigned long long k
 // as ONE launch (blockIdx.y = job = bit index of the keyframe in the batch masks of the map).
 struct KfScratch {
   LeafTable leaf;
-  int *pix_slot, *pix_rank, *bucket, *voxlist;   // pix_rank: position of the pixel inside its cell's bucket
+  int *pix_slot, *pix_rank, *bucket;   // pix_rank: position of the pixel inside its cell's bucket
+  // the keyframe's cell list (cell = position in it = point index): leaf-table slot, pixel count, bucket offset
+  int *cell_slot, *cell_count, *cell_off;
   int* counters;   // [0] pixels, [1] voxels (= points)
   float* pts;
   uint8_t *pts_rgb, *pts_label;
@@ -197,127 +200,185 @@ __device__ __forceinline__ unsigned long long leaf_key(const OcmConst& c, float 
          ((unsigned long long)(iz & 0x1fffff) << 42);
 }
 
-// Pixel of this thread for the warp-tiled kernels: a warp covers an 8 x 4 pixel tile (lane = ty * 8 + tx, so lanes are
-// in row-major order inside the tile).  Neighbouring pixels mostly fall into the same 1-cm cell, so the cell-level
-// atomics are issued once per (warp, cell) by the lowest lane of each __match_any group.
-__device__ __forceinline__ int tile_pixel(int rows, int cols) {
-  const int lane = threadIdx.x & 31;
-  const int tiles_x = (cols + 7) >> 3;
-  const int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
-  const int y = ty * 4 + (lane >> 3), x = tx * 8 + (lane & 7);
-  return (y < rows && x < cols) ? y * cols + x : -1;
-}
-__host__ __device__ inline int tile_blocks(int rows, int cols, int warps_per_block) {
-  const int tiles = ((cols + 7) >> 3) * ((rows + 3) >> 2);
-  return (tiles + warps_per_block - 1) / warps_per_block;
-}
+// K11a: gate + VoxelGrid cell of every pixel, binned per CTA tile of BIN_TW x BIN_TH pixels (one thread per pixel, one
+// warp per tile row).  The tile's distinct cells are deduplicated in shared memory, and each (tile, cell) makes the only
+// global accesses of the tile for that cell: one find-or-insert probe of the leaf table and one atomicAdd of its pixel
+// count, whose return value is the tile's first position in the cell's bucket.  New cells are appended to the cell list
+// with one atomicAdd per CTA.  Inside the tile, the positions follow ascending pixel index (rows of the tile in order,
+// lanes in order), so a cell's bucket is a few ascending runs.  32 x 16 rather than 32 x 8: k_ocm_bin itself costs the
+// same with either, but the cell list is appended tile by tile, so taller tiles hand k_ocm_scan_keys points that lie
+// closer together and its free-cell cache hits more often (one bench step's insert 16.7 against 17.4 ms, H100 80 GB
+// HBM3 at 700 W).
+constexpr int BIN_TW = 32, BIN_TH = 16, BIN_THREADS = BIN_TW * BIN_TH;
+// The shared table has twice as many entries as the tile has pixels: it cannot fill up, even when every pixel is its own
+// cell.
+constexpr int BIN_SLOTS = 2 * BIN_THREADS;
+static_assert(BIN_TW == 32 && BIN_TH <= 16, "a tile row is one warp; the per-row counts of a cell are 16 bytes");
 
-// K11a: gate + VoxelGrid cell of every pixel
-__global__ void k_ocm_bin(const KfJob* __restrict__ jobs, int* __restrict__ err) {
+__device__ __forceinline__ int bytes_sum(unsigned w) { return (int)__dp4a(w, 0x01010101u, 0u); }
+
+__global__ void __launch_bounds__(BIN_THREADS) k_ocm_bin(const KfJob* __restrict__ jobs, int* __restrict__ err) {
+  __shared__ unsigned long long s_key[BIN_SLOTS];
+  __shared__ uint4 s_rows[BIN_SLOTS];     // byte r: pixels of the cell in tile row r
+  __shared__ int s_slot[BIN_SLOTS], s_base[BIN_SLOTS];
+  __shared__ int s_fresh, s_fresh_base;
   const KfJob& J = jobs[blockIdx.y];
   const OcmConst& c = J.c;
-  const float* __restrict__ depth = J.depth;
   const LeafTable lt = J.s.leaf;
-  int* __restrict__ pix_slot = J.s.pix_slot;
-  int* __restrict__ counters = J.s.counters;
-  int* __restrict__ voxlist = J.s.voxlist;
-  const int lane = threadIdx.x & 31;
-  const int pix = tile_pixel(c.rows, c.cols);
+  for (int i = threadIdx.x; i < BIN_SLOTS; i += BIN_THREADS) {
+    s_key[i] = EMPTY_KEY;
+    s_rows[i] = make_uint4(0u, 0u, 0u, 0u);
+  }
+  if (threadIdx.x == 0) s_fresh = 0;
+  const int lane = threadIdx.x & 31, row = threadIdx.x >> 5;
+  const int tiles_x = (c.cols + BIN_TW - 1) / BIN_TW;
+  const int ty = blockIdx.x / tiles_x, tx = blockIdx.x - ty * tiles_x;
+  const int px = tx * BIN_TW + lane, py = ty * BIN_TH + row;
+  const int pix = (px < c.cols && py < c.rows) ? py * c.cols + px : -1;
   float x, y, z;
-  const bool ok = pix >= 0 && backproject(c, depth, pix, x, y, z);
-  const unsigned long long key = ok ? leaf_key(c, x, y, z) : (EMPTY_KEY - 1ull - (unsigned long long)lane);
+  const bool ok = pix >= 0 && backproject(c, J.depth, pix, x, y, z);
+  const unsigned long long key = ok ? leaf_key(c, x, y, z) : EMPTY_KEY;
   const unsigned grp = __match_any_sync(0xffffffffu, key);
-  const int leader = __ffs(grp) - 1;
-  int slot = -1, rank = 0;
-  if (ok && lane == leader) {   // lowest lane of the group = smallest pixel index of the group
-    bool fresh;
-    long long s;
-    // Branch on the slot's sign, not on the flag: the compiler cannot fold a sign test into the probe's exits, so the
-    // leader lanes reconverge before the cell atomics below.  Branching on the flag lets them run those atomics
-    // diverged (k_ocm_bin 12 % slower on an H100).
-    if (!table_probe<sizeof(LeafRec) / 8>(&lt.rec->key, lt.mask, key, &s, &fresh)) s = -1;
-    if (s < 0) { atomicExch(err, ERR_LEAF_TABLE_FULL); }
-    else {
-      slot = (int)s;
-      if (fresh) voxlist[atomicAdd(&counters[1], 1)] = slot;   // list of occupied cells: no table sweep later
-      rank = atomicAdd(&lt.rec[s].count, __popc(grp));          // the group's first position in the cell's bucket
-      atomicMin(&lt.rec[s].first, pix);
+  const int leader = __ffs(grp) - 1;       // lowest lane of the group = smallest pixel of the cell in this row
+  const bool lead = ok && lane == leader;
+  __syncthreads();
+  int ls = 0;                              // the cell's entry in the shared table
+  if (lead) {
+    ls = (int)hash_slot(key, BIN_SLOTS - 1);
+    for (;;) {
+      const unsigned long long old = atomicCAS(&s_key[ls], EMPTY_KEY, key);
+      if (old == EMPTY_KEY || old == key) break;
+      ls = (ls + 1) & (BIN_SLOTS - 1);
     }
+    reinterpret_cast<unsigned char*>(&s_rows[ls])[row] = (unsigned char)__popc(grp);
+  }
+  __syncthreads();
+  int before = 0, slot = -1, pos = -1;     // before: pixels of the cell in the rows above
+  if (lead) {
+    const uint4 r = s_rows[ls];
+    const unsigned w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int k = row - 4 * i;           // bytes of word i that belong to rows above this one
+      before += bytes_sum(k <= 0 ? 0u : (k >= 4 ? w[i] : w[i] & ((1u << (8 * k)) - 1u)));
+    }
+    if (before == 0) {                     // first row of the cell in the tile: the tile's one global probe for it
+      const int total = bytes_sum(r.x) + bytes_sum(r.y) + bytes_sum(r.z) + bytes_sum(r.w);
+      bool fresh;
+      long long s;
+      if (!table_probe<sizeof(LeafRec) / 8>(&lt.rec->key, lt.mask, key, &s, &fresh)) {
+        atomicExch(err, ERR_LEAF_TABLE_FULL);
+        s_slot[ls] = -1;
+        s_base[ls] = 0;
+      } else {
+        slot = (int)s;
+        s_slot[ls] = slot;
+        s_base[ls] = atomicAdd(&lt.rec[s].count, total);
+        if (fresh) pos = atomicAdd(&s_fresh, 1);
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_fresh) s_fresh_base = atomicAdd(&J.s.counters[1], s_fresh);
+  __syncthreads();
+  if (pos >= 0) J.s.cell_slot[s_fresh_base + pos] = slot;
+  int rank = 0;
+  if (lead) {
+    slot = s_slot[ls];
+    rank = s_base[ls] + before;
   }
   slot = __shfl_sync(0xffffffffu, slot, leader);
   rank = __shfl_sync(0xffffffffu, rank, leader) + __popc(grp & ((1u << lane) - 1u));
   if (pix >= 0) {
-    pix_slot[pix] = ok ? slot : -1;
+    J.s.pix_slot[pix] = ok ? slot : -1;
     J.s.pix_rank[pix] = rank;
   }
 }
 
-// K11b: bucket ranges for the occupied cells (arbitrary order: the cloud is a set)
-__global__ void k_ocm_ranges(const KfJob* __restrict__ jobs) {
+// K11b: bucket ranges of the cells in list order (the cloud is a set, so any order would do): a block scan of the
+// counts and one atomicAdd per CTA and round.  Moves each cell's count into the dense arrays and empties its leaf record,
+// leaving only the cell's list position there for k_ocm_scatter.
+constexpr int RANGES_THREADS = 256;
+__global__ void __launch_bounds__(RANGES_THREADS) k_ocm_ranges(const KfJob* __restrict__ jobs) {
+  using Scan = cub::BlockScan<int, RANGES_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ int s_base;
   const KfJob& J = jobs[blockIdx.y];
-  const LeafTable lt = J.s.leaf;
-  int* __restrict__ counters = J.s.counters;   // [0]=pixels, [1]=voxels
-  const int* __restrict__ voxlist = J.s.voxlist;
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= counters[1]) return;
-  const int s = voxlist[v];
-  lt.rec[s].offset = atomicAdd(&counters[0], lt.rec[s].count);
+  LeafRec* __restrict__ rec = J.s.leaf.rec;
+  const int n = J.s.counters[1];
+  for (int v0 = blockIdx.x * RANGES_THREADS; v0 < n; v0 += gridDim.x * RANGES_THREADS) {
+    const int v = v0 + threadIdx.x;
+    int s = 0, cnt = 0;
+    if (v < n) {
+      s = J.s.cell_slot[v];
+      cnt = rec[s].count;
+    }
+    int off, total;
+    Scan(tmp).ExclusiveSum(cnt, off, total);
+    if (threadIdx.x == 0) s_base = atomicAdd(&J.s.counters[0], total);
+    __syncthreads();
+    if (v < n) {
+      J.s.cell_count[v] = cnt;
+      J.s.cell_off[v] = s_base + off;
+      LeafRec r = empty_leaf();
+      r.cell = v;
+      rec[s] = r;
+    }
+    __syncthreads();   // tmp and s_base are reused by the next round
+  }
 }
 
 // K11c: scatter the pixel indices into their cell's bucket
 __global__ void k_ocm_scatter(const KfJob* __restrict__ jobs) {
   const KfJob& J = jobs[blockIdx.y];
-  const int pix = tile_pixel(J.c.rows, J.c.cols);
-  if (pix < 0) return;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= J.c.rows * J.c.cols) return;
   const int s = J.s.pix_slot[pix];
-  if (s >= 0) J.s.bucket[J.s.leaf.rec[s].offset + J.s.pix_rank[pix]] = pix;   // positions were handed out by k_ocm_bin
+  if (s >= 0) J.s.bucket[J.s.cell_off[J.s.leaf.rec[s].cell] + J.s.pix_rank[pix]] = pix;   // ranks come from k_ocm_bin
 }
 
 // K11d: per cell: restore pixel order, sequential float centroid (PCL VoxelGrid), transform to the world frame in
-// double (pcl::transformPointCloud), emit the point; also resets the cell's table entry for the next keyframe.
+// double (pcl::transformPointCloud), emit the point.  The label is that of the cell's smallest pixel.
 __global__ void k_ocm_centroids(const KfJob* __restrict__ jobs) {
   const KfJob& J = jobs[blockIdx.y];
   const OcmConst& c = J.c;
   const float* __restrict__ depth = J.depth;
   const uint8_t* __restrict__ rgb = J.rgb;
   const uint8_t* __restrict__ label = J.label;
-  const LeafTable lt = J.s.leaf;
-  const int* __restrict__ counters = J.s.counters;
-  const int* __restrict__ voxlist = J.s.voxlist;
+  const int* __restrict__ cell_count = J.s.cell_count;
+  const int* __restrict__ cell_off = J.s.cell_off;
   int* __restrict__ bucket = J.s.bucket;
   float* __restrict__ pts = J.s.pts;
   uint8_t* __restrict__ pts_rgb = J.s.pts_rgb;
   uint8_t* __restrict__ pts_label = J.s.pts_label;
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= counters[1]) return;
-  const int s = voxlist[v];
-  const int n = lt.rec[s].count;
-  int* b = bucket + lt.rec[s].offset;
-  for (int i = 1; i < n; ++i) {   // insertion sort: ascending pixel index = row-major order
-    const int val = b[i];
-    int j = i - 1;
-    while (j >= 0 && b[j] > val) { b[j + 1] = b[j]; --j; }
-    b[j + 1] = val;
-  }
-  float sx = 0.f, sy = 0.f, sz = 0.f, sr = 0.f, sg = 0.f, sb = 0.f;
-  for (int i = 0; i < n; ++i) {
-    float x, y, z;
-    backproject(c, depth, b[i], x, y, z);
-    sx += x; sy += y; sz += z;
-    const uint8_t* col = rgb + (size_t)b[i] * 3;   // b,g,r (cv::Mat BGR)
-    sr += (float)col[2]; sg += (float)col[1]; sb += (float)col[0];
-  }
-  const float fn = (float)n;
-  const double px = (double)(sx / fn), py = (double)(sy / fn), pz = (double)(sz / fn);
+  const int ncells = J.s.counters[1];
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < ncells; v += gridDim.x * blockDim.x) {
+    const int n = cell_count[v];
+    int* b = bucket + cell_off[v];
+    for (int i = 1; i < n; ++i) {   // insertion sort: ascending pixel index = row-major order
+      const int val = b[i];
+      int j = i - 1;
+      while (j >= 0 && b[j] > val) { b[j + 1] = b[j]; --j; }
+      b[j + 1] = val;
+    }
+    float sx = 0.f, sy = 0.f, sz = 0.f, sr = 0.f, sg = 0.f, sb = 0.f;
+    for (int i = 0; i < n; ++i) {
+      float x, y, z;
+      backproject(c, depth, b[i], x, y, z);
+      sx += x; sy += y; sz += z;
+      const uint8_t* col = rgb + (size_t)b[i] * 3;   // b,g,r (cv::Mat BGR)
+      sr += (float)col[2]; sg += (float)col[1]; sb += (float)col[0];
+    }
+    const float fn = (float)n;
+    const double px = (double)(sx / fn), py = (double)(sy / fn), pz = (double)(sz / fn);
 #pragma unroll
-  for (int i = 0; i < 3; ++i)
-    pts[(size_t)v * 3 + i] = (float)(c.Rt[i * 3 + 0] * px + c.Rt[i * 3 + 1] * py + c.Rt[i * 3 + 2] * pz + c.ti[i]);
-  pts_rgb[(size_t)v * 3 + 0] = (uint8_t)(sr / fn);
-  pts_rgb[(size_t)v * 3 + 1] = (uint8_t)(sg / fn);
-  pts_rgb[(size_t)v * 3 + 2] = (uint8_t)(sb / fn);
-  pts_label[v] = label ? label[lt.rec[s].first] : 0;
-  lt.rec[s] = empty_leaf();
+    for (int i = 0; i < 3; ++i)
+      pts[(size_t)v * 3 + i] = (float)(c.Rt[i * 3 + 0] * px + c.Rt[i * 3 + 1] * py + c.Rt[i * 3 + 2] * pz + c.ti[i]);
+    pts_rgb[(size_t)v * 3 + 0] = (uint8_t)(sr / fn);
+    pts_rgb[(size_t)v * 3 + 1] = (uint8_t)(sg / fn);
+    pts_rgb[(size_t)v * 3 + 2] = (uint8_t)(sb / fn);
+    pts_label[v] = label ? label[b[0]] : 0;
+  }
 }
 
 // leaf <= 0: no VoxelGrid; every gated pixel is a point (used for the T-variant style clouds)
@@ -371,21 +432,12 @@ __device__ __forceinline__ bool scan_touch_free(const MapView& m, unsigned long 
   return map_touch(m, key, j, false, 0u);
 }
 
-__global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__ jobs, MapView m, int* __restrict__ err) {
-  __shared__ unsigned long long s_seen[SCAN_CACHE];
-  for (int i = threadIdx.x; i < SCAN_CACHE; i += blockDim.x) s_seen[i] = EMPTY_KEY;
-  __syncthreads();
-  const int j = blockIdx.y;
-  const KfJob& J = jobs[j];
+__device__ __forceinline__ void scan_point(const KfJob& J, const MapView& m, unsigned long long* s_seen, int j, int v,
+                                           bool all_ground, int* __restrict__ err) {
   const OcmConst& c = J.c;
-  const int* __restrict__ counters = J.s.counters;
   const float* __restrict__ pts = J.s.pts;
   const uint8_t* __restrict__ pts_label = J.s.pts_label;
   const uint8_t* __restrict__ pts_rgb = J.s.pts_rgb;
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= counters[1]) return;
-  // perfect/src/MapDrawer.cc:676-680: a cloud of fewer than 50 points skips the plane extraction and is ALL ground
-  const bool all_ground = counters[1] < 50;
   const float e[3] = {pts[(size_t)v * 3], pts[(size_t)v * 3 + 1], pts[(size_t)v * 3 + 2]};
   int ke[3];
   const bool end_ok = coord_to_key(c, e[0], ke[0]) && coord_to_key(c, e[1], ke[1]) && coord_to_key(c, e[2], ke[2]);
@@ -452,6 +504,19 @@ __global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__
     pending = true;
     pending_key = pack_key(cur[0], cur[1], cur[2]);
   }
+}
+
+__global__ void __launch_bounds__(256) k_ocm_scan_keys(const KfJob* __restrict__ jobs, MapView m, int* __restrict__ err) {
+  __shared__ unsigned long long s_seen[SCAN_CACHE];
+  for (int i = threadIdx.x; i < SCAN_CACHE; i += blockDim.x) s_seen[i] = EMPTY_KEY;
+  __syncthreads();
+  const int j = blockIdx.y;
+  const KfJob& J = jobs[j];
+  const int n = J.s.counters[1];
+  // perfect/src/MapDrawer.cc:676-680: a cloud of fewer than 50 points skips the plane extraction and is ALL ground
+  const bool all_ground = n < 50;
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x)
+    scan_point(J, m, s_seen, j, v, all_ground, err);
 }
 
 // K14: replay, voxel by voxel, the observations of the batch in keyframe order (MapDrawer.cc:1007-1022 per keyframe:
@@ -661,6 +726,11 @@ struct ocm {
              float fy, float cx, float cy) {
     return insert_batch(1, &dd, &drgb, &dlabel, r, c, Tcw, fx, fy, cx, cy);
   }
+  // CTAs per keyframe of the kernels that loop over a keyframe's cells (k_ocm_ranges, k_ocm_centroids,
+  // k_ocm_scan_keys, 256 threads each): the cell count is only known on the device, so the grid is fixed --
+  // CELL_CTAS_PER_SM per SM, shared by the B keyframes of the launch -- and each CTA loops over the cells.
+  static constexpr int CELL_CTAS_PER_SM = 8;
+  unsigned cell_ctas(int B) const { return (unsigned)std::max(1, (CELL_CTAS_PER_SM * sms + B - 1) / B); }
   int check_err();
   int clear_map();
   int scan(unsigned long long* data, int n);
@@ -691,7 +761,7 @@ int ocm::ensure_scratch(int r, int c, int nslots) {
     B200_CHECK(s.block.carve(stream, [&](Carver& t) {
       k.leaf.rec = t.take<LeafRec>(leaf_cap);
       k.pix_slot = t.take<int>(npix); k.pix_rank = t.take<int>(npix); k.bucket = t.take<int>(npix);
-      k.voxlist = t.take<int>(npix);
+      k.cell_slot = t.take<int>(npix); k.cell_count = t.take<int>(npix); k.cell_off = t.take<int>(npix);
       k.pts = t.take<float>(3 * npix); k.pts_rgb = t.take<uint8_t>(3 * npix); k.pts_label = t.take<uint8_t>(npix);
     }));
     k.leaf.mask = leaf_cap - 1;
@@ -791,19 +861,19 @@ int ocm::insert_batch(int n, const float* const* dd, const uint8_t* const* drgb,
     B200_CUDA(cudaMemcpyAsync(dj, hj, sizeof(KfJob) * B, cudaMemcpyHostToDevice, stream));
     B200_CUDA(cudaEventRecord(job_ev[ring], stream));
     B200_CUDA(cudaMemsetAsync(d_counters, 0, 16 * B, stream));
-    const dim3 g256((npix + 255) / 256, B), g128((npix + 127) / 128, B);
+    const dim3 g256((npix + 255) / 256, B), gcell(cell_ctas(B), B);
     if (prm.leaf > 0) {
-      const dim3 gt(tile_blocks(r, c, 8), B);   // 8 x 4 pixel tile per warp
-      k_ocm_bin<<<gt, 256, 0, stream>>>(dj, d_err);
-      k_ocm_ranges<<<g256, 256, 0, stream>>>(dj);
-      k_ocm_scatter<<<gt, 256, 0, stream>>>(dj);
-      k_ocm_centroids<<<g128, 128, 0, stream>>>(dj);
+      const dim3 gt(((c + BIN_TW - 1) / BIN_TW) * ((r + BIN_TH - 1) / BIN_TH), B);
+      k_ocm_bin<<<gt, BIN_THREADS, 0, stream>>>(dj, d_err);
+      k_ocm_ranges<<<gcell, RANGES_THREADS, 0, stream>>>(dj);
+      k_ocm_scatter<<<g256, 256, 0, stream>>>(dj);
+      k_ocm_centroids<<<gcell, 256, 0, stream>>>(dj);
       launches += 4;
     } else {
       k_ocm_points_nofilter<<<g256, 256, 0, stream>>>(dj);
       launches += 1;
     }
-    k_ocm_scan_keys<<<g256, 256, 0, stream>>>(dj, map, d_err);
+    k_ocm_scan_keys<<<gcell, 256, 0, stream>>>(dj, map, d_err);
     // grid-stride sweep on a fixed grid (8 CTAs per SM)
     k_ocm_apply<<<8 * sms, 256, 0, stream>>>(hit_log, miss_log, cmin, cmax, map);
     launches += 2;
