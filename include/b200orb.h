@@ -627,6 +627,48 @@ int gcm_export(gcm_t* h, float* xyz, uint8_t* rgb, long long cap, long long* n);
 int gcm_sync(gcm_t* h);
 long long gcm_launch_count(const gcm_t* h);
 
+/* Semantic object clusters of the same loop (src/pointcloudmapping.cc:399-488).  The ncnn SSD detector stays outside:
+ * the caller passes its boxes (src/ncnn_dect.h:12-18, detector order).  For keyframe number `keyframe_index` (the `i`
+ * of :399, counted from 0 over every keyframe the map has been given):
+ *   - a box is used iff (double)prob > 0.54 (:418), else its record is GCM_BELOW_PROB;
+ *   - draw_rect_with_depth_threshold (:197-244, :426): the box's mean depth over its 30-70 % window, and its band
+ *     (|depth - mean| < 0.4) inside the rectangle shifted one row up and one column left; band pixels are painted in
+ *     colors_[class_id] (:47-60, B,G,R), a later box over an earlier one.  Flat indices wrap into the next row and
+ *     repeat, as the reference's do.  Deviation: indices outside [0, rows*cols) are skipped (the reference reads and
+ *     writes out of bounds there: boxes at x < 1 or y < 1 or past the bottom edge);
+ *   - "if((i%2==0)&&(objects.size()==0)) continue;" (:434): an even keyframe with n_objs == 0 adds nothing;
+ *   - otherwise generatePointCloud on the PAINTED image is appended to globalMap exactly as gcm_add_keyframe does
+ *     (:439, :482-485), and every used box gets ExtractIndices on its band, StatisticalOutlierRemoval (mean_k 50,
+ *     stddev_mul 1.0, :75-76), VoxelGrid(resolution), compute3DCentroid and getMinMax3D (:443-476) -> GCM_CLUSTER.
+ *     Deviation: a box with fewer than 51 band points gets GCM_FEW_POINTS and no cluster (PCL's filter reads past the
+ *     neighbour list it gets back there, and an empty box leaves the centroid uninitialised).
+ * clusters_out has n_objs records, one per box in order.  sem_merge (:246-322) stays with the caller, over the records
+ * and the detector's object names.  B200ORB_EINVAL for a class_id outside [0, 21) (the 21-entry colors_ / obj_size_
+ * tables, :50-70) or a non-finite rectangle or one beyond 2^24 px; B200ORB_ECAP when the boxes span more than 2^31 - 1
+ * band positions.  Synchronous like gcm_add_keyframe; the _device twin reads depth / colour from device memory, while
+ * objs and clusters_out stay on the host. */
+typedef struct GcmObject {
+  float x, y, width, height; /* cv::Rect_<float> */
+  int32_t class_id;
+  float prob;
+} GcmObject;
+#define GCM_CLUSTER 0    /* a cluster: every field below is set */
+#define GCM_BELOW_PROB 1 /* prob <= 0.54: the box is not used (n_* are 0) */
+#define GCM_FEW_POINTS 2 /* fewer than 51 band points: n_band is set, no cluster */
+typedef struct GcmCluster {
+  int32_t status;
+  int32_t n_band;    /* band indices (with repeats) = points ExtractIndices hands on */
+  int32_t n_inliers; /* after StatisticalOutlierRemoval */
+  int32_t n_voxels;  /* after VoxelGrid (= n_inliers where its index space overflows int: PCL returns the input) */
+  float centroid[3], min_pt[3], max_pt[3];
+} GcmCluster;
+int gcm_add_keyframe_objects(gcm_t* h, const float* depth, const uint8_t* bgr, int rows, int cols, const float Tcw[16],
+                             float fx, float fy, float cx, float cy, long long keyframe_index, const GcmObject* objs,
+                             int n_objs, GcmCluster* clusters_out);
+int gcm_add_keyframe_objects_device(gcm_t* h, const float* d_depth, const uint8_t* d_bgr, int rows, int cols,
+                                    const float Tcw[16], float fx, float fy, float cx, float cy, long long keyframe_index,
+                                    const GcmObject* objs, int n_objs, GcmCluster* clusters_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,7 +8,7 @@ from ._lib import B200OrbError, lib, library_path  # noqa: F401
 from .extractor import KP_DTYPE, ORBextractor  # noqa: F401
 from .matcher import ORBmatcher, FrameView, LastView, TrackPointsView, BowView, QueriesView  # noqa: F401
 from .pipeline import StreamTracker  # noqa: F401
-from .mapping import GlobalCloudMapping, PointCloudMapping  # noqa: F401
+from .mapping import GlobalCloudMapping, PointCloudMapping, SemanticClusters  # noqa: F401
 from .vocabulary import ORBVocabulary  # noqa: F401
 from .keyframedb import KeyFrameDatabase  # noqa: F401
 

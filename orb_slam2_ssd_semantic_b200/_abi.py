@@ -235,3 +235,21 @@ class TriKFView:
 
 class OrbmFrustumPoints(C.Structure):
     _fields_ = [("n", C.c_int), ("xw", vp), ("normal", vp), ("min_dist", vp), ("max_dist", vp)]
+
+
+# T-variant semantic clusters (gcm_add_keyframe_objects)
+GCM_CLUSTER, GCM_BELOW_PROB, GCM_FEW_POINTS = 0, 1, 2
+GCM_OBJECT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("width", "<f4"), ("height", "<f4"), ("class_id", "<i4"),
+                             ("prob", "<f4")])
+
+
+class GcmCluster(C.Structure):
+    _fields_ = [("status", C.c_int32), ("n_band", C.c_int32), ("n_inliers", C.c_int32), ("n_voxels", C.c_int32),
+                ("centroid", C.c_float * 3), ("min_pt", C.c_float * 3), ("max_pt", C.c_float * 3)]
+
+
+def gcm_objects(objects) -> np.ndarray:
+    """Detector boxes -> GcmObject array: a GCM_OBJECT_DTYPE array, or (x, y, width, height, class_id, prob) tuples."""
+    if isinstance(objects, np.ndarray) and objects.dtype == GCM_OBJECT_DTYPE:
+        return np.ascontiguousarray(objects)
+    return np.array([tuple(o) for o in objects], GCM_OBJECT_DTYPE)

@@ -36,6 +36,7 @@ EXPORTS = [
     "orbs_track_batch_u16_masked", "orbs_submit_batch_u16_masked", "orbs_track_batch_masked_device", "orbs_read_dynamic_mask",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
+    "gcm_add_keyframe_objects", "gcm_add_keyframe_objects_device",
     "ocm_default_params", "ocm_create", "ocm_destroy", "ocm_insert_keyframe", "ocm_insert_keyframe_device",
     "ocm_last_points", "ocm_num_leaves", "ocm_export_leaves", "ocm_query", "ocm_sync", "ocm_stream", "ocm_launch_count",
     "ocm_insert_keyframes_labeled_device", "ocm_insert_keyframes_u16_labeled", "ocm_merge_nccl", "ocm_nccl_unique_id",
@@ -167,6 +168,8 @@ def lib() -> C.CDLL:
     L.gcm_destroy.restype = None
     L.gcm_add_keyframe.argtypes = [vp, vp, vp, i, i, vp, f, f, f, f]
     L.gcm_add_keyframe_device.argtypes = [vp, vp, vp, i, i, vp, f, f, f, f]
+    L.gcm_add_keyframe_objects.argtypes = [vp, vp, vp, i, i, vp, f, f, f, f, C.c_longlong, vp, i, vp]
+    L.gcm_add_keyframe_objects_device.argtypes = [vp, vp, vp, i, i, vp, f, f, f, f, C.c_longlong, vp, i, vp]
     L.gcm_refilter.argtypes = [vp]
     L.gcm_size.argtypes = [vp]
     L.gcm_size.restype = C.c_longlong

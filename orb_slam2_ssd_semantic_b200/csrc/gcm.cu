@@ -97,31 +97,35 @@ __global__ void k_gcm_index(const float* __restrict__ xyz, long long n, float in
   }
 }
 
-__global__ void k_gcm_heads(const int* __restrict__ idx_sorted, long long n, uint8_t* __restrict__ head) {
+// Key = int (the map's cell index) or unsigned long long (gcm_sem.cu: box << 32 | cell index, never the sentinel)
+template <class Key>
+__global__ void k_gcm_heads(const Key* __restrict__ idx_sorted, long long n, uint8_t* __restrict__ head) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const int v = idx_sorted[i];
+  const Key v = idx_sorted[i];
   head[i] = (v != GCM_SENTINEL) && (i == 0 || idx_sorted[i - 1] != v);
 }
 
-// one thread per cell: sequential float sums in sorted (= input) order, centroid = sum / count
-__global__ void k_gcm_centroids(const int* __restrict__ idx_sorted, const int* __restrict__ pos_sorted,
+// one thread per cell: sequential float sums in sorted (= input) order, centroid = sum / count (colour only if kRgb)
+template <class Key, bool kRgb>
+__global__ void k_gcm_centroids(const Key* __restrict__ idx_sorted, const int* __restrict__ pos_sorted,
                                 const int* __restrict__ starts, const int* __restrict__ ncells, long long n,
                                 const float* __restrict__ xyz, const uint8_t* __restrict__ rgb,
                                 float* __restrict__ oxyz, uint8_t* __restrict__ orgb) {
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= *ncells) return;
   const int b = starts[u];
-  const int key = idx_sorted[b];
+  const Key key = idx_sorted[b];
   float sx = 0.f, sy = 0.f, sz = 0.f, sr = 0.f, sg = 0.f, sb = 0.f;
   int e = b;
   for (; e < n && idx_sorted[e] == key; ++e) {
     const size_t p = (size_t)pos_sorted[e];
     sx += xyz[p * 3]; sy += xyz[p * 3 + 1]; sz += xyz[p * 3 + 2];
-    sr += (float)rgb[p * 3]; sg += (float)rgb[p * 3 + 1]; sb += (float)rgb[p * 3 + 2];
+    if (kRgb) { sr += (float)rgb[p * 3]; sg += (float)rgb[p * 3 + 1]; sb += (float)rgb[p * 3 + 2]; }
   }
   const float fn = (float)(e - b);
   oxyz[(size_t)u * 3] = sx / fn; oxyz[(size_t)u * 3 + 1] = sy / fn; oxyz[(size_t)u * 3 + 2] = sz / fn;
+  if (!kRgb) return;
   orgb[(size_t)u * 3] = (uint8_t)(sr / fn); orgb[(size_t)u * 3 + 1] = (uint8_t)(sg / fn); orgb[(size_t)u * 3 + 2] = (uint8_t)(sb / fn);
 }
 
@@ -145,6 +149,7 @@ struct gcm {
   uint8_t *d_rgb = nullptr, *d_rgb2 = nullptr;
   DeviceBlock sort;           // gcm_refilter's sort of the map and its CUB scratch
   DeviceBlock stage;          // gcm_add_keyframe's uploads
+  DeviceBlock sem_pos, sem_pts;   // gcm_add_keyframe_objects: per-position scratch, per-band-point scratch (gcm_sem.cu)
   int reserve(long long need) {
     if (need <= cap) return B200ORB_OK;
     const long long nc = std::max<long long>(need, cap * 2);
@@ -253,7 +258,7 @@ int gcm_refilter(gcm_t* h) {
   k_gcm_index<<<4 * h->sms, 256, 0, st>>>(h->d_xyz, n, inv, h->d_mm, d_idx, d_pos, h->d_flag);
   size_t tb = tmp_bytes;
   B200_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_idx, d_idx2, d_pos, d_pos2, (int)n, 0, 32, st));
-  k_gcm_heads<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_idx2, n, d_head);
+  k_gcm_heads<int><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_idx2, n, d_head);
   tb = tmp_bytes;
   B200_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<int>(0), d_head, d_starts, h->d_flag + 1, (int)n,
                                        st));
@@ -267,7 +272,7 @@ int gcm_refilter(gcm_t* h) {
   }
   const int cells = flag[1];
   if (cells > 0) {
-    k_gcm_centroids<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(d_idx2, d_pos2, d_starts, h->d_flag + 1, n, h->d_xyz,
+    k_gcm_centroids<int, true><<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(d_idx2, d_pos2, d_starts, h->d_flag + 1, n, h->d_xyz,
                                                                     h->d_rgb, h->d_xyz2, h->d_rgb2);
     ++h->launches;
   }

@@ -9,7 +9,7 @@ import os
 import numpy as np
 
 from . import _lib
-from ._abi import OcmMergeStats, OcmParams, ptr
+from ._abi import GCM_CLUSTER, GcmCluster, OcmMergeStats, OcmParams, gcm_objects, ptr
 
 
 class PointCloudMapping:
@@ -236,6 +236,34 @@ class GlobalCloudMapping:
         _lib.check(self._L.gcm_add_keyframe_device(self._h, C.c_void_p(d_depth), C.c_void_p(d_bgr), rows, cols, ptr(T),
                                                    float(fx), float(fy), float(cx), float(cy)))
 
+    def insertKeyFrameObjects(self, Tcw, depth, color_bgr, fx, fy, cx, cy, keyframe_index, objects):
+        """One keyframe of the semantic loop (src/pointcloudmapping.cc:413-485) with the detector's boxes `objects` (a
+        GCM_OBJECT_DTYPE array or (x, y, width, height, class_id, prob) tuples, detector order): paints each box's depth
+        band, appends the painted keyframe's cloud unless keyframe_index is even and there are no boxes, and returns one
+        GcmCluster record per box (gcm_add_keyframe_objects)."""
+        depth = np.ascontiguousarray(depth, np.float32)
+        bgr = np.ascontiguousarray(color_bgr, np.uint8)
+        rows, cols = depth.shape
+        assert bgr.shape == (rows, cols, 3)
+        T = np.ascontiguousarray(Tcw, np.float32).reshape(16)
+        objs = gcm_objects(objects)
+        out = (GcmCluster * max(len(objs), 1))()
+        _lib.check(self._L.gcm_add_keyframe_objects(self._h, ptr(depth), ptr(bgr), rows, cols, ptr(T), float(fx), float(fy),
+                                                    float(cx), float(cy), int(keyframe_index),
+                                                    ptr(objs) if len(objs) else None, len(objs), out))
+        return list(out)[:len(objs)]
+
+    def insert_keyframe_objects_device(self, d_depth: int, d_bgr: int, rows: int, cols: int, Tcw, fx, fy, cx, cy,
+                                       keyframe_index, objects):
+        """insertKeyFrameObjects with depth and colour already in device memory."""
+        T = np.ascontiguousarray(Tcw, np.float32).reshape(16)
+        objs = gcm_objects(objects)
+        out = (GcmCluster * max(len(objs), 1))()
+        _lib.check(self._L.gcm_add_keyframe_objects_device(self._h, C.c_void_p(d_depth), C.c_void_p(d_bgr), rows, cols, ptr(T),
+                                                           float(fx), float(fy), float(cx), float(cy), int(keyframe_index),
+                                                           ptr(objs) if len(objs) else None, len(objs), out))
+        return list(out)[:len(objs)]
+
     def refilter(self):
         _lib.check(self._L.gcm_refilter(self._h))
 
@@ -250,3 +278,40 @@ class GlobalCloudMapping:
         rgb = np.zeros((max(n.value, 1), 3), np.uint8)
         _lib.check(self._L.gcm_export(self._h, ptr(xyz), ptr(rgb), n.value, C.byref(n)))
         return xyz[:n.value], rgb[:n.value]
+
+
+class SemanticClusters:
+    """The cluster database of the T variant (PointCloudMapping::clusters, sem_merge, src/pointcloudmapping.cc:246-322)
+    over named records.  Each cluster is a dict: object_name, class_id, prob (float32), centroid / minPt / maxPt
+    (float32[3]).  merge() takes a gcm_add_keyframe_objects record with status GCM_CLUSTER and the detector's name."""
+
+    OBJ_SIZE = np.full(21, 0.6, np.float32)    # obj_size_ (:62-70): metres within which two clusters are one object
+    OBJ_SIZE[5], OBJ_SIZE[9], OBJ_SIZE[15], OBJ_SIZE[20] = np.float32(0.06), np.float32(0.5), np.float32(0.35), np.float32(0.25)
+
+    def __init__(self):
+        self.clusters = []
+
+    def merge_record(self, name: str, class_id: int, prob, rec):
+        assert rec.status == GCM_CLUSTER
+        self.merge(name, class_id, prob, np.array(rec.centroid, np.float32), np.array(rec.min_pt, np.float32),
+                   np.array(rec.max_pt, np.float32))
+
+    def merge(self, name, class_id, prob, centroid, min_pt, max_pt):
+        f = np.float32
+        c = dict(object_name=name, class_id=int(class_id), prob=f(prob), centroid=np.asarray(centroid, f).copy(),
+                 minPt=np.asarray(min_pt, f).copy(), maxPt=np.asarray(max_pt, f).copy())
+        best, center_distance = None, f(100)
+        for x in self.clusters:                          # every cluster with the same name, in database order
+            if x["object_name"] != name:
+                continue
+            d = c["centroid"] - x["centroid"]            # Eigen norm(): float squares summed left to right, float sqrt
+            dist = np.sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2], dtype=f)
+            if dist < center_distance:
+                center_distance, best = dist, x
+        if best is not None and center_distance < self.OBJ_SIZE[c["class_id"]]:
+            best["prob"] = f(np.float64(f(best["prob"] + c["prob"])) / 2.0)
+            best["centroid"] = (best["centroid"] + c["centroid"]) / f(2.0)
+            best["minPt"] = np.where(best["minPt"] > c["minPt"], c["minPt"], best["minPt"])
+            best["maxPt"] = np.where(best["maxPt"] > c["maxPt"], c["maxPt"], best["maxPt"])   # the min of the maxima (:308-310)
+        else:
+            self.clusters.append(c)
