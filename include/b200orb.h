@@ -403,6 +403,22 @@ int dynm_filter_keypoints(dynm_t* h, const uint8_t* mask, int rows, int cols, si
  * masks [nframes][rows][cols]; filtered in place, asynchronous on the handle's stream */
 int dynm_filter_keypoints_batch_device(dynm_t* h, const uint8_t* d_mask, int nframes, int rows, int cols, OrbxKeyPoint* d_kps,
                                        uint8_t* d_desc, int32_t* d_counts, int cap);
+/* The dense optical flow of ComputeMask on the device (perfect/src/Flow.cc:26,29): pyrDown of the u8 gray image to
+ * Size(cols / 2, rows / 2), then calcOpticalFlowFarneback(prev, cur, flow, 0.5, 3, 15, 3, 5, 1.2, 0) of the previous and
+ * current half-resolution images, bit for bit as OpenCV 4.13 computes it at its baseline dispatch level
+ * (cv::setUseOptimized(false): SSE2/SSE3 code, no FMA, no IPP; with AVX2/FMA dispatch OpenCV's own result differs in
+ * the last bits).  Both half-resolution sides must lie in [16, 2048]; other sizes return B200ORB_EINVAL.
+ *
+ * dynm_farneback: exactly the call at Flow.cc:29 with its fixed arguments.  prev, cur: rows x cols u8 (continuous,
+ * half resolution); flow: rows x cols x 2 f32 (CV_32FC2).  Host buffers, synchronous. */
+int dynm_farneback(dynm_t* h, const uint8_t* prev, const uint8_t* cur, int rows, int cols, float* flow);
+/* Flow.cc:26-29 for nframes consecutive full-resolution gray images d_gray[n][rows][cols] u8 in HBM: pyrDown of each, then
+ * the flow from frame t-1 to frame t into d_flow[t][rows / 2][cols / 2][2] f32 -- the layout
+ * orbs_track_batch_masked_device takes.  d_prev is the frame before d_gray[0] (rows x cols u8 in HBM); NULL: the sequence
+ * starts at d_gray[0], whose flow is the zero field (the reference's first-frame `mask = ones`).  Asynchronous on the
+ * handle's stream; the scratch grows with min(nframes, 64) frames of the geometry (about 7 MB per frame at 640 x 480). */
+int dynm_flow_batch_device(dynm_t* h, const uint8_t* d_gray, const uint8_t* d_prev, int nframes, int rows, int cols,
+                           float* d_flow);
 
 /* ------------------------------------------------------------------------------------------------
  * Stream pipeline (batched many-frame mode of north_star): per frame t of a batch, what
@@ -486,6 +502,19 @@ int orbs_track_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* 
 int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
                                  const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
                                  uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
+/* Masked batches whose flow the device computes (perfect/src/Flow.cc:26-29, as dynm_flow_batch_device) from the gray
+ * images these entries upload anyway: the same arguments and outputs as the _masked pair, with prev_gray -- the rows x
+ * cols u8 frame before gray[0], page-locked for the submit form -- in place of flow.  prev_gray NULL: the sequence starts
+ * at gray[0], which takes the zero field.  Nothing but prev_gray is uploaded beyond what orbs_track_batch_u16 uploads.
+ * The predecessor is an argument rather than handle state, so two handles chained with orbs_chain_after can carry one
+ * sequence: each batch passes the last gray frame of the batch before.  Sizes dynm_flow_batch_device rejects return
+ * B200ORB_EINVAL before anything is enqueued. */
+int orbs_track_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                              const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                              uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
+int orbs_submit_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                               const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                               uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
 /* Device-resident form (as orbs_track_batch_device), d_flow in HBM. */
 int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,
                                    float binary_threshold, int nframes, int rows, int cols);

@@ -34,6 +34,7 @@ EXPORTS = [
     "orbv_db_launch_count",
     "orbs_create", "orbs_destroy", "orbs_track_batch", "orbs_track_batch_u16", "orbs_submit_batch_u16", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_track_batch_device", "orbs_device_results", "orbs_read_frame_glue", "orbs_sync",
     "orbs_track_batch_u16_masked", "orbs_submit_batch_u16_masked", "orbs_track_batch_masked_device", "orbs_read_dynamic_mask",
+    "orbs_track_batch_u16_flow", "orbs_submit_batch_u16_flow",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
     "gcm_add_keyframe_objects", "gcm_add_keyframe_objects_device",
@@ -44,6 +45,7 @@ EXPORTS = [
     "ocm_tree_build", "ocm_write_ot", "ocm_tree_leaves", "ocm_save_ot", "ocm_read_ot", "ocm_load_ot", "ocm_ot_leaves",
     "dynm_create", "dynm_destroy", "dynm_launch_count", "dynm_stream", "dynm_sync", "dynm_element", "dynm_mask_from_flow",
     "dynm_mask_from_flow_batch_device", "dynm_filter_keypoints", "dynm_filter_keypoints_batch_device",
+    "dynm_farneback", "dynm_flow_batch_device",
 ]
 
 
@@ -135,6 +137,8 @@ def lib() -> C.CDLL:
     L.dynm_mask_from_flow_batch_device.argtypes = [vp, vp, i, i, i, C.c_float, vp, i, i]
     L.dynm_filter_keypoints.argtypes = [vp, vp, i, i, sz, vp, vp, i, C.POINTER(i)]
     L.dynm_filter_keypoints_batch_device.argtypes = [vp, vp, i, i, i, vp, vp, vp, i]
+    L.dynm_farneback.argtypes = [vp, vp, vp, i, i, vp]
+    L.dynm_flow_batch_device.argtypes = [vp, vp, vp, i, i, i, vp]
     L.orbs_create.argtypes = [C.POINTER(OrbsParams), i, C.POINTER(vp)]
     L.orbs_destroy.argtypes = [vp]
     L.orbs_destroy.restype = None
@@ -148,6 +152,8 @@ def lib() -> C.CDLL:
     L.orbs_read_frame_glue.argtypes = [vp, i, vp, vp, vp, vp, i]
     L.orbs_track_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
     L.orbs_submit_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
+    L.orbs_track_batch_u16_flow.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
+    L.orbs_submit_batch_u16_flow.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
     L.orbs_track_batch_masked_device.argtypes = [vp, vp, vp, vp, vp, C.c_float, i, i, i]
     L.orbs_read_dynamic_mask.argtypes = [vp, i, vp, C.POINTER(i)]
     L.orbs_sync.argtypes = [vp]

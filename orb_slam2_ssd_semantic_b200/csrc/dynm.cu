@@ -4,8 +4,8 @@
 //     element;
 //   * the masked RGB-D Frame constructor (perfect/src/Frame.cc:356-377): when more than 65 % of the mask is 1, keypoints
 //     whose pixel is not 1 are dropped (with their descriptors), order kept.
-// The dense optical flow itself (OpenCV's Farneback) stays on the host side of the boundary: its float accumulation
-// order is OpenCV's SIMD code and cannot be restated bit for bit.  Everything here can: cv::pyrUp's float sequence
+// The dense optical flow itself (pyrDown + OpenCV's Farneback) is flow.cu's, behind dynm_farneback and
+// dynm_flow_batch_device below.  Everything here is bit-exact with cv2 too: cv::pyrUp's float sequence
 // (row pass: x*6 + left + right / (x + right)*4, reflect-101 on the left / top, replicate on the right / bottom; column
 // pass the same, times 1/64) and cv::erode / cv::dilate with the default border (outside pixels are ignored) were pinned
 // against cv2 4.13 (tools/make_dynmask_golden.py -> tests/golden/dynmask_*.npz).
@@ -229,6 +229,36 @@ int dynm_filter_keypoints(dynm_t* h, const uint8_t* mask, int rows, int cols, si
   B200_CUDA(cudaStreamSynchronize(h->stream));
   *n_out = m;
   return B200ORB_OK;
+}
+
+int dynm_farneback(dynm_t* h, const uint8_t* prev, const uint8_t* cur, int rows, int cols, float* flow) {
+  if (!h || !prev || !cur || !flow) { set_error("bad argument"); return B200ORB_EINVAL; }
+  FbGeom g;
+  B200_CHECK(fb_geometry(rows, cols, &g));
+  DeviceGuard dg(h->device);
+  const size_t px = (size_t)rows * cols;
+  FbScratch s;
+  float* d_out;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) { fb_take(t, s, g, 1); d_out = t.take<float>(px * 2); }));
+  B200_CUDA(cudaMemcpyAsync(s.half, prev, px, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(s.half + px, cur, px, cudaMemcpyHostToDevice, h->stream));
+  B200_CHECK(fb_pairs(h->stream, g, s, 2, d_out, &h->launches));
+  B200_CUDA(cudaMemcpyAsync(flow, d_out, px * 2 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200ORB_OK;
+}
+
+int dynm_flow_batch_device(dynm_t* h, const uint8_t* d_gray, const uint8_t* d_prev, int nframes, int rows, int cols,
+                           float* d_flow) {
+  if (!h || nframes < 0 || (nframes > 0 && (!d_gray || !d_flow))) { set_error("bad argument"); return B200ORB_EINVAL; }
+  FbGeom g;
+  B200_CHECK(fb_geometry(rows / 2, cols / 2, &g));
+  if (nframes == 0) return B200ORB_OK;
+  DeviceGuard dg(h->device);
+  const int C = std::min(nframes, FB_CHUNK);
+  FbScratch s;
+  B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) { fb_take(t, s, g, C); }));
+  return fb_batch(h->stream, g, s, C, d_gray, d_prev, nframes, rows, cols, d_flow, &h->launches);
 }
 
 }  // extern "C"

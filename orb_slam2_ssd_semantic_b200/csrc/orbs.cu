@@ -151,6 +151,9 @@ struct orbs {
   uint32_t* d_plane = nullptr;   // [maxF][rows][ceil(cols / 32)]
   unsigned* d_msum = nullptr;    // [maxF]
   float* d_flow = nullptr;       // [maxF][rows / 2][cols / 2][2]
+  uint8_t* d_prev_gray = nullptr;   // the _flow entries' prev_gray
+  FbGeom fbg;                       // and their Farneback geometry and scratch (chunks of min(maxF, FB_CHUNK) frames)
+  FbScratch fbs{};
   bool masked = false;           // the running batch went through mask_filter
   int mask_F = 0;                // frames of the last batch that carry a dynamic mask (0: it was not masked)
   bool have = false;
@@ -205,12 +208,21 @@ struct orbs {
     }
     return B200ORB_OK;
   }
-  int ensure_dyn(bool host_flow) {
-    const size_t planes = (size_t)maxF * rows * dynp_words(cols), flow = host_flow ? (size_t)maxF * (rows / 2) * (cols / 2) * 2 : 0;
+  // host_flow: d_flow receives the caller's flow; dev_flow: the device computes it there (and needs the Farneback scratch)
+  int ensure_dyn(bool host_flow, bool dev_flow = false) {
+    const size_t planes = (size_t)maxF * rows * dynp_words(cols);
+    const size_t flow = host_flow || dev_flow ? (size_t)maxF * (rows / 2) * (cols / 2) * 2 : 0;
+    if (dev_flow) B200_CHECK(fb_geometry(rows / 2, cols / 2, &fbg));
     return dyn.reserve(ex->stream, [&](Carver& t) {
       d_plane = t.take<uint32_t>(planes); d_msum = t.take<unsigned>(maxF); d_flow = t.take<float>(flow);
+      d_prev_gray = nullptr;
+      if (dev_flow) {
+        d_prev_gray = t.take<uint8_t>((size_t)rows * cols);
+        fb_take(t, fbs, fbg, fb_chunk());
+      }
     });
   }
+  int fb_chunk() const { return std::min(maxF, FB_CHUNK); }
   // Flow::ComputeMask + the masked Frame constructor's keypoint filter (perfect/src/Flow.cc:24-47, perfect/src/Frame.cc:
   // 356-377) on the F frames the extractor has just run, in place; kpd16 (the CV_16U depth under the keypoints) moves with
   // them.  dflow: [F][rows / 2][cols / 2][2] f32.
@@ -340,13 +352,18 @@ static int orbs_after_select(void* ctx, int f0, int F) {
 static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, const uint16_t* depth16, float factor,
                             const float* Tcw, int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc,
                             int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap, bool wait = true,
-                            const float* flow = nullptr, float thr = 0.f) {
+                            const float* flow = nullptr, float thr = 0.f, bool dev_flow = false,
+                            const uint8_t* prev_gray = nullptr) {
   if (!h || !gray || (!depth && !depth16) || !Tcw || !kps || !desc || !nkp || !cur2last || !nmatch || nframes <= 0 ||
       rows <= 0 || cols <= 0) {
     set_error("bad argument");
     return B200ORB_EINVAL;
   }
-  if (flow) B200_CHECK(h->check_masked(rows, cols));
+  if (flow || dev_flow) B200_CHECK(h->check_masked(rows, cols));
+  if (dev_flow) {
+    FbGeom fg;
+    B200_CHECK(fb_geometry(rows / 2, cols / 2, &fg));
+  }
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
@@ -366,7 +383,7 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
   const char* depth_up = depth ? (const char*)depth : (const char*)depth16;
   B200_CHECK(h->ensure(rows, cols, nframes, depth_bytes));
   if (cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", cap, h->cap); return B200ORB_ECAP; }
-  if (flow) B200_CHECK(h->ensure_dyn(true));
+  if (flow || dev_flow) B200_CHECK(h->ensure_dyn(flow != nullptr, dev_flow));
   cudaStream_t st = h->ex->stream;
   const size_t px = (size_t)rows * cols, F = nframes, fpx = (size_t)(rows / 2) * (cols / 2) * 2;
   // the inputs go up in chunks on a copy stream while the extractor already works on the chunks that have arrived
@@ -388,6 +405,8 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
       B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->chain_prev->gather_ev, 0));
     }
     h->chain_prev = nullptr;
+    if (dev_flow && prev_gray)
+      B200_CUDA(cudaMemcpyAsync(h->d_prev_gray, prev_gray, px, cudaMemcpyHostToDevice, h->copy_stream));
     for (int c = 0; c < nchunk; ++c) {
       const size_t f0 = F * c / nchunk, f1 = F * (c + 1) / nchunk;
       B200_CUDA(cudaMemcpyAsync(h->d_gray + px * f0, gray + px * f0, px * (f1 - f0), cudaMemcpyHostToDevice, h->copy_stream));
@@ -405,7 +424,10 @@ static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, 
   }
   h->ex->after_select = nullptr;
   if (depth16) B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
-  if (flow) B200_CHECK(h->mask_filter(h->d_flow, thr, depth16 ? h->d_kpd16 : nullptr, nframes));
+  if (dev_flow)
+    B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, prev_gray ? h->d_prev_gray : nullptr, nframes, rows, cols,
+                        h->d_flow, &h->launches));
+  if (flow || dev_flow) B200_CHECK(h->mask_filter(h->d_flow, thr, depth16 ? h->d_kpd16 : nullptr, nframes));
   B200_CUDA(cudaMemcpyAsync(h->d_T, Tcw, F * 64, cudaMemcpyHostToDevice, st));
   B200_CHECK(h->run(depth ? static_cast<const float*>(h->d_depth) : nullptr, depth16 ? h->d_kpd16 : nullptr, factor, h->d_T,
                     nframes));
@@ -461,6 +483,20 @@ int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t*
   if (!flow) { set_error("bad argument"); return B200ORB_EINVAL; }
   return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
                           nmatch, cap, /*wait=*/false, flow, binary_threshold);
+}
+
+int orbs_track_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                              const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                              uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
+  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
+                          nmatch, cap, /*wait=*/true, nullptr, binary_threshold, /*dev_flow=*/true, prev_gray);
+}
+
+int orbs_submit_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
+                               const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
+                               uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
+  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
+                          nmatch, cap, /*wait=*/false, nullptr, binary_threshold, /*dev_flow=*/true, prev_gray);
 }
 
 int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,

@@ -2,9 +2,11 @@
 
 `Flow` follows FlowSLAM::Flow (perfect/include/Flow.h:18-37): ComputeMask(GrayImg, BInaryThreshold) keeps the previous
 half-resolution gray image and returns the static / dynamic mask.  The dense optical flow between the two half-resolution
-images is OpenCV's calcOpticalFlowFarneback in the reference (perfect/src/Flow.cc:29) and stays a host callable here
-(`flow_fn(prev, cur) -> rows x cols x 2 float32`, default: cv2's, when cv2 is importable); everything after it -- pyrUp of
-the flow, the threshold loop, erode, erode, dilate -- runs on the GPU (dynm_mask_from_flow).
+images is OpenCV's calcOpticalFlowFarneback in the reference (perfect/src/Flow.cc:29) and is a host callable here
+(`flow_fn(prev, cur) -> rows x cols x 2 float32`, default: cv2's, when cv2 is importable); `DynamicMask.farneback` is the
+same call on the GPU, bit-exact with OpenCV 4.13 at its baseline dispatch level (`Flow(flow_fn=dm.farneback)`).
+Everything after it -- pyrUp of the flow, the threshold loop, erode, erode, dilate -- runs on the GPU
+(dynm_mask_from_flow).
 
 `filter_keypoints` is the keypoint loop of the masked RGB-D Frame constructor (perfect/src/Frame.cc:356-377).
 """
@@ -67,6 +69,31 @@ class DynamicMask:
         _lib.check(self._L.dynm_filter_keypoints(self._h, _p(mask), mask.shape[0], mask.shape[1], mask.strides[0], _p(kps),
                                                  _p(desc), len(kps), C.byref(n)))
         return kps[:n.value].copy(), desc[:n.value].copy()
+
+    def farneback(self, prev: np.ndarray, cur: np.ndarray) -> np.ndarray:
+        """calcOpticalFlowFarneback(prev, cur, None, 0.5, 3, 15, 3, 5, 1.2, 0) of two half-resolution u8 images on the GPU
+        (perfect/src/Flow.cc:29), bit-exact with OpenCV 4.13 at its baseline dispatch level -> rows x cols x 2 float32."""
+        prev = np.ascontiguousarray(prev, np.uint8)
+        cur = np.ascontiguousarray(cur, np.uint8)
+        if prev.ndim != 2 or prev.shape != cur.shape:
+            raise ValueError("prev and cur must be two rows x cols uint8 images of one size")
+        rows, cols = prev.shape
+        flow = np.zeros((rows, cols, 2), np.float32)
+        _lib.check(self._L.dynm_farneback(self._h, _p(prev), _p(cur), rows, cols, _p(flow)))
+        return flow
+
+    def flow_batch_device(self, d_gray: int, d_prev, nframes: int, rows: int, cols: int, d_flow: int):
+        """pyrDown + Farneback (Flow.cc:26-29) of nframes full-resolution u8 frames in HBM (device pointers) into
+        d_flow[nframes][rows/2][cols/2][2] f32; d_prev = the frame before d_gray[0] or None / 0 (frame 0 then takes the
+        zero field).  Asynchronous on this handle's stream (stream())."""
+        _lib.check(self._L.dynm_flow_batch_device(self._h, C.c_void_p(d_gray), C.c_void_p(d_prev or None), int(nframes),
+                                                  int(rows), int(cols), C.c_void_p(d_flow)))
+
+    def stream(self) -> int:
+        return int(self._L.dynm_stream(self._h) or 0)
+
+    def sync(self):
+        _lib.check(self._L.dynm_sync(self._h))
 
     def launch_count(self) -> int:
         return int(self._L.dynm_launch_count(self._h))

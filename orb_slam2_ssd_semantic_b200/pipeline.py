@@ -126,6 +126,49 @@ class StreamTracker:
                                                         ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
         return out
 
+    @staticmethod
+    def _check_prev(prev_gray, rows: int, cols: int):
+        if prev_gray is not None and (prev_gray.dtype != np.uint8 or prev_gray.shape != (rows, cols)):
+            raise ValueError("prev_gray must be a rows x cols uint8 image or None")
+
+    def track_batch_u16_flow(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                             prev_gray=None, binary_threshold: float = 40.0, out=None):
+        """track_batch_u16_masked with the optical flow computed on the device from the gray frames (pyrDown +
+        calcOpticalFlowFarneback, perfect/src/Flow.cc:26-29): prev_gray is the frame before gray[0], None when the
+        sequence starts at gray[0] (its flow is the zero field).  No flow crosses the host link."""
+        gray = np.ascontiguousarray(gray, np.uint8)
+        depth_u16 = np.ascontiguousarray(depth_u16, np.uint16)
+        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
+        F, rows, cols = gray.shape
+        assert depth_u16.shape == gray.shape and Tcw.shape[0] == F
+        if prev_gray is not None:
+            prev_gray = np.ascontiguousarray(prev_gray, np.uint8)
+        self._check_prev(prev_gray, rows, cols)
+        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
+        _lib.check(self._L.orbs_track_batch_u16_flow(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
+                                                     ptr(Tcw), None if prev_gray is None else ptr(prev_gray),
+                                                     float(binary_threshold), F, rows, cols, ptr(kps), ptr(desc), ptr(nkp),
+                                                     ptr(c2l), ptr(nm), self.cap))
+        return kps, desc, nkp, c2l, nm
+
+    def submit_batch_u16_flow(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                              prev_gray, binary_threshold: float, out):
+        """Asynchronous track_batch_u16_flow (as submit_batch_u16): every input, prev_gray included, must be page-locked,
+        C-contiguous and untouched until sync()."""
+        for a, dt in ((gray, np.uint8), (depth_u16, np.uint16), (Tcw, np.float32)) + \
+                (((prev_gray, np.uint8),) if prev_gray is not None else ()):
+            if a.dtype != dt or not a.flags.c_contiguous:
+                raise ValueError("submit_batch_u16_flow takes C-contiguous %s arrays (no hidden copies)" % np.dtype(dt).name)
+        F, rows, cols = gray.shape
+        assert depth_u16.shape == gray.shape and Tcw.size == F * 16
+        self._check_prev(prev_gray, rows, cols)
+        kps, desc, nkp, c2l, nm = out
+        _lib.check(self._L.orbs_submit_batch_u16_flow(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
+                                                      ptr(Tcw), None if prev_gray is None else ptr(prev_gray),
+                                                      float(binary_threshold), F, rows, cols, ptr(kps), ptr(desc), ptr(nkp),
+                                                      ptr(c2l), ptr(nm), self.cap))
+        return out
+
     def track_batch_masked_device(self, d_gray: int, d_depth: int, d_Tcw: int, d_flow: int, binary_threshold: float,
                                   nframes: int, rows: int, cols: int):
         """track_batch_device with the dynamic mask; d_flow = [nframes][rows/2][cols/2][2] f32 in HBM. Asynchronous."""
