@@ -5,7 +5,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B200ORB_LIB: development override (e.g. the clock-instrumented build `make timing` produces)
+# B200ORB_LIB: development override, the path of another build of the library
 _SO = os.environ.get("B200ORB_LIB") or os.path.join(_HERE, "libb200orb.so")
 
 

@@ -15,6 +15,7 @@
 #include <new>
 
 #include "dynm_plane.cuh"
+#include "flow.cuh"
 
 namespace b200 {
 
@@ -90,6 +91,63 @@ __global__ void __launch_bounds__(DYNP_THREADS) k_dynm_filter(const uint8_t* __r
   const bool filter = (double)s > (double)(rows * cols) * 0.65;   // :358
   dynp_compact(f, n, cap, rows, cols, kps, desc, nullptr, counts, ws,
                [&](int y, int x) { return !filter || m[(size_t)y * cols + x] == 1; });
+}
+
+// One CTA per frame f of a batch, after extraction: threshold into plane A, erode, erode, dilate between A and B; the final
+// plane also goes to planes[f] (H x NW words) and its popcount, cv::sum(mask), to sums[f]; then the masked constructor's
+// filter, in place on the extractor's outputs.
+__global__ void __launch_bounds__(DYNP_THREADS, 2) k_dynm_plane_filter(const float* __restrict__ flow, int h, int w, float thr,
+                                                                     int H, int W, uint32_t* __restrict__ planes,
+                                                                     unsigned* __restrict__ sums, OrbxKeyPoint* __restrict__ kps,
+                                                                     uint8_t* __restrict__ desc, uint16_t* __restrict__ kpd16,
+                                                                     int* __restrict__ counts, int cap) {
+  extern __shared__ uint32_t dynp_sm[];
+  const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int nw = dynp_words(W), nwords = H * nw;
+  uint32_t* A = dynp_sm;
+  uint32_t* B = dynp_sm + nwords;
+  int* ws = reinterpret_cast<int*>(dynp_sm + 2 * nwords);
+  const uint32_t last = dynp_last(W);
+  const int n = min(counts[f], cap);
+  const float* fl = flow + (size_t)f * h * w * 2;
+  for (int it = tid >> 5; it < nwords; it += DYNP_THREADS / 32) {
+    const int Y = it / nw, X = (it - Y * nw) * 32 + lane;
+    const uint32_t bits = __ballot_sync(0xffffffffu, dynp_threshold(fl, h, w, thr, X, Y, W));
+    if (lane == 0) A[it] = bits;
+  }
+  __syncthreads();
+  plane_morph<true, true>(A, B, H, nw, last, nullptr);
+  __syncthreads();
+  plane_morph<true, false>(B, A, H, nw, last, nullptr);
+  __syncthreads();
+  const unsigned pop = plane_morph<false, false>(A, B, H, nw, last, planes + (size_t)f * nwords);
+  int total;
+  block_excl_scan((int)pop, ws, &total);   // its barriers also publish B
+  if (tid == 0) sums[f] = (unsigned)total;
+  const bool filter = (double)total > (double)(H * W) * 0.65;   // perfect/src/Frame.cc:358
+  dynp_compact(f, n, cap, H, W, kps, desc, kpd16, counts, ws,
+               [&](int y, int x) { return !filter || ((B[y * nw + (x >> 5)] >> (x & 31)) & 1u); });
+}
+
+int launch_dynm_plane_filter(int F, const float* flow, int h, int w, float thr, int H, int W, uint32_t* planes, unsigned* sums,
+                             OrbxKeyPoint* kps, uint8_t* desc, uint16_t* kpd16, int* counts, int cap, cudaStream_t stream,
+                             long long* launches) {
+  const size_t smem = dynp_smem_bytes(H, W);
+  B200_CUDA(cudaFuncSetAttribute(k_dynm_plane_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_dynm_plane_filter<<<F, DYNP_THREADS, smem, stream>>>(flow, h, w, thr, H, W, planes, sums, kps, desc, kpd16, counts, cap);
+  ++*launches;
+  B200_CUDA(cudaGetLastError());
+  return B200ORB_OK;
+}
+
+int dynm_check_geometry(int rows, int cols, int mask_rows, int mask_cols) {
+  if (rows < 2 || cols < 2) { set_error("flow field smaller than 2x2"); return B200ORB_EINVAL; }
+  if (mask_rows < 2 * rows || mask_rows > 2 * rows + 1 || mask_cols < 2 * cols || mask_cols > 2 * cols + 1) {
+    set_error("mask %dx%d does not belong to a %dx%d flow field (the gray image is 2 rows (+1) x 2 cols (+1))", mask_cols,
+              mask_rows, cols, rows);
+    return B200ORB_EINVAL;
+  }
+  return B200ORB_OK;
 }
 
 }  // namespace b200

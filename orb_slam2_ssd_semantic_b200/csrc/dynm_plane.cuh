@@ -1,8 +1,8 @@
 // dynm_plane.cuh -- Flow::ComputeMask + the masked RGB-D Frame constructor's keypoint loop (perfect/src/Flow.cc:24-47,
 // perfect/src/Frame.cc:356-377) on bit planes: the stages as device functions of one mask word or one chunk of keypoints,
-// whoever drives them.  Two drivers: k_dynm_plane_filter below (the batch tracker, orbs.cu, between extraction and the
-// frame glue: one CTA per frame, both planes in shared memory) and the per-stage dynm_* entries (dynm.cu: grid-wide
-// launches over planes in global memory).
+// whoever drives them.  Two drivers, both in dynm.cu: k_dynm_plane_filter (the batch tracker, orbs.cu, launches it through
+// launch_dynm_plane_filter below between extraction and the frame glue: one CTA per frame, both planes in shared memory)
+// and the per-stage dynm_* entries (grid-wide launches over planes in global memory).
 #pragma once
 #include "common.cuh"
 
@@ -36,15 +36,8 @@ __device__ __forceinline__ float pyrup_at(const float* __restrict__ src, int X, 
   return __fmul_rn(__fmul_rn(__fadd_rn(r1, r2), 4.f), 0.015625f);
 }
 
-static int dynm_check_geometry(int rows, int cols, int mask_rows, int mask_cols) {
-  if (rows < 2 || cols < 2) { set_error("flow field smaller than 2x2"); return B200ORB_EINVAL; }
-  if (mask_rows < 2 * rows || mask_rows > 2 * rows + 1 || mask_cols < 2 * cols || mask_cols > 2 * cols + 1) {
-    set_error("mask %dx%d does not belong to a %dx%d flow field (the gray image is 2 rows (+1) x 2 cols (+1))", mask_cols,
-              mask_rows, cols, rows);
-    return B200ORB_EINVAL;
-  }
-  return B200ORB_OK;
-}
+// EINVAL (with a message) unless the flow field is at least 2 x 2 and the mask_rows x mask_cols mask belongs to it.
+int dynm_check_geometry(int rows, int cols, int mask_rows, int mask_cols);
 
 // ---- bit planes ------------------------------------------------------------------------------------------------------
 // A mask of H x W pixels is H rows of NW = ceil(W / 32) words; bit j of word k of a row is pixel 32 k + j.  `last` masks
@@ -182,40 +175,13 @@ __device__ __forceinline__ unsigned plane_morph(const uint32_t* __restrict__ src
   return pop;
 }
 
-// One CTA per frame f of a batch, after extraction: threshold into plane A, erode, erode, dilate between A and B; the final
-// plane also goes to planes[f] (H x NW words) and its popcount, cv::sum(mask), to sums[f]; then the masked constructor's
-// filter, in place on the extractor's outputs.
-__global__ void __launch_bounds__(DYNP_THREADS, 2) k_dynm_plane_filter(const float* __restrict__ flow, int h, int w, float thr,
-                                                                     int H, int W, uint32_t* __restrict__ planes,
-                                                                     unsigned* __restrict__ sums, OrbxKeyPoint* __restrict__ kps,
-                                                                     uint8_t* __restrict__ desc, uint16_t* __restrict__ kpd16,
-                                                                     int* __restrict__ counts, int cap) {
-  extern __shared__ uint32_t dynp_sm[];
-  const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
-  const int nw = dynp_words(W), nwords = H * nw;
-  uint32_t* A = dynp_sm;
-  uint32_t* B = dynp_sm + nwords;
-  int* ws = reinterpret_cast<int*>(dynp_sm + 2 * nwords);
-  const uint32_t last = dynp_last(W);
-  const int n = min(counts[f], cap);
-  const float* fl = flow + (size_t)f * h * w * 2;
-  for (int it = tid >> 5; it < nwords; it += DYNP_THREADS / 32) {
-    const int Y = it / nw, X = (it - Y * nw) * 32 + lane;
-    const uint32_t bits = __ballot_sync(0xffffffffu, dynp_threshold(fl, h, w, thr, X, Y, W));
-    if (lane == 0) A[it] = bits;
-  }
-  __syncthreads();
-  plane_morph<true, true>(A, B, H, nw, last, nullptr);
-  __syncthreads();
-  plane_morph<true, false>(B, A, H, nw, last, nullptr);
-  __syncthreads();
-  const unsigned pop = plane_morph<false, false>(A, B, H, nw, last, planes + (size_t)f * nwords);
-  int total;
-  block_excl_scan((int)pop, ws, &total);   // its barriers also publish B
-  if (tid == 0) sums[f] = (unsigned)total;
-  const bool filter = (double)total > (double)(H * W) * 0.65;   // perfect/src/Frame.cc:358
-  dynp_compact(f, n, cap, H, W, kps, desc, kpd16, counts, ws,
-               [&](int y, int x) { return !filter || ((B[y * nw + (x >> 5)] >> (x & 31)) & 1u); });
-}
+// One CTA per frame f of F frames of a batch, after extraction (k_dynm_plane_filter, dynm.cu): threshold, erode, erode,
+// dilate of the half-resolution flow [F][h][w][2] into two bit planes in shared memory; the final plane goes to planes[f]
+// (H x dynp_words(W) words) and its popcount, cv::sum(mask), to sums[f]; then the masked constructor's filter, in place on
+// the extractor's [F][cap] outputs (kps, desc, counts and, when given, kpd16).  Sets the kernel's dynamic shared memory
+// to dynp_smem_bytes(H, W), which the caller has checked against the device.
+int launch_dynm_plane_filter(int F, const float* flow, int h, int w, float thr, int H, int W, uint32_t* planes, unsigned* sums,
+                             OrbxKeyPoint* kps, uint8_t* desc, uint16_t* kpd16, int* counts, int cap, cudaStream_t stream,
+                             long long* launches);
 
 }  // namespace b200

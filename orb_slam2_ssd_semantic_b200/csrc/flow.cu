@@ -13,17 +13,15 @@
 // sweep followed by a full update is the same computation.
 #include <cmath>
 
-#include "common.cuh"
+#include "flow.cuh"
 
 namespace b200 {
 
 constexpr int FB_N = 5;                 // poly_n
 constexpr int FB_M = 7;                 // winsize 15 / 2
-constexpr int FB_LEVELS = 3;
 constexpr int FB_MIN_LEVEL = 32;        // optflowgf.cpp's min_size: a level is added while both sides stay >= 32
 constexpr int FB_MIN_SIDE = 16;         // half-resolution sides the kernels accept (>= 2 x the 5-pixel border band)
 constexpr int FB_MAX_SIDE = 2048;
-constexpr int FB_CHUNK = 64;            // frames per pass through the scratch buffers
 
 // Level blur kernels: cv::getGaussianKernel(ksize, sigma, CV_32F) at sigma = (1/scale - 1)/2, ksize = max(cvRound(5 sigma)
 // | 1, 3) for scales 1, 1/2, 1/4, 1/8.  OpenCV evaluates them with its soft-float exp; these are its float results.
@@ -103,13 +101,7 @@ static FbTables fb_tables() {
   return T;
 }
 
-// Pyramid geometry of a half-resolution rows x cols pair: top = the coarsest level index, h[k] x w[k] = cvRound(side *
-// 0.5^k) (half to even).
-struct FbGeom {
-  int H = 0, W = 0, top = 0;
-  int h[FB_LEVELS + 1] = {}, w[FB_LEVELS + 1] = {};
-};
-static int fb_geometry(int H, int W, FbGeom* g) {
+int fb_geometry(int H, int W, FbGeom* g) {
   if (H < FB_MIN_SIDE || W < FB_MIN_SIDE || H > FB_MAX_SIDE || W > FB_MAX_SIDE) {
     set_error("dense flow of %dx%d half-resolution images: both sides must lie in [%d, %d]", W, H, FB_MIN_SIDE, FB_MAX_SIDE);
     return B200ORB_EINVAL;
@@ -130,18 +122,7 @@ static int fb_geometry(int H, int W, FbGeom* g) {
   return B200ORB_OK;
 }
 
-// Scratch of one chunk of up to C pairs (C + 1 images) of H x W half-resolution images.
-struct FbScratch {
-  uint8_t* half;   // [C + 1][H][W] u8
-  float* tmp;      // [C + 1][H][W] row pass of the blur
-  float* blur;     // [C + 1][H][W]
-  float* img;      // [C + 1][h1][w1] the blurred image at level k >= 1
-  float* R;        // [C + 1][H][W][5] polynomial expansions
-  float* M;        // [C][H][W][5] the matrices of FarnebackUpdateMatrices
-  double* V;       // [C][H][W][5] the running column sums of each row
-  float* fl[2];    // [C][h1][w1][2] flow of levels >= 1, ping-pong
-};
-static void fb_take(Carver& t, FbScratch& s, const FbGeom& g, int C) {
+void fb_take(Carver& t, FbScratch& s, const FbGeom& g, int C) {
   const size_t px = (size_t)g.H * g.W, px1 = g.top ? (size_t)g.h[1] * g.w[1] : 1, I = (size_t)C + 1;
   s.half = t.take<uint8_t>(I * px);
   s.tmp = t.take<float>(I * px);
@@ -419,8 +400,7 @@ __global__ void __launch_bounds__(128) k_fb_hsolve(const double* __restrict__ V,
 
 static inline unsigned fb_blocks(size_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
-// Farneback of the nimg - 1 consecutive pairs of the half-resolution images in s.half -> out [nimg - 1][H][W][2].
-static int fb_pairs(cudaStream_t st, const FbGeom& g, const FbScratch& s, int nimg, float* out, long long* launches) {
+int fb_pairs(cudaStream_t st, const FbGeom& g, const FbScratch& s, int nimg, float* out, long long* launches) {
   static const FbTables T = fb_tables();
   const int P = nimg - 1, H = g.H, W = g.W;
   const size_t px = (size_t)H * W;
@@ -467,10 +447,8 @@ static int fb_pairs(cudaStream_t st, const FbGeom& g, const FbScratch& s, int ni
   return B200ORB_OK;
 }
 
-// Flow::ComputeMask's pyrDown + Farneback for n full-resolution frames in HBM (SH x SW each): out[t] is the flow from
-// frame t-1 to frame t, where frame -1 is `d_prev`; without it out[0] is the zero field.  Chunks of at most C frames.
-static int fb_batch(cudaStream_t st, const FbGeom& g, const FbScratch& s, int C, const uint8_t* d_gray, const uint8_t* d_prev,
-                    int n, int SH, int SW, float* out, long long* launches) {
+int fb_batch(cudaStream_t st, const FbGeom& g, const FbScratch& s, int C, const uint8_t* d_gray, const uint8_t* d_prev,
+             int n, int SH, int SW, float* out, long long* launches) {
   const size_t spx = (size_t)SH * SW, fpx = (size_t)g.H * g.W * 2;
   if (!d_prev) B200_CUDA(cudaMemsetAsync(out, 0, fpx * sizeof(float), st));
   for (int f0 = 0; f0 < n; f0 += C) {

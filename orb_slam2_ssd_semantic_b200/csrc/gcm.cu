@@ -13,11 +13,9 @@
 #include <memory>
 #include <new>
 
-#include "common.cuh"
+#include "gcm.cuh"
 
 namespace b200 {
-
-constexpr int GCM_SENTINEL = 0x7fffffff;
 
 __device__ __forceinline__ unsigned f2ord(float f) {   // order-preserving float -> unsigned
   const unsigned u = __float_as_uint(f);
@@ -97,79 +95,20 @@ __global__ void k_gcm_index(const float* __restrict__ xyz, long long n, float in
   }
 }
 
-// Key = int (the map's cell index) or unsigned long long (gcm_sem.cu: box << 32 | cell index, never the sentinel)
-template <class Key>
-__global__ void k_gcm_heads(const Key* __restrict__ idx_sorted, long long n, uint8_t* __restrict__ head) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const Key v = idx_sorted[i];
-  head[i] = (v != GCM_SENTINEL) && (i == 0 || idx_sorted[i - 1] != v);
-}
-
-// one thread per cell: sequential float sums in sorted (= input) order, centroid = sum / count (colour only if kRgb)
-template <class Key, bool kRgb>
-__global__ void k_gcm_centroids(const Key* __restrict__ idx_sorted, const int* __restrict__ pos_sorted,
-                                const int* __restrict__ starts, const int* __restrict__ ncells, long long n,
-                                const float* __restrict__ xyz, const uint8_t* __restrict__ rgb,
-                                float* __restrict__ oxyz, uint8_t* __restrict__ orgb) {
-  const int u = blockIdx.x * blockDim.x + threadIdx.x;
-  if (u >= *ncells) return;
-  const int b = starts[u];
-  const Key key = idx_sorted[b];
-  float sx = 0.f, sy = 0.f, sz = 0.f, sr = 0.f, sg = 0.f, sb = 0.f;
-  int e = b;
-  for (; e < n && idx_sorted[e] == key; ++e) {
-    const size_t p = (size_t)pos_sorted[e];
-    sx += xyz[p * 3]; sy += xyz[p * 3 + 1]; sz += xyz[p * 3 + 2];
-    if (kRgb) { sr += (float)rgb[p * 3]; sg += (float)rgb[p * 3 + 1]; sb += (float)rgb[p * 3 + 2]; }
-  }
-  const float fn = (float)(e - b);
-  oxyz[(size_t)u * 3] = sx / fn; oxyz[(size_t)u * 3 + 1] = sy / fn; oxyz[(size_t)u * 3 + 2] = sz / fn;
-  if (!kRgb) return;
-  orgb[(size_t)u * 3] = (uint8_t)(sr / fn); orgb[(size_t)u * 3 + 1] = (uint8_t)(sg / fn); orgb[(size_t)u * 3 + 2] = (uint8_t)(sb / fn);
+int gcm_backproject(gcm* h, const float* d_depth, const uint8_t* d_bgr, int rows, int cols, float fx, float fy, float cx,
+                    float cy) {
+  const long long npix = (long long)rows * cols;
+  k_gcm_backproject<<<(unsigned)((npix + 255) / 256), 256, 0, h->stream>>>(d_depth, d_bgr, rows, cols, fx, fy, cx, cy, h->d_T,
+                                                                          h->d_xyz + h->n * 3, h->d_rgb + h->n * 3);
+  ++h->launches;
+  B200_CUDA(cudaGetLastError());
+  h->n += npix;
+  return B200ORB_OK;
 }
 
 }  // namespace b200
 
 using namespace b200;
-
-struct gcm {
-  int device = 0;
-  int sms = 1;
-  float leaf = 0.f;
-  Stream stream;
-  long long launches = 0;
-  long long n = 0, cap = 0;   // points in the global map / capacity of the point block
-  DeviceBlock words;
-  unsigned* d_mm = nullptr;
-  int* d_flag = nullptr;      // [0] overflow, [1] number of cells
-  double* d_T = nullptr;      // Rt (9) + ti (3)
-  DeviceBlock points;         // two sets of `cap` points: the map, and gcm_refilter's output
-  float *d_xyz = nullptr, *d_xyz2 = nullptr;
-  uint8_t *d_rgb = nullptr, *d_rgb2 = nullptr;
-  DeviceBlock sort;           // gcm_refilter's sort of the map and its CUB scratch
-  DeviceBlock stage;          // gcm_add_keyframe's uploads
-  DeviceBlock sem_pos, sem_pts;   // gcm_add_keyframe_objects: per-position scratch, per-band-point scratch (gcm_sem.cu)
-  int reserve(long long need) {
-    if (need <= cap) return B200ORB_OK;
-    const long long nc = std::max<long long>(need, cap * 2);
-    DeviceBlock grown;
-    float *xyz, *xyz2;
-    uint8_t *rgb, *rgb2;
-    B200_CHECK(grown.carve(stream, [&](Carver& t) {
-      xyz = t.take<float>(3 * nc); rgb = t.take<uint8_t>(3 * nc); xyz2 = t.take<float>(3 * nc); rgb2 = t.take<uint8_t>(3 * nc);
-    }));
-    if (n > 0) {
-      B200_CUDA(cudaMemcpyAsync(xyz, d_xyz, 12 * n, cudaMemcpyDeviceToDevice, stream));
-      B200_CUDA(cudaMemcpyAsync(rgb, d_rgb, 3 * n, cudaMemcpyDeviceToDevice, stream));
-    }
-    B200_CUDA(cudaStreamSynchronize(stream));
-    points = std::move(grown);
-    d_xyz = xyz; d_rgb = rgb; d_xyz2 = xyz2; d_rgb2 = rgb2;
-    cap = nc;
-    return B200ORB_OK;
-  }
-};
 
 extern "C" {
 
@@ -206,12 +145,7 @@ int gcm_add_keyframe_device(gcm_t* h, const float* d_depth, const uint8_t* d_bgr
   }
   B200_CUDA(cudaMemcpyAsync(h->d_T, RtTi, sizeof(RtTi), cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));   // RtTi is a local; the call is not on a hot path
-  k_gcm_backproject<<<(unsigned)((npix + 255) / 256), 256, 0, h->stream>>>(d_depth, d_bgr, rows, cols, fx, fy, cx, cy, h->d_T,
-                                                                          h->d_xyz + h->n * 3, h->d_rgb + h->n * 3);
-  ++h->launches;
-  B200_CUDA(cudaGetLastError());
-  h->n += npix;
-  return B200ORB_OK;
+  return gcm_backproject(h, d_depth, d_bgr, rows, cols, fx, fy, cx, cy);
 }
 
 int gcm_add_keyframe(gcm_t* h, const float* depth, const uint8_t* bgr, int rows, int cols, const float Tcw[16], float fx,

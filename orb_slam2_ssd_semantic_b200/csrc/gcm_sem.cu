@@ -1,6 +1,6 @@
 // gcm_sem.cu -- the semantic object clusters of PointCloudMapping::viewer (src/pointcloudmapping.cc:399-488) for one
 // keyframe and any number of detector boxes: draw_rect_with_depth_threshold (:197-244) paints each box's depth band and
-// lists its flat indices, generatePointCloud runs on the painted image (gcm.cu's k_gcm_backproject), and every box's
+// lists its flat indices, generatePointCloud runs on the painted image (gcm_backproject, gcm.cu), and every box's
 // band points go through ExtractIndices, StatisticalOutlierRemoval(50, 1.0), VoxelGrid(resolution), compute3DCentroid
 // and getMinMax3D (:443-476).  PCL semantics follow oracle/sem_ref.cpp, which states them.
 //
@@ -11,12 +11,17 @@
 //   per query, candidates tiled in shared memory the 51 smallest squared distances -> mean of the 50 square roots
 //   per box (one thread, sequential double sums) SOR mean / stddev -> threshold
 //   CUB select                                   ordered keep-compaction
-//   per box bounding box, then one stable radix sort of (box << 32 | cell) with gcm.cu's cell heads and float sums
+//   per box bounding box, then one stable radix sort of (box << 32 | cell) with gcm.cuh's cell heads and float sums
 //   per box (one thread)                         centroid (float sums in cell order) and min / max
 // The host syncs twice, to size the per-point buffers and the sort; the call is synchronous like gcm_add_keyframe.
+#include <cub/cub.cuh>
+#include <thrust/iterator/counting_iterator.h>
+
 #include <cfloat>
 #include <cmath>
 #include <vector>
+
+#include "gcm.cuh"
 
 namespace b200 {
 
@@ -358,6 +363,8 @@ static int sem_check_args(const gcm_t* h, const void* depth, const void* bgr, in
 }
 }  // namespace b200
 
+using namespace b200;
+
 extern "C" {
 
 int gcm_add_keyframe_objects_device(gcm_t* h, const float* d_depth, const uint8_t* d_bgr, int rows, int cols,
@@ -424,11 +431,7 @@ int gcm_add_keyframe_objects_device(gcm_t* h, const float* d_depth, const uint8_
     h->launches += 2;
   }
   const long long n0 = h->n;
-  k_gcm_backproject<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(d_depth, B > 0 ? d_paint : d_bgr, rows, cols, fx, fy, cx, cy,
-                                                                    h->d_T, h->d_xyz + n0 * 3, h->d_rgb + n0 * 3);
-  ++h->launches;
-  B200_CUDA(cudaGetLastError());
-  h->n += npix;
+  B200_CHECK(gcm_backproject(h, d_depth, B > 0 ? d_paint : d_bgr, rows, cols, fx, fy, cx, cy));
   if (B == 0) { B200_CUDA(cudaStreamSynchronize(st)); return B200ORB_OK; }
   std::vector<int> bstart(B + 1, 0);
   if (P > 0) {

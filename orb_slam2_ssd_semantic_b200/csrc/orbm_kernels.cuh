@@ -19,7 +19,7 @@
 // A query with more than LCAP candidates is flagged and re-walked inside the resolve (exact, just slower).
 // k_match_last_fused does K7-K10 of one LAST frame pair in one CTA when the pair fits in shared memory.
 #pragma once
-#include "common.cuh"
+#include "orbm_host.h"
 
 namespace b200 {
 
@@ -27,38 +27,11 @@ constexpr int GRID_COLS = ORBM_GRID_COLS, GRID_ROWS = ORBM_GRID_ROWS, GRID_CELLS
 constexpr int LCAP = 64;                 // candidate-list capacity per query
 constexpr unsigned KEY_INF = 0xffffffffu;
 
-struct MatchCam {            // per-call constants (Frame statics + ORBmatcher ctor args)
-  float fx, fy, cx, cy, bf, b;
-  float min_x, max_x, min_y, max_y;
-  float sf[MAX_LEVELS];
-  float th, nnratio;
-  int mono, check_ori, nlevels;
-  int last_obs_default;      // Observations() of query MapPoints when no array is given
-};
-
-struct CurView {             // SoA view of the "current" frames; instance p reads at p*stride
-  const float *x, *y, *ang, *uright;
-  const int* oct;
-  const uint8_t* desc;
-  const int* obs;            // nullable: pre-existing mvpMapPoints state (-1 NULL, else Observations())
-  const int* n;
-  const float* Tcw;          // p*16
-  const int* goff;           // p*(GRID_CELLS+1)
-  const int* gidx;           // p*stride
-  size_t stride;
-};
-
 __device__ __forceinline__ int hamming256(const uint4 a0, const uint4 a1, const uint8_t* b) {
   // generic loads: the candidate descriptors live in shared memory in the fused kernel, in global memory otherwise
   const uint4 b0 = *reinterpret_cast<const uint4*>(b), b1 = *(reinterpret_cast<const uint4*>(b) + 1);
   return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
          __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
-
-// cv::Mat small-matrix gemm row: float accumulation, "+C" added in double (see oracle/match_ref.cpp header)
-__device__ __forceinline__ float gemm3(const float* a, float b0, float b1, float b2, float c) {
-  const float t = __fadd_rn(__fadd_rn(__fmul_rn(a[0], b0), __fmul_rn(a[1], b1)), __fmul_rn(a[2], b2));
-  return __double2float_rn(__dadd_rn((double)t, (double)c));
 }
 
 __device__ __forceinline__ int grid_cell(float x, float y, float min_x, float min_y, float inv_w, float inv_h) {

@@ -9,18 +9,6 @@ namespace b200 {
 
 constexpr int CAND_WARPS = 8;
 
-struct LastView {            // LastFrame side; instance p reads at p*stride
-  const float* xw;
-  const uint8_t* valid;
-  const int* oct;
-  const float* ang;
-  const uint8_t* desc;
-  const int* obs;            // nullable
-  const int* n;
-  const float* Tcw;
-  size_t stride;
-};
-
 struct ListView {            // per query: LCAP entries + count (negative = overflowed, true count = -n)
   unsigned* list;
   int* count;

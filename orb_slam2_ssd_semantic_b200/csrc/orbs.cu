@@ -5,6 +5,7 @@
 #include <new>
 
 #include "dynm_plane.cuh"
+#include "flow.cuh"
 #include "orbm_host.h"
 #include "orbx_host.h"
 
@@ -112,7 +113,7 @@ __global__ void k_fill_i32(int* p, int v, size_t n) {
 }  // namespace b200
 
 // The host-buffer entries upload a batch in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
-constexpr int MAX_CHUNKS = 7;
+static constexpr int MAX_CHUNKS = 7;
 
 struct orbs {
   OrbsParams prm{};
@@ -228,12 +229,8 @@ struct orbs {
   // them.  dflow: [F][rows / 2][cols / 2][2] f32.
   int mask_filter(const float* dflow, float thr, uint16_t* kpd16, int F) {
     if (thr < 40.0f) thr = 40.0f;   // perfect/src/Flow.cc:24
-    const size_t smem = dynp_smem_bytes(rows, cols);
-    B200_CUDA(cudaFuncSetAttribute(k_dynm_plane_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_dynm_plane_filter<<<F, DYNP_THREADS, smem, ex->stream>>>(dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum,
-                                                               ex->d_kps, ex->d_desc, kpd16, ex->d_n, cap);
-    ++launches;
-    B200_CUDA(cudaGetLastError());
+    B200_CHECK(launch_dynm_plane_filter(F, dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum, ex->d_kps, ex->d_desc,
+                                        kpd16, ex->d_n, cap, ex->stream, &launches));
     masked = true;
     return B200ORB_OK;
   }

@@ -11,7 +11,7 @@
 #include <new>
 #include <vector>
 
-#include "orbm_kernels.cuh"
+#include "common.cuh"
 
 namespace b200 {
 

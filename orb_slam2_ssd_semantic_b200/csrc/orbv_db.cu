@@ -25,6 +25,8 @@
 #include <new>
 #include <vector>
 
+#include "common.cuh"
+
 namespace b200 {
 
 struct DbSlot {

@@ -1,7 +1,6 @@
 // orbx.cu -- host side + C-ABI of the ORB extractor (reference: src/ORBextractor.cc,
 // include/ORBextractor.h).  Kernels live in orbx_kernels.cuh.
 #include <cmath>
-#include <cstdarg>
 #include <cstdlib>
 #include <memory>
 #include <new>
@@ -11,30 +10,6 @@
 #include "orbx_host.h"
 
 namespace b200 {
-
-static thread_local char g_err[512] = "";
-void set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-}
-
-int check_device(int device) {
-  int n = 0;
-  cudaError_t e = cudaGetDeviceCount(&n);
-  if (e != cudaSuccess || n == 0) {
-    set_error("no CUDA device available (%s); libb200orb has no CPU fallback",
-              e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
-    cudaGetLastError();
-    return B200ORB_ENOGPU;
-  }
-  if (device < 0 || device >= n) {
-    set_error("device %d out of range (0..%d)", device, n - 1);
-    return B200ORB_EINVAL;
-  }
-  return B200ORB_OK;
-}
 
 static const signed char kPatternHost[1024] = {
 #include "../../include/orb_pattern_31.inc"
@@ -404,14 +379,6 @@ int b200orb_get_tuning(int* exp_mask, int* fast_wpc, int* qt_minblocks) {
   if (fast_wpc) *fast_wpc = FAST_WARPS;
   if (qt_minblocks) *qt_minblocks = QT_MIN_CTAS;
   return B200ORB_OK;
-}
-
-const char* b200orb_last_error(void) { return g_err; }
-const char* b200orb_version(void) { return "b200orb 0.1 (sm_90a)"; }
-int b200orb_device_count(void) {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
-  return n;
 }
 
 int orbx_create(const OrbxParams* p, int device, orbx_t** out) {

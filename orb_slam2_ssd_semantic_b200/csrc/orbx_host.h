@@ -1,10 +1,54 @@
-// orbx_host.h -- definition of the extractor handle (shared by orbx.cu and the stream pipeline orbs.cu).
+// orbx_host.h -- definition of the extractor handle and the types of its tables (shared by orbx.cu and the stream
+// pipeline orbs.cu).  The kernels are orbx_kernels.cuh's.
 #pragma once
 #include <vector>
 
-#include "orbx_kernels.cuh"
+#include "common.cuh"
 
 namespace b200 {
+
+struct PyrView {                 // one image pyramid (raw or blurred) of a batch
+  uint8_t* p[MAX_LEVELS];        // frame 0 of level l
+  size_t fstride[MAX_LEVELS];    // bytes between consecutive frames of level l
+  int pitch[MAX_LEVELS];
+  int w[MAX_LEVELS], h[MAX_LEVELS];
+};
+
+struct CellDesc {                // one FAST cell (src/ORBextractor.cc:798-838)
+  short level;
+  short x0, y0;                  // ROI origin in level coordinates (= iniX, iniY)
+  short rw, rh;                  // ROI size (maxX-iniX, maxY-iniY); detection range is the ROI minus 3 px
+  short pad;
+  int slot_off;                  // offset of this cell's segment inside a frame's cand[]
+};
+
+struct LevelTab {                // per-level constants of the extractor
+  int cell_begin[MAX_LEVELS + 1];   // cells of level l: [cell_begin[l], cell_begin[l+1])
+  int slot_begin[MAX_LEVELS + 1];   // cand slots of level l
+  int nfeat[MAX_LEVELS];            // mnFeaturesPerLevel
+  int sel_off[MAX_LEVELS + 1];      // offset of level l inside a frame's sel[] / capacity
+  int n_ini[MAX_LEVELS];            // DistributeOctTree nIni (:545)
+  int box_h[MAX_LEVELS];            // maxBorderY-minBorderY: height of the initial nodes (:558)
+  float hx[MAX_LEVELS];             // DistributeOctTree hX (:547)
+  float sf[MAX_LEVELS];             // mvScaleFactor
+  float kp_size[MAX_LEVELS];        // (float)(int)(PATCH_SIZE*mvScaleFactor[l]) (:846)
+  int nlevels;
+};
+
+__device__ __forceinline__ unsigned pack_kp(int x, int y, int resp) {
+  return (unsigned)x | ((unsigned)y << 12) | ((unsigned)resp << 24);
+}
+__device__ __forceinline__ int kp_x(unsigned v) { return v & 0xfff; }
+__device__ __forceinline__ int kp_y(unsigned v) { return (v >> 12) & 0xfff; }
+__device__ __forceinline__ int kp_r(unsigned v) { return v >> 24; }
+
+struct OrientTab {
+  int umax[HALF_PATCH_SIZE + 1];
+};
+
+struct BlurTile { short level, x0, y0, pad; };   // one warp-tile of k_blur7_strip: 128 columns x BLS_ROWS rows of one level
+struct BlurEdge { short level, x0, y0, pad; };   // one border column group of k_blur7_edges
+
 enum { ST_RESIZE = 0, ST_FAST, ST_QUADTREE, ST_BLUR, ST_ORIENT_DESC, ST_GLUE, ST_MATCH, ST_COUNT };
 struct StageEvents {
   Event ev[ST_COUNT + 1];   // null: the boundary was not recorded

@@ -13,46 +13,11 @@
 //   sel       per (frame, level): quad-tree survivors in the reference's list order, same packing
 //   kps/desc  per frame: cap x OrbxKeyPoint (28 B) / cap x 32 B, level-major like operator() concatenates
 #pragma once
-#include "common.cuh"
+#include "orbx_host.h"
 #define B200_HD __host__ __device__ __forceinline__
 #include "../../include/glibc_sincosf.h"
 
 namespace b200 {
-
-struct PyrView {                 // one image pyramid (raw or blurred) of a batch
-  uint8_t* p[MAX_LEVELS];        // frame 0 of level l
-  size_t fstride[MAX_LEVELS];    // bytes between consecutive frames of level l
-  int pitch[MAX_LEVELS];
-  int w[MAX_LEVELS], h[MAX_LEVELS];
-};
-
-struct CellDesc {                // one FAST cell (src/ORBextractor.cc:798-838)
-  short level;
-  short x0, y0;                  // ROI origin in level coordinates (= iniX, iniY)
-  short rw, rh;                  // ROI size (maxX-iniX, maxY-iniY); detection range is the ROI minus 3 px
-  short pad;
-  int slot_off;                  // offset of this cell's segment inside a frame's cand[]
-};
-
-struct LevelTab {                // per-level constants of the extractor
-  int cell_begin[MAX_LEVELS + 1];   // cells of level l: [cell_begin[l], cell_begin[l+1])
-  int slot_begin[MAX_LEVELS + 1];   // cand slots of level l
-  int nfeat[MAX_LEVELS];            // mnFeaturesPerLevel
-  int sel_off[MAX_LEVELS + 1];      // offset of level l inside a frame's sel[] / capacity
-  int n_ini[MAX_LEVELS];            // DistributeOctTree nIni (:545)
-  int box_h[MAX_LEVELS];            // maxBorderY-minBorderY: height of the initial nodes (:558)
-  float hx[MAX_LEVELS];             // DistributeOctTree hX (:547)
-  float sf[MAX_LEVELS];             // mvScaleFactor
-  float kp_size[MAX_LEVELS];        // (float)(int)(PATCH_SIZE*mvScaleFactor[l]) (:846)
-  int nlevels;
-};
-
-__device__ __forceinline__ unsigned pack_kp(int x, int y, int resp) {
-  return (unsigned)x | ((unsigned)y << 12) | ((unsigned)resp << 24);
-}
-__device__ __forceinline__ int kp_x(unsigned v) { return v & 0xfff; }
-__device__ __forceinline__ int kp_y(unsigned v) { return (v >> 12) & 0xfff; }
-__device__ __forceinline__ int kp_r(unsigned v) { return v >> 24; }
 
 // ---------------------------------------------------------------------------------------------------
 // K1  pyramid level l from level l-1: cv::resize INTER_LINEAR 8UC1 (SURVEY App. A.2; call site :1134).
@@ -728,10 +693,6 @@ __global__ void __launch_bounds__(QT_THREADS, QT_MIN_CTAS) k_quadtree(LevelTab l
 // K5  orientation (IC_Angle :59-88 on the raw level) + steered BRIEF (computeOrbDescriptor :92-131 on the
 //     blurred level) + final KeyPoint assembly (:846-856, :1104-1110).  One warp per keypoint at a time.
 // ---------------------------------------------------------------------------------------------------
-struct OrientTab {
-  int umax[HALF_PATCH_SIZE + 1];
-};
-
 __device__ __forceinline__ float fast_atan2_deg(float y, float x) {   // cv::fastAtan2, SURVEY App. A.5 (no FMA)
   const float scale = (float)(180.0 / 3.14159265358979323846);
   const float P1 = __fmul_rn(0.9997878412794807f, scale), P3 = __fmul_rn(-0.3258083974640975f, scale),
@@ -958,8 +919,6 @@ __device__ __forceinline__ HRow blur_hrow_border(const uint8_t* __restrict__ row
                          b[8] | (b[9] << 8) | (b[10] << 16) | (b[11] << 24));
 }
 
-struct BlurTile { short level, x0, y0, pad; };   // one warp-tile: 128 columns x BLS_ROWS rows of one level
-
 // All levels in ONE launch (a thread walks 35+6 rows sequentially, so a per-level launch is bounded below by that
 // latency chain; one launch lets the small levels hide inside the big ones).  One warp per tile, blockIdx.y = frame.
 __global__ void __launch_bounds__(32) k_blur7_strip(PyrView src, PyrView dstv, const BlurTile* __restrict__ tiles) {
@@ -1025,8 +984,6 @@ __global__ void __launch_bounds__(32) k_blur7_strip(PyrView src, PyrView dstv, c
 // Border column groups of every level (the group at x0 = 0 and the last one or two groups): same register-ring walk
 // as k_blur7_strip with the horizontal pass fetched through BORDER_REFLECT_101; one thread per (group, 35-row strip).
 // ~3 % of the pixels.
-struct BlurEdge { short level, x0, y0, pad; };
-
 __global__ void __launch_bounds__(64) k_blur7_edges(PyrView src, PyrView dstv, const BlurEdge* __restrict__ edges, int nedges) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nedges) return;

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Attribute the executed instructions of one kernel of an .ncu-rep to CUDA source lines (no GPU needed): SASS page of the
-report + `nvdisasm -g` line info of the cubin inside libb200orb.so.
+report + `nvdisasm -g` line info of the cubin inside libb200orb.so that holds the kernel.
 usage: ncu_lines.py rep.ncu-rep kernel-regex mangled-substring [source-file]"""
 import collections
 import csv
@@ -16,9 +16,14 @@ root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 tmp = tempfile.mkdtemp()
 subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(root, "orb_slam2_ssd_semantic_b200", "libb200orb.so")], cwd=tmp,
                capture_output=True)
-cubin = [f for f in os.listdir(tmp) if f.endswith(".cubin")][0]
-dis = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, cubin)], capture_output=True, text=True).stdout.splitlines()
-start = next(i for i, l in enumerate(dis) if l.startswith(".text.") and mangled in l)
+# one cubin per module of the library: disassemble the one that holds the kernel
+for cubin in sorted(f for f in os.listdir(tmp) if f.endswith(".cubin")):
+    dis = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, cubin)], capture_output=True, text=True).stdout.splitlines()
+    start = next((i for i, l in enumerate(dis) if l.startswith(".text.") and mangled in l), None)
+    if start is not None:
+        break
+else:
+    sys.exit("no cubin of libb200orb.so holds a kernel matching " + mangled)
 cur, off2line = None, {}
 for l in dis[start + 1:]:
     if l.startswith("//-----") and "text." in l:

@@ -13,8 +13,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 out_path = sys.argv[1]
 tmp = tempfile.mkdtemp()
 subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(ROOT, "orb_slam2_ssd_semantic_b200", "libb200orb.so")], cwd=tmp, capture_output=True)
-cubin = max((f for f in os.listdir(tmp) if f.endswith(".cubin")), key=lambda f: os.path.getsize(os.path.join(tmp, f)))
-dis = subprocess.run(["nvdisasm", "-c", os.path.join(tmp, cubin)], capture_output=True, text=True).stdout.splitlines()
+# one cubin per module of the library: the disassembly of all of them, one after the other
+dis = [l for cubin in sorted(f for f in os.listdir(tmp) if f.endswith(".cubin"))
+       for l in subprocess.run(["nvdisasm", "-c", os.path.join(tmp, cubin)], capture_output=True, text=True).stdout.splitlines()]
 kernels = [("k_fast_cells<48>", "k_fast_cellsILi48E"), ("k_orient_desc", "k_orient_descENS"),
            ("k_quadtree", "10k_quadtreeENS"), ("k_match_last_fused", "k_match_last_fused"),
            ("k_blur7_strip", "k_blur7_strip"), ("k_resize_g", "k_resize_g"), ("k_ocm_scan_keys", "k_ocm_scan_keys"),
@@ -27,7 +28,7 @@ for l in dis:
     m = re.match(r"\s+/\*([0-9a-f]{4,})\*/\s+(@!?U?P\d\s+)?(\S+)", l)
     if m:
         tot[m.group(3).split(".")[0].rstrip(";")] += 1
-out.append("# whole cubin: %d instructions.  UTMALDG %d, UTMASTG %d, UTCMMA / tcgen05 %d, HMMA %d, IMMA %d, LDGSTS %d (no TMA, no tensor"
+out.append("# all cubins: %d instructions.  UTMALDG %d, UTMASTG %d, UTCMMA / tcgen05 %d, HMMA %d, IMMA %d, LDGSTS %d (no TMA, no tensor"
            % (sum(tot.values()), tot["UTMALDG"], tot["UTMASTG"], tot["UTCMMA"], tot["HMMA"], tot["IMMA"], tot["LDGSTS"]))
 out.append("# ops: integer / bitwise byte work on 31..43-px tiles at 4-byte alignment, DESIGN.md section 4);  VIMNMX3 %d, VIMNMX %d, POPC %d,"
            % (tot["VIMNMX3"], tot["VIMNMX"], tot["POPC"]))
