@@ -419,6 +419,19 @@ int dynm_farneback(dynm_t* h, const uint8_t* prev, const uint8_t* cur, int rows,
  * handle's stream; the scratch grows with min(nframes, 64) frames of the geometry (about 7 MB per frame at 640 x 480). */
 int dynm_flow_batch_device(dynm_t* h, const uint8_t* d_gray, const uint8_t* d_prev, int nframes, int rows, int cols,
                            float* d_flow);
+/* The homography branch of ComputeMask (perfect/src/Flow.cc:73-80): cv::warpPerspective(GrayImg, dest, Homo,
+ * GrayImg.size()) on the device -- u8, one channel, INTER_LINEAR, BORDER_CONSTANT 0, Homo inverted first (no
+ * WARP_INVERSE_MAP) -- bit for bit as OpenCV 4.13 computes it, at every dispatch level.  H: the forward map as
+ * findHomography returns it, row-major double[9]; a singular H inverts to zeros and, as in OpenCV, every pixel then takes
+ * the value of pixel (0, 0).  Both sides must lie in [1, 32766] (cv::remap asserts < SHRT_MAX); other sizes return
+ * B200ORB_EINVAL before anything is enqueued.
+ *
+ * dynm_warp_perspective: gray, dst: rows x cols u8 (continuous).  Host buffers, synchronous. */
+int dynm_warp_perspective(dynm_t* h, const uint8_t* gray, int rows, int cols, const double* H, uint8_t* dst);
+/* nframes images d_gray[n][rows][cols] u8, each warped by its own d_H[n][9] into d_dst[n][rows][cols] (all in HBM; d_dst
+ * must not overlap d_gray).  At most 65535 frames per call.  Asynchronous on the handle's stream. */
+int dynm_warp_perspective_batch_device(dynm_t* h, const uint8_t* d_gray, int nframes, int rows, int cols, const double* d_H,
+                                       uint8_t* d_dst);
 
 /* ------------------------------------------------------------------------------------------------
  * Stream pipeline (batched many-frame mode of north_star): per frame t of a batch, what

@@ -45,7 +45,7 @@ EXPORTS = [
     "ocm_tree_build", "ocm_write_ot", "ocm_tree_leaves", "ocm_save_ot", "ocm_read_ot", "ocm_load_ot", "ocm_ot_leaves",
     "dynm_create", "dynm_destroy", "dynm_launch_count", "dynm_stream", "dynm_sync", "dynm_element", "dynm_mask_from_flow",
     "dynm_mask_from_flow_batch_device", "dynm_filter_keypoints", "dynm_filter_keypoints_batch_device",
-    "dynm_farneback", "dynm_flow_batch_device",
+    "dynm_farneback", "dynm_flow_batch_device", "dynm_warp_perspective", "dynm_warp_perspective_batch_device",
 ]
 
 
@@ -139,6 +139,8 @@ def lib() -> C.CDLL:
     L.dynm_filter_keypoints_batch_device.argtypes = [vp, vp, i, i, i, vp, vp, vp, i]
     L.dynm_farneback.argtypes = [vp, vp, vp, i, i, vp]
     L.dynm_flow_batch_device.argtypes = [vp, vp, vp, i, i, i, vp]
+    L.dynm_warp_perspective.argtypes = [vp, vp, i, i, vp, vp]
+    L.dynm_warp_perspective_batch_device.argtypes = [vp, vp, i, i, i, vp, vp]
     L.orbs_create.argtypes = [C.POINTER(OrbsParams), i, C.POINTER(vp)]
     L.orbs_destroy.argtypes = [vp]
     L.orbs_destroy.restype = None

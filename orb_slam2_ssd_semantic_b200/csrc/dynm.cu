@@ -14,6 +14,7 @@
 #include <memory>
 #include <new>
 
+#include "dynm.cuh"
 #include "dynm_plane.cuh"
 #include "flow.cuh"
 
@@ -153,13 +154,6 @@ int dynm_check_geometry(int rows, int cols, int mask_rows, int mask_cols) {
 }  // namespace b200
 
 using namespace b200;
-
-struct dynm {
-  int device = 0;
-  Stream stream;
-  long long launches = 0;
-  DeviceBlock buf;   // each entry carves its buffer list out of it
-};
 
 // device core of ComputeMask: d_flow [F][rows][cols][2] -> d_mask [F][H][W]; d_planes = 2 F H ceil(W / 32) words
 static int dynm_mask_core(dynm* h, const float* d_flow, int F, int rows, int cols, float thr, uint8_t* d_mask,

@@ -1,8 +1,11 @@
 // shim/Flow.h -- drop-in for the reference's perfect/include/Flow.h (same guard, same class): FlowSLAM::Flow keeps its
-// interface (ComputeMask x2), its two members and its host-side OpenCV calls for what cannot be restated bit for bit
-// (pyrDown of the gray image, calcOpticalFlowFarneback, warpPerspective -- perfect/src/Flow.cc:26,29,80); everything after
+// interface (ComputeMask x2), its two members and its host-side OpenCV calls (pyrDown of the gray image,
+// calcOpticalFlowFarneback, warpPerspective -- perfect/src/Flow.cc:26,29,78); everything after
 // the optical flow -- pyrUp of the flow field, the threshold loop, erode, erode, dilate with the 21x21 ellipse
-// (perfect/src/Flow.cc:30-47) -- runs on the GPU through dynm_mask_from_flow (include/b200orb.h).  There is no CPU
+// (perfect/src/Flow.cc:30-47) -- runs on the GPU through dynm_mask_from_flow (include/b200orb.h).  The library has
+// device twins of the host calls too (dynm_farneback, dynm_warp_perspective), but the shim keeps OpenCV's: the host
+// build's Farneback (AVX2 / FMA dispatch) differs in the last bits from the baseline dispatch the device twin follows,
+// and warping alone on the device would only add an upload and a download between two host calls.  There is no CPU
 // fallback: the constructor throws when the library has no device.
 #ifndef FLOW_H
 #define FLOW_H
@@ -47,7 +50,7 @@ class Flow {
     std::swap(mImGrayLast, mImGrayCurrent);
   }
 
-  // perfect/src/Flow.cc:76-83
+  // perfect/src/Flow.cc:73-80
   void ComputeMask(const cv::Mat& GrayImg, const cv::Mat& Homo, cv::Mat& mask, float BInaryThreshold) {
     cv::Mat dest;
     cv::warpPerspective(GrayImg, dest, Homo, GrayImg.size());

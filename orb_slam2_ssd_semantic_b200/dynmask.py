@@ -6,7 +6,8 @@ images is OpenCV's calcOpticalFlowFarneback in the reference (perfect/src/Flow.c
 (`flow_fn(prev, cur) -> rows x cols x 2 float32`, default: cv2's, when cv2 is importable); `DynamicMask.farneback` is the
 same call on the GPU, bit-exact with OpenCV 4.13 at its baseline dispatch level (`Flow(flow_fn=dm.farneback)`).
 Everything after it -- pyrUp of the flow, the threshold loop, erode, erode, dilate -- runs on the GPU
-(dynm_mask_from_flow).
+(dynm_mask_from_flow).  The homography overload (perfect/src/Flow.cc:73-80, `ComputeMask(GrayImg, Homo=H)` here) first
+warps the gray image by cv::warpPerspective on the GPU (`DynamicMask.warp_perspective`, bit-exact with OpenCV 4.13).
 
 `filter_keypoints` is the keypoint loop of the masked RGB-D Frame constructor (perfect/src/Frame.cc:356-377).
 """
@@ -89,6 +90,25 @@ class DynamicMask:
         _lib.check(self._L.dynm_flow_batch_device(self._h, C.c_void_p(d_gray), C.c_void_p(d_prev or None), int(nframes),
                                                   int(rows), int(cols), C.c_void_p(d_flow)))
 
+    def warp_perspective(self, gray: np.ndarray, H) -> np.ndarray:
+        """cv::warpPerspective(gray, dest, H, gray.size()) on the GPU (perfect/src/Flow.cc:78: INTER_LINEAR,
+        BORDER_CONSTANT 0, H inverted first), bit-exact with OpenCV 4.13.  H: the 3x3 forward map -> rows x cols uint8."""
+        gray = np.ascontiguousarray(gray, np.uint8)
+        H = np.ascontiguousarray(H, np.float64)
+        if gray.ndim != 2:
+            raise ValueError("gray must be rows x cols uint8")
+        if H.size != 9:
+            raise ValueError("H must be a 3x3 matrix")
+        dst = np.zeros_like(gray)
+        _lib.check(self._L.dynm_warp_perspective(self._h, _p(gray), gray.shape[0], gray.shape[1], _p(H), _p(dst)))
+        return dst
+
+    def warp_perspective_batch_device(self, d_gray: int, nframes: int, rows: int, cols: int, d_H: int, d_dst: int):
+        """warp_perspective of nframes u8 images in HBM (device pointers), frame n by its own H d_H[n][9] float64, into
+        d_dst[nframes][rows][cols].  Asynchronous on this handle's stream (stream())."""
+        _lib.check(self._L.dynm_warp_perspective_batch_device(self._h, C.c_void_p(d_gray), int(nframes), int(rows),
+                                                              int(cols), C.c_void_p(d_H), C.c_void_p(d_dst)))
+
     def stream(self) -> int:
         return int(self._L.dynm_stream(self._h) or 0)
 
@@ -119,8 +139,13 @@ class Flow:
         self.mImGrayLast = None
         self.mImGrayCurrent = None
 
-    def ComputeMask(self, GrayImg: np.ndarray, BInaryThreshold: float = 40.0):
-        """-> mask (rows x cols uint8, 1 = static) or None for an empty image (the reference leaves `mask` untouched)."""
+    def ComputeMask(self, GrayImg: np.ndarray, BInaryThreshold: float = 40.0, Homo=None):
+        """-> mask (rows x cols uint8, 1 = static) or None for an empty image (the reference leaves `mask` untouched).
+        Homo (3x3, the forward map findHomography returns): the overload of Flow.cc:73-80, which computes the mask of
+        warpPerspective(GrayImg, Homo) -- warped on the GPU -- instead of GrayImg's.  An empty GrayImg returns None with
+        Homo too, where the reference's warpPerspective of the empty Mat throws."""
+        if Homo is not None and GrayImg is not None and GrayImg.size:
+            GrayImg = self._dm.warp_perspective(GrayImg, Homo)          # :78
         if GrayImg is None or GrayImg.size == 0:
             return None
         mask = np.ones(GrayImg.shape[:2], np.uint8)                      # :25
