@@ -655,7 +655,8 @@ long long ocm_launch_count(const ocm_t* h);
  *   gcm_refilter               "voxel.setInputCloud(globalMap); voxel.filter(*tmp); globalMap->swap(*tmp)" (:490-493),
  *                              VoxelGrid leaf = the constructor's resolution (:40)
  *   gcm_export                 the points of globalMap (what viewer / global_color.pcd receive, :496-521), cell order
- * B200ORB_EGEOM from gcm_refilter: the cell index space overflows int for this leaf (PCL leaves the cloud unfiltered). */
+ * B200ORB_EGEOM from gcm_refilter: the cell index space overflows int for this leaf (PCL leaves the cloud unfiltered);
+ * the map then keeps its finite points in insertion order, as the reference's globalMap, which never holds a NaN. */
 typedef struct gcm gcm_t;
 int gcm_create(float leaf, int device, gcm_t** out);
 void gcm_destroy(gcm_t* h);

@@ -6,7 +6,8 @@
 // The refilter of N points is order-exact and fully parallel:
 //   bounding box (ordered-int atomics) -> linear cell index per point -> stable radix sort of (index, position)
 //   -> cell heads -> one thread per cell sums its points in sorted (= input) order in float -> centroids in index order.
-// Non-finite points stay in the list with a sentinel index and fall off the end of the sort (removeNaNFromPointCloud).
+// Non-finite points stay in the list with the no-cell key (gcm.cuh) and fall off the end of the sort
+// (removeNaNFromPointCloud).
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
@@ -65,33 +66,60 @@ __global__ void k_gcm_minmax(const float* __restrict__ xyz, long long n, unsigne
   }
 }
 
-// PCL VoxelGrid::applyFilter: min_b = floor(min * inv), div_b, linear index; flag[0] = index space overflows int
+// PCL VoxelGrid::applyFilter: the overflow test, then min_b = floor(min * inv), div_b, linear index.  Where the index
+// space overflows int (flag[0]), PCL builds no grid and neither does this: every point keeps the no-cell key, and no
+// div_b product is formed (it could overflow int).
 __global__ void k_gcm_index(const float* __restrict__ xyz, long long n, float inv, const unsigned* __restrict__ mm,
-                            int* __restrict__ idx, int* __restrict__ pos, int* __restrict__ flag) {
+                            unsigned* __restrict__ idx, int* __restrict__ pos, int* __restrict__ flag) {
   const float mn[3] = {ord2f(mm[0]), ord2f(mm[1]), ord2f(mm[2])}, mx[3] = {ord2f(mm[3]), ord2f(mm[4]), ord2f(mm[5])};
-  int min_b[3], div_b[3];
+  const long long dx = (long long)((mx[0] - mn[0]) * inv) + 1, dy = (long long)((mx[1] - mn[1]) * inv) + 1,
+                  dz = (long long)((mx[2] - mn[2]) * inv) + 1;
+  const bool grid = dx * dy * dz <= 2147483647LL;
+  if (!grid && blockIdx.x == 0 && threadIdx.x == 0) flag[0] = 1;
+  int min_b[3] = {0, 0, 0}, m1 = 0, m2 = 0;
+  if (grid) {
+    int div_b[3];
 #pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    min_b[k] = (int)floorf(mn[k] * inv);
-    div_b[k] = (int)floorf(mx[k] * inv) - min_b[k] + 1;
+    for (int k = 0; k < 3; ++k) {
+      min_b[k] = (int)floorf(mn[k] * inv);
+      div_b[k] = (int)floorf(mx[k] * inv) - min_b[k] + 1;
+    }
+    m1 = div_b[0];
+    m2 = div_b[0] * div_b[1];
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const long long dx = (long long)((mx[0] - mn[0]) * inv) + 1, dy = (long long)((mx[1] - mn[1]) * inv) + 1,
-                    dz = (long long)((mx[2] - mn[2]) * inv) + 1;
-    if (dx * dy * dz > 2147483647LL) flag[0] = 1;
-  }
-  const int m1 = div_b[0], m2 = div_b[0] * div_b[1];
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float x = xyz[i * 3], y = xyz[i * 3 + 1], z = xyz[i * 3 + 2];
-    int v = GCM_SENTINEL;
-    if (isfinite(x) && isfinite(y) && isfinite(z)) {
+    unsigned v = gcm_no_cell<unsigned>();
+    if (grid && isfinite(x) && isfinite(y) && isfinite(z)) {
       const int i0 = (int)(floorf(x * inv) - (float)min_b[0]);
       const int i1 = (int)(floorf(y * inv) - (float)min_b[1]);
       const int i2 = (int)(floorf(z * inv) - (float)min_b[2]);
-      v = i0 + i1 * m1 + i2 * m2;
+      v = (unsigned)(i0 + i1 * m1 + i2 * m2);
     }
     idx[i] = v;
     pos[i] = (int)i;
+  }
+}
+
+// gcm_refilter's overflow path: the positions of the finite points (read from the points: there are no cell keys),
+// and their gather
+struct GcmFinite {
+  const float* xyz;
+  __device__ bool operator()(int i) const {
+    const size_t p = (size_t)i * 3;
+    return isfinite(xyz[p]) && isfinite(xyz[p + 1]) && isfinite(xyz[p + 2]);
+  }
+};
+
+__global__ void k_gcm_gather(const int* __restrict__ sel, const int* __restrict__ m, const float* __restrict__ xyz,
+                             const uint8_t* __restrict__ rgb, float* __restrict__ oxyz, uint8_t* __restrict__ orgb) {
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= *m) return;
+  const size_t p = (size_t)sel[u];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    oxyz[(size_t)u * 3 + k] = xyz[p * 3 + k];
+    orgb[(size_t)u * 3 + k] = rgb[p * 3 + k];
   }
 }
 
@@ -172,17 +200,21 @@ int gcm_refilter(gcm_t* h) {
   cudaStream_t st = h->stream;
   const long long n = h->n;
   const float inv = 1.0f / h->leaf;
-  // CUB scratch for the larger of the two primitives at n points
-  size_t s1 = 0, s2 = 0;
-  int *d_idx, *d_idx2, *d_pos, *d_pos2, *d_starts;
+  // CUB scratch for the largest of the three primitives at n points
+  size_t s1 = 0, s2 = 0, s3 = 0;
+  unsigned *d_idx, *d_idx2;
+  int *d_pos, *d_pos2, *d_starts;
   uint8_t* d_head;
   void* d_tmp;
-  cub::DeviceRadixSort::SortPairs(nullptr, s1, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)n, 0, 32, st);
+  cub::DeviceRadixSort::SortPairs(nullptr, s1, (unsigned*)nullptr, (unsigned*)nullptr, (int*)nullptr, (int*)nullptr, (int)n, 0, 32,
+                                  st);
   cub::DeviceSelect::Flagged(nullptr, s2, thrust::counting_iterator<int>(0), (uint8_t*)nullptr, (int*)nullptr, (int*)nullptr,
                              (int)n, st);
-  const size_t tmp_bytes = std::max(s1, s2);
+  cub::DeviceSelect::If(nullptr, s3, thrust::counting_iterator<int>(0), (int*)nullptr, (int*)nullptr, (int)n, GcmFinite{nullptr},
+                        st);
+  const size_t tmp_bytes = std::max(std::max(s1, s2), s3);
   B200_CHECK(h->sort.reserve(st, [&](Carver& t) {
-    d_idx = t.take<int>(n); d_idx2 = t.take<int>(n); d_pos = t.take<int>(n); d_pos2 = t.take<int>(n);
+    d_idx = t.take<unsigned>(n); d_idx2 = t.take<unsigned>(n); d_pos = t.take<int>(n); d_pos2 = t.take<int>(n);
     d_starts = t.take<int>(n); d_head = t.take<uint8_t>(n); d_tmp = t.take<char>(tmp_bytes);
   }));
   static const unsigned mm0[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
@@ -192,7 +224,7 @@ int gcm_refilter(gcm_t* h) {
   k_gcm_index<<<4 * h->sms, 256, 0, st>>>(h->d_xyz, n, inv, h->d_mm, d_idx, d_pos, h->d_flag);
   size_t tb = tmp_bytes;
   B200_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_idx, d_idx2, d_pos, d_pos2, (int)n, 0, 32, st));
-  k_gcm_heads<int><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_idx2, n, d_head);
+  k_gcm_heads<unsigned><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_idx2, n, d_head);
   tb = tmp_bytes;
   B200_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<int>(0), d_head, d_starts, h->d_flag + 1, (int)n,
                                        st));
@@ -201,13 +233,27 @@ int gcm_refilter(gcm_t* h) {
   B200_CUDA(cudaStreamSynchronize(st));
   h->launches += 5;
   if (flag[0]) {   // PCL: "Leaf size is too small for the input dataset. Integer indices would overflow." -> output = input
+    // The reference's globalMap never holds a non-finite point (removeNaNFromPointCloud runs before "*globalMap += ...",
+    // :484-485), so the map keeps its finite points, in insertion order.
+    tb = tmp_bytes;
+    B200_CUDA(cub::DeviceSelect::If(d_tmp, tb, thrust::counting_iterator<int>(0), d_starts, h->d_flag + 1, (int)n,
+                                    GcmFinite{h->d_xyz}, st));
+    k_gcm_gather<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_starts, h->d_flag + 1, h->d_xyz, h->d_rgb, h->d_xyz2, h->d_rgb2);
+    h->launches += 2;
+    B200_CUDA(cudaGetLastError());
+    int kept = 0;
+    B200_CUDA(cudaMemcpyAsync(&kept, h->d_flag + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    std::swap(h->d_xyz, h->d_xyz2);
+    std::swap(h->d_rgb, h->d_rgb2);
+    h->n = kept;
     set_error("VoxelGrid index space overflows int for this leaf size (PCL returns the cloud unfiltered)");
     return B200ORB_EGEOM;
   }
   const int cells = flag[1];
   if (cells > 0) {
-    k_gcm_centroids<int, true><<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(d_idx2, d_pos2, d_starts, h->d_flag + 1, n, h->d_xyz,
-                                                                    h->d_rgb, h->d_xyz2, h->d_rgb2);
+    k_gcm_centroids<unsigned, true><<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(d_idx2, d_pos2, d_starts, h->d_flag + 1, n,
+                                                                                     h->d_xyz, h->d_rgb, h->d_xyz2, h->d_rgb2);
     ++h->launches;
   }
   B200_CUDA(cudaGetLastError());

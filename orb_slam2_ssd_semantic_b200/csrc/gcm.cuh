@@ -5,15 +5,23 @@
 
 namespace b200 {
 
-constexpr int GCM_SENTINEL = 0x7fffffff;
+// Key = unsigned (the map's cell index) or unsigned long long (gcm_sem.cu: box << 32 | cell index).  Cell indices
+// exist only in a grid that passes PCL's overflow test (where it fails, k_gcm_index gives every point the no-cell key
+// and k_sem_cellkey numbers the points instead).  Such an index lies in [0, INT_MAX] -- INT_MAX itself included: div_b
+// may exceed PCL's dx, dy, dz by one, so the last cell can have index INT_MAX -- and a box is below 2^31, so the
+// all-ones key is never a cell: it marks a point without one and sorts last.
+template <class Key>
+__host__ __device__ constexpr Key gcm_no_cell() {
+  static_assert(Key(0) < Key(-1), "cell keys are unsigned");
+  return ~Key(0);
+}
 
-// Key = int (the map's cell index) or unsigned long long (gcm_sem.cu: box << 32 | cell index, never the sentinel)
 template <class Key>
 __global__ void k_gcm_heads(const Key* __restrict__ idx_sorted, long long n, uint8_t* __restrict__ head) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const Key v = idx_sorted[i];
-  head[i] = (v != GCM_SENTINEL) && (i == 0 || idx_sorted[i - 1] != v);
+  head[i] = (v != gcm_no_cell<Key>()) && (i == 0 || idx_sorted[i - 1] != v);
 }
 
 // one thread per cell: sequential float sums in sorted (= input) order, centroid = sum / count (colour only if kRgb)

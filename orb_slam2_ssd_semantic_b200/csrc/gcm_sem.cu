@@ -302,10 +302,12 @@ __global__ void k_sem_cellkey(const float* __restrict__ bxyz, const int* __restr
   pos[i] = i;
 }
 
-// compute3DCentroid (float sums in output order, / count as float) and getMinMax3D over the box's voxel centroids
+// compute3DCentroid (float sums in output order, / count as float) and getMinMax3D over the box's voxel centroids, or
+// over its inliers themselves where its VoxelGrid overflowed (a one-point centroid 0.f + x would turn -0.0 into +0.0)
 __global__ void k_sem_finish(const unsigned long long* __restrict__ key, const int* __restrict__ cstart,
-                             const int* __restrict__ ncells, const float* __restrict__ cxyz, const int* __restrict__ bstart,
-                             const int* __restrict__ kstart, int B, GcmCluster* __restrict__ out) {
+                             const int* __restrict__ ncells, const float* __restrict__ cxyz, const float* __restrict__ kxyz,
+                             const SemVoxel* __restrict__ vg, const int* __restrict__ bstart, const int* __restrict__ kstart,
+                             int B, GcmCluster* __restrict__ out) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   GcmCluster c = {};
@@ -326,11 +328,12 @@ __global__ void k_sem_finish(const unsigned long long* __restrict__ key, const i
     }
     c.n_inliers = kstart[b + 1] - kstart[b];
     c.n_voxels = lo - c0;
+    const float* vox = c.n_voxels > 0 && vg[b].overflow ? kxyz + (size_t)kstart[b] * 3 : cxyz + (size_t)c0 * 3;
     float s[3] = {0.f, 0.f, 0.f}, mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-    for (int u = c0; u < lo; ++u)
+    for (int u = 0; u < c.n_voxels; ++u)
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        const float v = cxyz[(size_t)u * 3 + k];
+        const float v = vox[(size_t)u * 3 + k];
         s[k] += v;
         mn[k] = v < mn[k] ? v : mn[k];
         mx[k] = v > mx[k] ? v : mx[k];
@@ -513,7 +516,7 @@ int gcm_add_keyframe_objects_device(gcm_t* h, const float* d_depth, const uint8_
           d_key2, d_pos2, d_cstart, d_ncells, nk, d_kxyz, nullptr, d_cxyz, nullptr);
       h->launches += 4;
     }
-    k_sem_finish<<<gB, 64, 0, st>>>(d_key2, d_cstart, d_ncells, d_cxyz, d_bst, d_kstart, B, d_out);
+    k_sem_finish<<<gB, 64, 0, st>>>(d_key2, d_cstart, d_ncells, d_cxyz, d_kxyz, d_vg, d_bst, d_kstart, B, d_out);
     ++h->launches;
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(res.data(), d_out, sizeof(GcmCluster) * B, cudaMemcpyDeviceToHost, st));

@@ -176,7 +176,7 @@ def test_global_cloud_refilter_matches_oracle(oracle):
         acc_xyz, acc_rgb = oracle.global_refilter(acc_xyz, acc_rgb, leaf)
         gx, gc = gpu.points()
         assert len(gx) == len(acc_xyz) and len(acc_xyz) > 1000
-        assert np.abs(gx - acc_xyz).max() <= 1e-5       # bit-equal in practice: same order, same float sums
+        assert (gx.view(np.uint32) == acc_xyz.view(np.uint32)).all()   # same order, same float sums: bit-equal
         assert (gc == acc_rgb).all()
     with pytest.raises(Exception):
         GlobalCloudMapping(0.0)
