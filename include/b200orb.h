@@ -82,10 +82,11 @@ int orbx_sync(orbx_t* h);
 void* orbx_stream(orbx_t* h);   /* cudaStream_t the handle launches on */
 
 /* Backs the public member mvImagePyramid (include/ORBextractor.h:80): level image of frame `frame` of the
- * last extract.  bordered=0: rows x cols level (the ROI the reference stores); bordered=1: the
- * (rows+38)x(cols+38) parent buffer with the BORDER_REFLECT_101 frame (src/ORBextractor.cc:1125-1142). */
+ * last extract.  kind=0: rows x cols level (the ROI the reference stores); kind=1: the
+ * (rows+38)x(cols+38) parent buffer with the BORDER_REFLECT_101 frame (src/ORBextractor.cc:1125-1142);
+ * kind=2: rows x cols GaussianBlur 7x7 of the level, the image the descriptors read (:1094-1095). */
 int orbx_level_dims(const orbx_t* h, int level, int* rows, int* cols);
-int orbx_get_level(orbx_t* h, int frame, int level, int bordered, uint8_t* dst, size_t dst_stride);
+int orbx_get_level(orbx_t* h, int frame, int level, int kind, uint8_t* dst, size_t dst_stride);
 
 /* GetScaleFactors / GetInverseScaleFactors / GetScaleSigmaSquares / GetInverseScaleSigmaSquares
  * (include/ORBextractor.h:63-77) + mnFeaturesPerLevel; each array has nlevels entries (NULL = skip). */
@@ -94,6 +95,10 @@ int orbx_scale_tables(const orbx_t* h, float* sf, float* inv_sf, float* sigma2, 
 
 /* Diagnostics for parity tests: FAST candidates per level of frame `frame` of the last extract. */
 int orbx_candidates_per_level(orbx_t* h, int frame, int* counts /*nlevels*/);
+/* The FAST candidates of one level of frame `frame` of the last extract, in the order the quad-tree reads them
+ * (vToDistributeKeys, src/ORBextractor.cc:788-843): cell by cell, row-major inside a cell.  xys[3*i..3*i+2] = x, y (level
+ * pixels) and score.  *n = the count; cap < *n: B200ORB_ECAP and nothing written. */
+int orbx_get_candidates(orbx_t* h, int frame, int level, int32_t* xys, int cap, int* n);
 /* Number of CUDA kernels launched by this handle since creation (bench.py's gpu_launches). */
 long long orbx_launch_count(const orbx_t* h);
 /* Per-stage device time via CUDA events on the handle's stream (bench.py's roofline leg).  Stages:

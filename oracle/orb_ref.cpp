@@ -71,6 +71,7 @@ struct Extractor {
   int umax[HALF_PATCH_SIZE + 1];
   std::vector<Plane> pyr;      // bordered level buffers (w+38)x(h+38); level image is the ROI at (19,19)
   std::vector<int> lw, lh;
+  std::vector<std::vector<KeyPoint>> cand;   // per level: vToDistributeKeys of the last extract (:788-843)
   long seq_counter = 0;
 
   Extractor(int nf, float sfac, int nl, int ini, int mn)
@@ -101,7 +102,7 @@ struct Extractor {
       umax[v] = v0;
       ++v0;
     }
-    pyr.resize(nl); lw.resize(nl); lh.resize(nl);
+    pyr.resize(nl); lw.resize(nl); lh.resize(nl); cand.resize(nl);
   }
 
   uint8_t* lvl(int l, int y) { return pyr[l].row(y + EDGE_THRESHOLD) + EDGE_THRESHOLD; }
@@ -310,7 +311,8 @@ struct Extractor {
     const int maxBorderX = lw[level] - EDGE_THRESHOLD + 3;
     const int maxBorderY = lh[level] - EDGE_THRESHOLD + 3;
     const float width = (float)(maxBorderX - minBorderX), height = (float)(maxBorderY - minBorderY);
-    std::vector<KeyPoint> toDist;
+    std::vector<KeyPoint>& toDist = cand[level];
+    toDist.clear();
     keypoints.clear();
     if (ncand) *ncand = 0;
     if (width <= 0 || height <= 0) return 0;
@@ -419,6 +421,22 @@ void orb_ref_get_level(void* h, int level, int bordered, uint8_t* dst) {
   } else {
     for (int y = 0; y < hh; ++y) memcpy(dst + (size_t)y * w, e->lvl(level, y), w);
   }
+}
+
+// FAST candidates of `level` of the last extract, in vToDistributeKeys order: triples (x, y, score) in level pixels
+// (shifted by minBorderX / minBorderY).  Returns the count; writes only when it fits in cap.
+int orb_ref_candidates(void* h, int level, int* out, int cap) {
+  Extractor* e = (Extractor*)h;
+  if (level < 0 || level >= e->nlevels) return -1;
+  const std::vector<KeyPoint>& v = e->cand[level];
+  const int n = (int)v.size(), minBorder = EDGE_THRESHOLD - 3;
+  if (n > cap) return n;
+  for (int i = 0; i < n; ++i) {
+    out[3 * i] = (int)v[i].x + minBorder;
+    out[3 * i + 1] = (int)v[i].y + minBorder;
+    out[3 * i + 2] = (int)v[i].response;
+  }
+  return n;
 }
 
 // ---- primitives exposed for direct pinning against cv2 ----

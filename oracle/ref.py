@@ -41,6 +41,8 @@ def lib() -> C.CDLL:
         L.orb_ref_tables.argtypes = [C.c_void_p] + [C.c_void_p] * 6
         L.orb_ref_level_dims.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.orb_ref_get_level.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.orb_ref_candidates.restype = C.c_int
+        L.orb_ref_candidates.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.orb_ref_resize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
         L.orb_ref_blur.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.orb_ref_fast.restype = C.c_int
@@ -101,6 +103,16 @@ class RefExtractor:
         out = np.zeros(shp, np.uint8)
         self.L.orb_ref_get_level(self.h, l, int(bordered), _p(out))
         return out
+
+    def candidates(self, l: int) -> np.ndarray:
+        """FAST candidates of level l of the last call, [n, 3] int32 (x, y, score) in level pixels, vToDistributeKeys
+        order."""
+        n = self.L.orb_ref_candidates(self.h, l, None, 0)
+        if n < 0:
+            raise ValueError("bad level %d" % l)
+        out = np.zeros((max(n, 1), 3), np.int32)
+        self.L.orb_ref_candidates(self.h, l, _p(out), n)
+        return out[:n]
 
 
 def resize(src: np.ndarray, dw: int, dh: int) -> np.ndarray:

@@ -500,17 +500,19 @@ int orbx_level_dims(const orbx_t* h, int level, int* rows, int* cols) {
   return B200ORB_OK;
 }
 
-int orbx_get_level(orbx_t* h, int frame, int level, int bordered, uint8_t* dst, size_t dst_stride) {
-  if (!h || !dst || !h->have_results || level < 0 || level >= h->prm.nlevels || frame < 0 || frame >= h->lastF) {
+int orbx_get_level(orbx_t* h, int frame, int level, int kind, uint8_t* dst, size_t dst_stride) {
+  if (!h || !dst || !h->have_results || level < 0 || level >= h->prm.nlevels || frame < 0 || frame >= h->lastF ||
+      kind < 0 || kind > 2) {
     set_error("bad argument / no extract yet");
     return B200ORB_EINVAL;
   }
   DeviceGuard g(h->device);
   const int w = h->lw[level], hh = h->lh[level];
-  const uint8_t* src = h->rawv.p[level] + (size_t)frame * h->rawv.fstride[level];
-  if (!bordered) {
+  const PyrView& v = (kind == 2) ? h->blurv : h->rawv;
+  const uint8_t* src = v.p[level] + (size_t)frame * v.fstride[level];
+  if (kind != 1) {
     if (dst_stride < (size_t)w) { set_error("dst_stride too small"); return B200ORB_EINVAL; }
-    B200_CUDA(cudaMemcpy2DAsync(dst, dst_stride, src, h->rawv.pitch[level], w, hh, cudaMemcpyDeviceToHost, h->stream));
+    B200_CUDA(cudaMemcpy2DAsync(dst, dst_stride, src, v.pitch[level], w, hh, cudaMemcpyDeviceToHost, h->stream));
     B200_CUDA(cudaStreamSynchronize(h->stream));
     return B200ORB_OK;
   }
@@ -545,6 +547,41 @@ int orbx_candidates_per_level(orbx_t* h, int frame, int* counts) {
   B200_CUDA(cudaMemcpyAsync(counts, h->d_candcnt + (size_t)frame * h->prm.nlevels, sizeof(int) * h->prm.nlevels,
                             cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
+  return B200ORB_OK;
+}
+
+int orbx_get_candidates(orbx_t* h, int frame, int level, int32_t* xys, int cap, int* n) {
+  if (!h || !n || !h->have_results || level < 0 || level >= h->prm.nlevels || frame < 0 || frame >= h->lastF) {
+    set_error("bad argument / no extract yet");
+    return B200ORB_EINVAL;
+  }
+  DeviceGuard g(h->device);
+  const int c0 = h->ltab.cell_begin[level], nc = h->ltab.cell_begin[level + 1] - c0;
+  const int s0 = h->ltab.slot_begin[level], ns = h->ltab.slot_begin[level + 1] - s0;
+  std::vector<CellDesc> cells(nc);
+  std::vector<int> cnt(nc);
+  std::vector<unsigned> slots(ns);
+  B200_CUDA(cudaMemcpyAsync(cells.data(), h->d_cells + c0, sizeof(CellDesc) * nc, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaMemcpyAsync(cnt.data(), h->d_cellcnt + (size_t)frame * h->ncells + c0, sizeof(int) * nc,
+                            cudaMemcpyDeviceToHost, h->stream));
+  if (ns > 0)
+    B200_CUDA(cudaMemcpyAsync(slots.data(), h->d_cand + (size_t)frame * h->slots_per_frame + s0, sizeof(unsigned) * ns,
+                              cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  int total = 0;
+  for (int c = 0; c < nc; ++c) total += cnt[c];
+  *n = total;
+  if (cap < total) { set_error("level %d has %d FAST candidates > cap %d", level, total, cap); return B200ORB_ECAP; }
+  if (total > 0 && !xys) { set_error("null output buffer"); return B200ORB_EINVAL; }
+  // the cells' segments in cell order: the order k_quadtree gathers them in
+  int k = 0;
+  for (int c = 0; c < nc; ++c)
+    for (int i = 0; i < cnt[c]; ++i, ++k) {
+      const unsigned v = slots[cells[c].slot_off - s0 + i];
+      xys[3 * k] = (int32_t)(v & 0xfff);
+      xys[3 * k + 1] = (int32_t)((v >> 12) & 0xfff);
+      xys[3 * k + 2] = (int32_t)(v >> 24);
+    }
   return B200ORB_OK;
 }
 

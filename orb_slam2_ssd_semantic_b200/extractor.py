@@ -108,12 +108,17 @@ class ORBextractor:
         return [(kps[f, :n[f]].copy(), desc[f, :n[f]].copy()) for f in range(F)]
 
     # -- mvImagePyramid (include/ORBextractor.h:80) -----------------------------------------------------------
-    def image_pyramid_level(self, level: int, frame: int = 0, bordered: bool = False) -> np.ndarray:
+    def image_pyramid_level(self, level: int, frame: int = 0, bordered: bool = False, blurred: bool = False) -> np.ndarray:
+        """Level `level` of frame `frame` of the last extract; `bordered` adds the REFLECT_101 frame, `blurred` returns the
+        7x7 Gaussian blur of the level that the descriptors read instead."""
+        if bordered and blurred:
+            raise ValueError("the blurred level has no bordered form")
         r, c = C.c_int(), C.c_int()
         _lib.check(self._L.orbx_level_dims(self._h, level, C.byref(r), C.byref(c)))
         shp = (r.value + 38, c.value + 38) if bordered else (r.value, c.value)
         out = np.zeros(shp, np.uint8)
-        _lib.check(self._L.orbx_get_level(self._h, frame, level, int(bordered), _p(out), out.strides[0]))
+        kind = 2 if blurred else int(bordered)
+        _lib.check(self._L.orbx_get_level(self._h, frame, level, kind, _p(out), out.strides[0]))
         return out
 
     @property
@@ -124,6 +129,16 @@ class ORBextractor:
         out = np.zeros(self.nlevels, np.int32)
         _lib.check(self._L.orbx_candidates_per_level(self._h, frame, _p(out)))
         return out
+
+    def fast_candidates(self, level: int, frame: int = 0) -> np.ndarray:
+        """FAST survivors of one level, [n, 3] int32 (x, y, score) in level pixels, in the quad-tree's input order."""
+        n = C.c_int(0)
+        rc = self._L.orbx_get_candidates(self._h, frame, level, None, 0, C.byref(n))
+        if rc != -2:   # B200ORB_ECAP: *n is the count, nothing written
+            _lib.check(rc)
+        out = np.zeros((max(n.value, 1), 3), np.int32)
+        _lib.check(self._L.orbx_get_candidates(self._h, frame, level, _p(out), n.value, C.byref(n)))
+        return out[:n.value]
 
     def launch_count(self) -> int:
         return int(self._L.orbx_launch_count(self._h))
