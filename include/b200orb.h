@@ -419,7 +419,7 @@ int dynm_filter_keypoints_batch_device(dynm_t* h, const uint8_t* d_mask, int nfr
 int dynm_farneback(dynm_t* h, const uint8_t* prev, const uint8_t* cur, int rows, int cols, float* flow);
 /* Flow.cc:26-29 for nframes consecutive full-resolution gray images d_gray[n][rows][cols] u8 in HBM: pyrDown of each, then
  * the flow from frame t-1 to frame t into d_flow[t][rows / 2][cols / 2][2] f32 -- the layout
- * orbs_track_batch_masked_device takes.  d_prev is the frame before d_gray[0] (rows x cols u8 in HBM); NULL: the sequence
+ * OrbsBatch.flow takes.  d_prev is the frame before d_gray[0] (rows x cols u8 in HBM); NULL: the sequence
  * starts at d_gray[0], whose flow is the zero field (the reference's first-frame `mask = ones`).  Asynchronous on the
  * handle's stream; the scratch grows with min(nframes, 64) frames of the geometry (about 7 MB per frame at 640 x 480). */
 int dynm_flow_batch_device(dynm_t* h, const uint8_t* d_gray, const uint8_t* d_prev, int nframes, int rows, int cols,
@@ -456,86 +456,85 @@ typedef struct {
 } OrbsParams;
 int orbs_create(const OrbsParams* p, int device, orbs_t** out);
 void orbs_destroy(orbs_t* h);
-/* Host-buffer entry: gray[n][rows][cols] u8, depth[n][rows][cols] f32 metres, Tcw[n][16] f32 row-major.
- * Outputs (host): kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1), nmatch[n]. */
-int orbs_track_batch(orbs_t* h, const uint8_t* gray, const float* depth, const float* Tcw, int nframes,
-                     int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp, int32_t* cur2last,
-                     int32_t* nmatch, int cap);
-/* Same with the depth image as the sensor delivers it (CV_16U, e.g. TUM PNGs).  The tracking path reads depth only
- * under the keypoints (Frame::ComputeStereoFromRGBD, src/Frame.cc:850-871): the device gathers those pixels and converts
- * them as imDepth.convertTo(CV_32F, mDepthMapFactor) of Tracking::GrabImageRGBD does (src/Tracking.cc:366-367; float
- * multiply by depth_factor = 1.0f / DepthMapFactor).  When depth_u16 is page-locked host memory (cudaHostAlloc /
- * cudaHostRegister) the pixels are read in place over PCIe and the depth images are not uploaded at all; pageable
- * depth is uploaded as CV_16U, half the host->device traffic of f32 depth. */
-int orbs_track_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                         int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
-                         int32_t* cur2last, int32_t* nmatch, int cap);
-/* Pipelining aid for two handles used alternately: the next batch submitted to h starts its kernels only when the kernels
- * of prev's last submitted batch are done; h's uploads and prev's downloads proceed meanwhile, so the stages upload(k+1) |
- * kernels(k) | download(k-1) overlap without two batches' kernels sharing the SMs.  The dependency is consumed by h's next
- * submit; prev must stay alive until then. */
+/* One batch of orbs_submit: gray[n][rows][cols] u8, Tcw[n][16] f32 row-major, one depth image per frame.  Exactly seven
+ * forms are accepted:
+ *   host batches (device = 0):    f32 depth | CV_16U depth | CV_16U depth + flow | CV_16U depth + device_flow
+ *   device batches (device = 1):  f32 depth | f32 depth + flow
+ * Every other combination -- and a NULL input, a non-positive size, both depths or neither, prev_gray without
+ * device_flow -- returns B200ORB_EINVAL before anything is enqueued and before any handle state changes. */
+typedef struct {
+  int nframes, rows, cols;
+  int device;                   /* 1: every input below is an HBM pointer and the results stay in HBM
+                                   (orbs_device_results); 0: host buffers, uploaded in chunks (orbs_set_chunk_frames) */
+  const uint8_t* gray;          /* [n][rows][cols] u8 */
+  const float* depth;           /* [n][rows][cols] f32 metres, or NULL when depth_u16 is given */
+  /* The depth image as the sensor delivers it (CV_16U, e.g. TUM PNGs; host batches only).  The tracking path reads depth
+   * only under the keypoints (Frame::ComputeStereoFromRGBD, src/Frame.cc:850-871): the device gathers those pixels and
+   * converts them as imDepth.convertTo(CV_32F, mDepthMapFactor) of Tracking::GrabImageRGBD does (src/Tracking.cc:366-367;
+   * float multiply by depth_factor = 1.0f / DepthMapFactor).  When depth_u16 is page-locked host memory (cudaHostAlloc /
+   * cudaHostRegister) the pixels are read in place over PCIe and the depth images are not uploaded at all; pageable
+   * depth is uploaded as CV_16U, half the host->device traffic of f32 depth. */
+  const uint16_t* depth_u16;
+  float depth_factor;
+  const float* Tcw;             /* [n][16] */
+  /* Masked batches: the `perfect` variant's live path per frame (perfect/src/Tracking.cc:703-719).  Between extraction
+   * and the frame glue, one kernel per batch does Flow::ComputeMask after calcOpticalFlowFarneback (perfect/src/Flow.cc:
+   * 14-53: pyrUp of the flow, mask = 0 where x*x + y*y >= max(binary_threshold, 40), erode, erode, dilate with the 21 x 21
+   * ellipse) and the keypoint loop of the masked RGB-D Frame constructor (perfect/src/Frame.cc:328-427, :356-377: when the
+   * mask's sum is above 65 % of the pixels, keypoints whose pixel is not 1 are dropped with their descriptors, order
+   * kept).  Frame t is then tracked against the filtered frame t-1 with SearchByProjection(cur, last)
+   * (perfect/src/Tracking.cc:1933), and orbs_read_dynamic_mask returns the mask FrameDrawer receives
+   * (perfect/src/FrameDrawer.cc:262).
+   * flow[n][rows/2][cols/2][2] f32 is what calcOpticalFlowFarneback returns for the pyrDown'ed previous and current gray
+   * images (CV_32FC2, continuous); mask pixels beyond the 2 (rows/2) x 2 (cols/2) it covers stay 1.  A frame without a
+   * previous image (the sequence's first) takes a zero flow field: its mask is all ones and it keeps every keypoint, the
+   * reference's `mask = ones` case.  A host batch uploads it chunk by chunk next to the gray images.  The results keep the
+   * layout of unmasked batches and describe the FILTERED frames (nkp, kps, desc, cur2last against frame t-1's filtered
+   * keypoints), as do orbs_device_results and orbs_read_frame_glue.  A masked batch launches one kernel more than the
+   * same unmasked batch; orbx_profile_read counts its time in stage 5.
+   * Geometry (flow and device_flow): a frame's mask is held as two bit planes in one CTA's shared memory,
+   * 8 * rows * ceil(cols / 32) + 132 bytes; on an H100 (232448 bytes per CTA) rows * ceil(cols / 32) <= 29039: 1280 x 720
+   * and 1241 x 376 fit, 1280 x 725 is the largest 1280-wide image.  Larger images and flow fields under 2 x 2 return
+   * B200ORB_EINVAL before anything is enqueued. */
+  const float* flow;
+  /* Masked host batches whose flow the device computes (perfect/src/Flow.cc:26-29, as dynm_flow_batch_device) from the
+   * gray images the batch uploads anyway, in place of flow; nothing but prev_gray is uploaded beyond what the unmasked
+   * batch uploads.  Sizes dynm_flow_batch_device rejects return B200ORB_EINVAL before anything is enqueued. */
+  int device_flow;
+  /* With device_flow: the rows x cols u8 frame before gray[0]; NULL: the sequence starts at gray[0], which takes the zero
+   * field.  The predecessor is an argument rather than handle state, so two handles chained with orbs_chain_after can
+   * carry one sequence: each batch passes the last gray frame of the batch before. */
+  const uint8_t* prev_gray;
+  float binary_threshold;       /* masked batches: Flow::ComputeMask's threshold (raised to 40) */
+} OrbsBatch;
+/* Host results: kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1), nmatch[n]; cap below
+ * orbx_max_keypoints of the handle's extractor returns B200ORB_ECAP. */
+typedef struct { OrbxKeyPoint* kps; uint8_t* desc; int32_t* nkp; int32_t* cur2last; int32_t* nmatch; int cap; } OrbsResults;
+/* Tracks one batch; out is non-NULL exactly when !b->device.  Never waits: uploads, kernels and result downloads are
+ * enqueued on the handle's streams (orbs_stream for the kernels) and the results are valid after orbs_sync(h); the
+ * host buffers must stay untouched until then.  With page-locked host buffers the copies are plain DMA, and two
+ * handles used alternately keep two batches in flight, so the upload of batch k+1 and the download of batch k-1 overlap
+ * the kernels of batch k (what the reference's grab thread / tracking thread split does for one frame,
+ * Examples/RGB-D/rgbd_tum.cc:88-109, done here for whole batches).
+ * Only host batches take part in orbs_chain_after: a host batch consumes the dependency set on h and records the end
+ * of its kernels for a handle chained after h.  A device batch neither waits for the dependency (it stays set for h's
+ * next host batch) nor records. */
+int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out);
+/* Pipelining aid for two handles used alternately: the next host batch submitted to h starts its kernels only when the
+ * kernels of prev's last host batch are done; h's uploads and prev's downloads proceed meanwhile, so the stages
+ * upload(k+1) | kernels(k) | download(k-1) overlap without two batches' kernels sharing the SMs.  The dependency is
+ * consumed by h's next host batch; prev must stay alive until then. */
 int orbs_chain_after(orbs_t* h, orbs_t* prev);
-/* Frames per upload chunk of the host-buffer entries (default 128, at most 7 chunks per call): the extraction of a chunk
+/* Frames per upload chunk of host batches (default 128, at most 7 chunks per call): the extraction of a chunk
  * starts as soon as it has arrived while the next one is still crossing PCIe.  Gray images and any depth that is
  * uploaded go up chunk by chunk. */
 int orbs_set_chunk_frames(orbs_t* h, int frames);
-/* Streaming form of orbs_track_batch_u16: enqueues uploads, kernels and result downloads on the handle's streams and
- * returns; the outputs are valid after orbs_sync(h).  All host buffers must be page-locked and stay untouched until
- * then; depth_u16 is then read in place under the keypoints.  Two handles used alternately keep two batches in
- * flight, so the upload of batch k+1 and the download of batch k-1 overlap the kernels of batch k (what the reference's
- * grab thread / tracking thread split does for one frame, Examples/RGB-D/rgbd_tum.cc:88-109, done here for whole
- * batches). */
-int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                          int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
-                          int32_t* cur2last, int32_t* nmatch, int cap);
-/* Device-resident entry (inputs already in HBM, results left in HBM; asynchronous on orbs_stream). */
-int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw,
-                            int nframes, int rows, int cols);
 int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d_desc, const int32_t** d_nkp,
                         const int32_t** d_cur2last, const int32_t** d_nmatch, int* cap);
 /* Frame glue of frame `frame` of the last batch: mvuRight / mvDepth (Frame::ComputeStereoFromRGBD, src/Frame.cc:850-871), the
  * world point Frame::UnprojectStereo gives per keypoint under that frame's pose (:879-899) and whether the keypoint has
  * depth; host arrays of at least the handle's keypoint capacity (NULL = skip). */
 int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, float* xw, uint8_t* valid, int cap);
-/* Masked batches: the `perfect` variant's live path per frame (perfect/src/Tracking.cc:703-719).  Between extraction and the
- * frame glue, one kernel per batch does Flow::ComputeMask after calcOpticalFlowFarneback (perfect/src/Flow.cc:14-53: pyrUp
- * of the flow, mask = 0 where x*x + y*y >= max(binary_threshold, 40), erode, erode, dilate with the 21 x 21 ellipse) and
- * the keypoint loop of the masked RGB-D Frame constructor (perfect/src/Frame.cc:328-427, :356-377: when the mask's sum is
- * above 65 % of the pixels, keypoints whose pixel is not 1 are dropped with their descriptors, order kept).  Frame t is
- * then tracked against the filtered frame t-1 with SearchByProjection(cur, last) (perfect/src/Tracking.cc:1933), and
- * orbs_read_dynamic_mask returns the mask FrameDrawer receives (perfect/src/FrameDrawer.cc:262).
- * flow[n][rows/2][cols/2][2] f32 is what calcOpticalFlowFarneback returns for the pyrDown'ed previous and current gray
- * images (CV_32FC2, continuous); mask pixels beyond the 2 (rows/2) x 2 (cols/2) it covers stay 1.  A frame without a
- * previous image (the sequence's first) takes a zero flow field: its mask is all ones and it keeps every keypoint, the
- * reference's `mask = ones` case.  Outputs keep the layout of the unmasked entries and describe the FILTERED frames
- * (nkp, kps, desc, cur2last against frame t-1's filtered keypoints), as do orbs_device_results and orbs_read_frame_glue.
- * Geometry: a frame's mask is held as two bit planes in one CTA's shared memory, 8 * rows * ceil(cols / 32) + 132 bytes;
- * on an H100 (232448 bytes per CTA) rows * ceil(cols / 32) <= 29039: 1280 x 720 and 1241 x 376 fit, 1280 x 725 is the
- * largest 1280-wide image.  Larger images and flow fields under 2 x 2 return B200ORB_EINVAL before anything is enqueued.
- * A masked batch launches one kernel more than the same unmasked batch; orbx_profile_read counts its time in stage 5. */
-int orbs_track_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                                const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                                uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
-/* Streaming form (as orbs_submit_batch_u16): flow is page-locked too and goes up chunk by chunk next to the gray images. */
-int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                                 const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                                 uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
-/* Masked batches whose flow the device computes (perfect/src/Flow.cc:26-29, as dynm_flow_batch_device) from the gray
- * images these entries upload anyway: the same arguments and outputs as the _masked pair, with prev_gray -- the rows x
- * cols u8 frame before gray[0], page-locked for the submit form -- in place of flow.  prev_gray NULL: the sequence starts
- * at gray[0], which takes the zero field.  Nothing but prev_gray is uploaded beyond what orbs_track_batch_u16 uploads.
- * The predecessor is an argument rather than handle state, so two handles chained with orbs_chain_after can carry one
- * sequence: each batch passes the last gray frame of the batch before.  Sizes dynm_flow_batch_device rejects return
- * B200ORB_EINVAL before anything is enqueued. */
-int orbs_track_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                              const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                              uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
-int orbs_submit_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                               const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                               uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap);
-/* Device-resident form (as orbs_track_batch_device), d_flow in HBM. */
-int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,
-                                   float binary_threshold, int nframes, int rows, int cols);
 /* Frame `frame` of the last batch, which must have been masked: mask[rows][cols] 0 / 1 (the Flow::ComputeMask result,
  * FrameDrawer's mDynMask), *filtered = whether the 65 % rule dropped keypoints of this frame (NULL = skip either). */
 int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered);

@@ -48,6 +48,16 @@ class OrbsParams(C.Structure):
                 ("max_frames", C.c_int)]
 
 
+class OrbsBatch(C.Structure):
+    _fields_ = [("nframes", C.c_int), ("rows", C.c_int), ("cols", C.c_int), ("device", C.c_int), ("gray", vp),
+                ("depth", vp), ("depth_u16", vp), ("depth_factor", C.c_float), ("Tcw", vp), ("flow", vp),
+                ("device_flow", C.c_int), ("prev_gray", vp), ("binary_threshold", C.c_float)]
+
+
+class OrbsResults(C.Structure):
+    _fields_ = [("kps", vp), ("desc", vp), ("nkp", vp), ("cur2last", vp), ("nmatch", vp), ("cap", C.c_int)]
+
+
 class OcmParams(C.Structure):
     _fields_ = [("resolution", C.c_double), ("prob_hit", C.c_double), ("prob_miss", C.c_double),
                 ("clamp_min", C.c_double), ("clamp_max", C.c_double), ("depth_min", C.c_float),

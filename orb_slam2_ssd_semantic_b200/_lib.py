@@ -15,7 +15,7 @@ class B200OrbError(RuntimeError):
         self.code = code
 
 
-from ._abi import OrbmFrustumPoints, OrbmTriKF, OcmParams, OrbmBow, OrbmFrame, OrbmLast, OrbmQueries, OrbmTrackPoints, OrbsParams, OrbxParams  # noqa: E402,F401
+from ._abi import OrbmFrustumPoints, OrbmTriKF, OcmParams, OrbmBow, OrbmFrame, OrbmLast, OrbmQueries, OrbmTrackPoints, OrbsBatch, OrbsParams, OrbsResults, OrbxParams  # noqa: E402,F401
 
 
 _lib = None
@@ -32,9 +32,8 @@ EXPORTS = [
     "orbm_search_by_projection_points", "orbm_search_by_bow", "orbm_search_by_bow_kf", "orbm_search_projected", "orbm_search_best", "orbm_search_for_initialization", "orbm_search_for_triangulation", "orbm_is_in_frustum", "orbm_undistort_keypoints", "orbv_create", "orbv_destroy", "orbv_num_words", "orbv_launch_count", "orbv_transform",
     "orbv_db_create", "orbv_db_destroy", "orbv_db_add", "orbv_db_erase", "orbv_db_clear", "orbv_db_query", "orbv_db_state",
     "orbv_db_launch_count",
-    "orbs_create", "orbs_destroy", "orbs_track_batch", "orbs_track_batch_u16", "orbs_submit_batch_u16", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_track_batch_device", "orbs_device_results", "orbs_read_frame_glue", "orbs_sync",
-    "orbs_track_batch_u16_masked", "orbs_submit_batch_u16_masked", "orbs_track_batch_masked_device", "orbs_read_dynamic_mask",
-    "orbs_track_batch_u16_flow", "orbs_submit_batch_u16_flow",
+    "orbs_create", "orbs_destroy", "orbs_submit", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_device_results",
+    "orbs_read_frame_glue", "orbs_sync", "orbs_read_dynamic_mask",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
     "gcm_add_keyframe_objects", "gcm_add_keyframe_objects_device",
@@ -145,19 +144,11 @@ def lib() -> C.CDLL:
     L.orbs_create.argtypes = [C.POINTER(OrbsParams), i, C.POINTER(vp)]
     L.orbs_destroy.argtypes = [vp]
     L.orbs_destroy.restype = None
-    L.orbs_track_batch.argtypes = [vp, vp, vp, vp, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_track_batch_u16.argtypes = [vp, vp, vp, C.c_float, vp, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_submit_batch_u16.argtypes = [vp, vp, vp, C.c_float, vp, i, i, i, vp, vp, vp, vp, vp, i]
+    L.orbs_submit.argtypes = [vp, C.POINTER(OrbsBatch), C.POINTER(OrbsResults)]
     L.orbs_set_chunk_frames.argtypes = [vp, i]
     L.orbs_chain_after.argtypes = [vp, vp]
-    L.orbs_track_batch_device.argtypes = [vp, vp, vp, vp, i, i, i]
     L.orbs_device_results.argtypes = [vp] + [C.POINTER(vp)] * 5 + [C.POINTER(i)]
     L.orbs_read_frame_glue.argtypes = [vp, i, vp, vp, vp, vp, i]
-    L.orbs_track_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_submit_batch_u16_masked.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_track_batch_u16_flow.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_submit_batch_u16_flow.argtypes = [vp, vp, vp, C.c_float, vp, vp, C.c_float, i, i, i, vp, vp, vp, vp, vp, i]
-    L.orbs_track_batch_masked_device.argtypes = [vp, vp, vp, vp, vp, C.c_float, i, i, i]
     L.orbs_read_dynamic_mask.argtypes = [vp, i, vp, C.POINTER(i)]
     L.orbs_sync.argtypes = [vp]
     L.orbs_stream.argtypes = [vp]

@@ -112,7 +112,7 @@ __global__ void k_fill_i32(int* p, int v, size_t n) {
 
 }  // namespace b200
 
-// The host-buffer entries upload a batch in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
+// Host batches are uploaded in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
 static constexpr int MAX_CHUNKS = 7;
 
 struct orbs {
@@ -129,7 +129,7 @@ struct orbs {
   uint8_t* d_valid = nullptr;
   int *d_c2l = nullptr, *d_nm = nullptr, *d_acc = nullptr;
   void* d_match_scratch = nullptr;
-  // Host-input block, carved by the first host-buffer call: the uploaded inputs and the depth under the keypoints.
+  // Host-input block, carved by the first host batch: the uploaded inputs and the depth under the keypoints.
   DeviceBlock in;
   int in_depth_bytes = -1;  // depth staging per pixel it holds: 4 for f32 input, 2 for pageable CV_16U, 0 for page-locked,
                             // -1 while it holds no inputs of the current geometry
@@ -138,24 +138,23 @@ struct orbs {
   uint16_t* d_kpd16 = nullptr;    // [maxF][cap] CV_16U depth under the keypoints
   void* d_depth = nullptr;        // [maxF][rows][cols] uploaded depth, f32 or CV_16U
   const uint16_t* gather_src = nullptr;   // the CV_16U batch k_depth_prefetch reads during a call
-  int chunk_frames = 128;   // frames per upload chunk of the host-buffer entries
+  int chunk_frames = 128;   // frames per upload chunk of host batches
   Stream copy_stream;
   Stream gather_stream;     // k_depth_prefetch, beside the extractor's stream
   Event chunk_ev[MAX_CHUNKS];
   Event inputs_free_ev;     // the previous call's kernels are done with the host-input block
   Event sel_ev, gather_ev;
-  Event compute_done_ev;    // recorded after the last kernel of a host-buffer batch (before its downloads)
-  orbs* chain_prev = nullptr;              // orbs_chain_after: the next batch's kernels wait for that handle's kernels
-  // Dynamic-mask block, reserved by the first masked call: the final bit plane and mask sum per frame, and the flow the
-  // host-buffer entries upload.
+  Event compute_done_ev;    // recorded after the last kernel of a host batch (before its downloads)
+  orbs* chain_prev = nullptr;              // orbs_chain_after: the next host batch's kernels wait for that handle's kernels
+  // Dynamic-mask block, reserved by the first masked batch: the final bit plane and mask sum per frame, and the flow of
+  // host batches (uploaded or computed on the device).
   DeviceBlock dyn;
   uint32_t* d_plane = nullptr;   // [maxF][rows][ceil(cols / 32)]
   unsigned* d_msum = nullptr;    // [maxF]
   float* d_flow = nullptr;       // [maxF][rows / 2][cols / 2][2]
-  uint8_t* d_prev_gray = nullptr;   // the _flow entries' prev_gray
+  uint8_t* d_prev_gray = nullptr;   // prev_gray of batches with device_flow
   FbGeom fbg;                       // and their Farneback geometry and scratch (chunks of min(maxF, FB_CHUNK) frames)
   FbScratch fbs{};
-  bool masked = false;           // the running batch went through mask_filter
   int mask_F = 0;                // frames of the last batch that carry a dynamic mask (0: it was not masked)
   bool have = false;
   int create_streams() {
@@ -165,7 +164,7 @@ struct orbs {
     for (Event* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev}) B200_CHECK(e->create());
     return B200ORB_OK;
   }
-  // depth_bytes: depth staging per pixel a host-buffer call needs; -1 for the device entry, which needs no host-input
+  // depth_bytes: depth staging per pixel a host batch needs; -1 for a device batch, which needs no host-input
   // block.  Either block is replaced only after the stream is synchronised: every copy-stream and gather-stream
   // operation of earlier calls is joined into it by an event.
   int ensure(int r, int c, int F, int depth_bytes) {
@@ -195,7 +194,7 @@ struct orbs {
     }
     return B200ORB_OK;
   }
-  // Masked entries, before they touch any state: the flow field is at least 2 x 2 and both bit planes of a frame fit one
+  // Masked batches, before they touch any state: the flow field is at least 2 x 2 and both bit planes of a frame fit one
   // CTA's shared memory (on an H100, 232448 bytes: rows * ceil(cols / 32) <= 29039, e.g. 1280 x 725).
   int check_masked(int r, int c) const {
     B200_CHECK(dynm_check_geometry(r / 2, c / 2, r, c));
@@ -209,11 +208,12 @@ struct orbs {
     }
     return B200ORB_OK;
   }
-  // host_flow: d_flow receives the caller's flow; dev_flow: the device computes it there (and needs the Farneback scratch)
-  int ensure_dyn(bool host_flow, bool dev_flow = false) {
+  // host_flow: d_flow receives the caller's flow; dev_flow (the Farneback geometry of the batch, or NULL): the device
+  // computes it there and needs the Farneback scratch
+  int ensure_dyn(bool host_flow, const FbGeom* dev_flow) {
     const size_t planes = (size_t)maxF * rows * dynp_words(cols);
     const size_t flow = host_flow || dev_flow ? (size_t)maxF * (rows / 2) * (cols / 2) * 2 : 0;
-    if (dev_flow) B200_CHECK(fb_geometry(rows / 2, cols / 2, &fbg));
+    if (dev_flow) fbg = *dev_flow;
     return dyn.reserve(ex->stream, [&](Carver& t) {
       d_plane = t.take<uint32_t>(planes); d_msum = t.take<unsigned>(maxF); d_flow = t.take<float>(flow);
       d_prev_gray = nullptr;
@@ -229,14 +229,13 @@ struct orbs {
   // them.  dflow: [F][rows / 2][cols / 2][2] f32.
   int mask_filter(const float* dflow, float thr, uint16_t* kpd16, int F) {
     if (thr < 40.0f) thr = 40.0f;   // perfect/src/Flow.cc:24
-    B200_CHECK(launch_dynm_plane_filter(F, dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum, ex->d_kps, ex->d_desc,
-                                        kpd16, ex->d_n, cap, ex->stream, &launches));
-    masked = true;
-    return B200ORB_OK;
+    return launch_dynm_plane_filter(F, dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum, ex->d_kps, ex->d_desc,
+                                    kpd16, ex->d_n, cap, ex->stream, &launches);
   }
   // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  Depth is the gathered CV_16U
-  // value under each keypoint times `factor` when kpd16 is given, else the f32 image batch dd.
-  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F) {
+  // value under each keypoint times `factor` when kpd16 is given, else the f32 image batch dd.  masked: the frames went
+  // through mask_filter, so orbs_read_dynamic_mask may read their masks.
+  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool masked) {
     cudaStream_t st = ex->stream;
     GlueOut go{d_x, d_y, d_ang, d_ur, d_dep, d_xw, d_oct, d_valid};
     k_frame_glue<<<dim3((cap + 255) / 256, F), 256, 0, st>>>(ex->d_kps, ex->d_n, cap, dd, kpd16, factor, rows, cols, dT, prm.fx, prm.fy,
@@ -269,7 +268,6 @@ struct orbs {
     B200_CHECK(ex->prof_mark(ST_MATCH + 1));
     lastF = F;
     mask_F = masked ? F : 0;
-    masked = false;
     have = true;
     return B200ORB_OK;
   }
@@ -293,15 +291,6 @@ int orbs_create(const OrbsParams* p, int device, orbs_t** out) {
   return B200ORB_OK;
 }
 void orbs_destroy(orbs_t* h) { destroy_handle(h); }
-
-int orbs_track_batch_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, int nframes,
-                            int rows, int cols) {
-  if (!h || !d_gray || !d_depth || !d_Tcw || nframes <= 0 || rows <= 0 || cols <= 0) { set_error("bad argument"); return B200ORB_EINVAL; }
-  DeviceGuard g(h->device);
-  B200_CHECK(h->ensure(rows, cols, nframes, -1));
-  B200_CHECK(h->ex->run(d_gray, cols, (size_t)rows * cols, nframes));
-  return h->run(d_depth, nullptr, 0.f, d_Tcw, nframes);
-}
 
 int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d_desc, const int32_t** d_nkp,
                         const int32_t** d_cur2last, const int32_t** d_nmatch, int* cap) {
@@ -330,7 +319,7 @@ int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, floa
   return B200ORB_OK;
 }
 
-// orbx::after_select hook of the CV_16U entries: the keypoints of frames [f0, f0 + F) are selected -> fetch the depth
+// orbx::after_select hook of CV_16U batches: the keypoints of frames [f0, f0 + F) are selected -> fetch the depth
 // under them on the side stream (the stream of the extractor goes on with blur and descriptors meanwhile)
 static int orbs_after_select(void* ctx, int f0, int F) {
   orbs* h = static_cast<orbs*>(ctx);
@@ -346,169 +335,126 @@ static int orbs_after_select(void* ctx, int f0, int F) {
   return B200ORB_OK;
 }
 
-static int track_batch_host(orbs_t* h, const uint8_t* gray, const float* depth, const uint16_t* depth16, float factor,
-                            const float* Tcw, int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc,
-                            int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap, bool wait = true,
-                            const float* flow = nullptr, float thr = 0.f, bool dev_flow = false,
-                            const uint8_t* prev_gray = nullptr) {
-  if (!h || !gray || (!depth && !depth16) || !Tcw || !kps || !desc || !nkp || !cur2last || !nmatch || nframes <= 0 ||
-      rows <= 0 || cols <= 0) {
-    set_error("bad argument");
-    return B200ORB_EINVAL;
+// The seven batch forms include/b200orb.h lists under OrbsBatch; every other combination is refused.
+static bool batch_form_ok(const OrbsBatch* b, const OrbsResults* out) {
+  if (!b->gray || !b->Tcw || b->nframes <= 0 || b->rows <= 0 || b->cols <= 0) return false;
+  if (!b->depth == !b->depth_u16 || (b->flow && b->device_flow) || (b->prev_gray && !b->device_flow)) return false;
+  if (b->device) return !out && b->depth && !b->device_flow;
+  return out && out->kps && out->desc && out->nkp && out->cur2last && out->nmatch &&
+         (b->depth_u16 || !(b->flow || b->device_flow));
+}
+
+// Host batch: the inputs go up in chunks on a copy stream while the extractor already works on the chunks that have
+// arrived (PCIe and SMs overlap); everything after extraction runs on the whole batch.  d16_alias: the device alias of
+// page-locked CV_16U depth, read in place; depth_bytes: the depth uploaded per pixel.
+static int upload_and_extract(orbs_t* h, const OrbsBatch* b, const uint16_t* d16_alias, int depth_bytes) {
+  cudaStream_t st = h->ex->stream;
+  const int cols = b->cols;
+  const size_t px = (size_t)b->rows * cols, F = b->nframes, fpx = (size_t)(b->rows / 2) * (cols / 2) * 2;
+  const char* depth_up = b->depth ? (const char*)b->depth : (const char*)b->depth_u16;
+  const int nchunk = (int)std::min<size_t>(MAX_CHUNKS, (F + h->chunk_frames - 1) / h->chunk_frames);   // >= 64-frame chunks keep each launch wide enough
+  h->gather_src = d16_alias ? d16_alias : static_cast<const uint16_t*>(h->d_depth);
+  h->ex->after_select = b->depth_u16 ? &orbs_after_select : nullptr;
+  h->ex->after_select_ctx = h;
+  B200_CUDA(cudaEventRecord(h->inputs_free_ev, st));
+  B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->inputs_free_ev, 0));
+  // orbs_chain_after: this batch's kernels start when the other handle's kernels are done -- the uploads enqueued
+  // below (copy stream) and that handle's downloads run meanwhile, and kernels of two batches never share the SMs.
+  // The uploads start only once that handle's in-place depth reads (k_depth_prefetch) are done: both cross the host
+  // link toward the device, the reads are latency-bound and its matcher waits for them, while these uploads are
+  // needed only when this batch's kernels start.
+  if (h->chain_prev) {
+    B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
+    B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->chain_prev->gather_ev, 0));
   }
-  if (flow || dev_flow) B200_CHECK(h->check_masked(rows, cols));
-  if (dev_flow) {
-    FbGeom fg;
-    B200_CHECK(fb_geometry(rows / 2, cols / 2, &fg));
+  h->chain_prev = nullptr;
+  if (b->prev_gray)
+    B200_CUDA(cudaMemcpyAsync(h->d_prev_gray, b->prev_gray, px, cudaMemcpyHostToDevice, h->copy_stream));
+  for (int c = 0; c < nchunk; ++c) {
+    const size_t f0 = F * c / nchunk, f1 = F * (c + 1) / nchunk;
+    B200_CUDA(cudaMemcpyAsync(h->d_gray + px * f0, b->gray + px * f0, px * (f1 - f0), cudaMemcpyHostToDevice, h->copy_stream));
+    const size_t o = px * f0 * depth_bytes;
+    if (depth_bytes)
+      B200_CUDA(cudaMemcpyAsync((char*)h->d_depth + o, depth_up + o, px * (f1 - f0) * depth_bytes, cudaMemcpyHostToDevice,
+                                h->copy_stream));
+    if (b->flow)
+      B200_CUDA(cudaMemcpyAsync(h->d_flow + fpx * f0, b->flow + fpx * f0, fpx * (f1 - f0) * 4, cudaMemcpyHostToDevice,
+                                h->copy_stream));
+    B200_CUDA(cudaEventRecord(h->chunk_ev[c], h->copy_stream));
+    B200_CUDA(cudaStreamWaitEvent(st, h->chunk_ev[c], 0));
+    B200_CHECK(h->ex->run(h->d_gray + px * f0, cols, px, (int)(f1 - f0), (int)f0));
   }
+  h->ex->after_select = nullptr;
+  if (b->depth_u16) B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
+  return B200ORB_OK;
+}
+
+// Host batch: the results of the F frames go down into `out` behind the batch's kernels.
+static int download(orbs_t* h, const OrbsResults* out, size_t F) {
+  cudaStream_t st = h->ex->stream;
+  const size_t hc = h->cap, cap = out->cap;
+  if (cap == hc) {
+    B200_CUDA(cudaMemcpyAsync(out->kps, h->ex->d_kps, sizeof(OrbxKeyPoint) * hc * F, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpyAsync(out->desc, h->ex->d_desc, 32 * hc * F, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpyAsync(out->cur2last, h->d_c2l, 4 * hc * F, cudaMemcpyDeviceToHost, st));
+  } else {
+    B200_CUDA(cudaMemcpy2DAsync(out->kps, sizeof(OrbxKeyPoint) * cap, h->ex->d_kps, sizeof(OrbxKeyPoint) * hc,
+                                sizeof(OrbxKeyPoint) * hc, F, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpy2DAsync(out->desc, 32 * cap, h->ex->d_desc, 32 * hc, 32 * hc, F, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaMemcpy2DAsync(out->cur2last, 4 * cap, h->d_c2l, 4 * hc, 4 * hc, F, cudaMemcpyDeviceToHost, st));
+  }
+  B200_CUDA(cudaMemcpyAsync(out->nkp, h->ex->d_n, 4 * F, cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaMemcpyAsync(out->nmatch, h->d_nm, 4 * F, cudaMemcpyDeviceToHost, st));
+  return B200ORB_OK;
+}
+
+int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
+  if (!h || !b || !batch_form_ok(b, out)) { set_error("bad argument"); return B200ORB_EINVAL; }
+  const int F = b->nframes, rows = b->rows, cols = b->cols;
+  const bool masked = b->flow || b->device_flow;
+  if (masked) B200_CHECK(h->check_masked(rows, cols));
+  FbGeom fg;
+  if (b->device_flow) B200_CHECK(fb_geometry(rows / 2, cols / 2, &fg));
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
   // Page-locked depth (cudaHostAlloc / cudaHostRegister, e.g. torch.pin_memory) is read in place over PCIe, so its
   // 0.6 MB/frame images are never uploaded; pageable depth is uploaded next to the gray images and read from HBM.
   const uint16_t* d16_alias = nullptr;
-  if (depth16) {
+  if (b->depth_u16) {
     cudaPointerAttributes at;
     void* dev_alias = nullptr;
-    if (cudaPointerGetAttributes(&at, depth16) == cudaSuccess && at.type == cudaMemoryTypeHost &&
-        cudaHostGetDevicePointer(&dev_alias, const_cast<uint16_t*>(depth16), 0) == cudaSuccess && dev_alias)
+    if (cudaPointerGetAttributes(&at, b->depth_u16) == cudaSuccess && at.type == cudaMemoryTypeHost &&
+        cudaHostGetDevicePointer(&dev_alias, const_cast<uint16_t*>(b->depth_u16), 0) == cudaSuccess && dev_alias)
       d16_alias = reinterpret_cast<const uint16_t*>(dev_alias);
     else
       cudaGetLastError();
   }
-  const int depth_bytes = depth ? 4 : (d16_alias ? 0 : 2);   // per pixel uploaded
-  const char* depth_up = depth ? (const char*)depth : (const char*)depth16;
-  B200_CHECK(h->ensure(rows, cols, nframes, depth_bytes));
-  if (cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", cap, h->cap); return B200ORB_ECAP; }
-  if (flow || dev_flow) B200_CHECK(h->ensure_dyn(flow != nullptr, dev_flow));
-  cudaStream_t st = h->ex->stream;
-  const size_t px = (size_t)rows * cols, F = nframes, fpx = (size_t)(rows / 2) * (cols / 2) * 2;
-  // the inputs go up in chunks on a copy stream while the extractor already works on the chunks that have arrived
-  // (PCIe and SMs overlap); everything after extraction runs on the whole batch.
-  const int nchunk = (int)std::min<size_t>(MAX_CHUNKS, (F + h->chunk_frames - 1) / h->chunk_frames);   // >= 64-frame chunks keep each launch wide enough
-  h->gather_src = d16_alias ? d16_alias : static_cast<const uint16_t*>(h->d_depth);
-  h->ex->after_select = depth16 ? &orbs_after_select : nullptr;
-  h->ex->after_select_ctx = h;
-  {
-    B200_CUDA(cudaEventRecord(h->inputs_free_ev, st));
-    B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->inputs_free_ev, 0));
-    // orbs_chain_after: this batch's kernels start when the other handle's kernels are done -- the uploads enqueued
-    // below (copy stream) and that handle's downloads run meanwhile, and kernels of two batches never share the SMs.
-    // The uploads start only once that handle's in-place depth reads (k_depth_prefetch) are done: both cross the host
-    // link toward the device, the reads are latency-bound and its matcher waits for them, while these uploads are
-    // needed only when this batch's kernels start.
-    if (h->chain_prev) {
-      B200_CUDA(cudaStreamWaitEvent(st, h->chain_prev->compute_done_ev, 0));
-      B200_CUDA(cudaStreamWaitEvent(h->copy_stream, h->chain_prev->gather_ev, 0));
-    }
-    h->chain_prev = nullptr;
-    if (dev_flow && prev_gray)
-      B200_CUDA(cudaMemcpyAsync(h->d_prev_gray, prev_gray, px, cudaMemcpyHostToDevice, h->copy_stream));
-    for (int c = 0; c < nchunk; ++c) {
-      const size_t f0 = F * c / nchunk, f1 = F * (c + 1) / nchunk;
-      B200_CUDA(cudaMemcpyAsync(h->d_gray + px * f0, gray + px * f0, px * (f1 - f0), cudaMemcpyHostToDevice, h->copy_stream));
-      const size_t o = px * f0 * depth_bytes;
-      if (depth_bytes)
-        B200_CUDA(cudaMemcpyAsync((char*)h->d_depth + o, depth_up + o, px * (f1 - f0) * depth_bytes, cudaMemcpyHostToDevice,
-                                  h->copy_stream));
-      if (flow)
-        B200_CUDA(cudaMemcpyAsync(h->d_flow + fpx * f0, flow + fpx * f0, fpx * (f1 - f0) * 4, cudaMemcpyHostToDevice,
-                                  h->copy_stream));
-      B200_CUDA(cudaEventRecord(h->chunk_ev[c], h->copy_stream));
-      B200_CUDA(cudaStreamWaitEvent(st, h->chunk_ev[c], 0));
-      B200_CHECK(h->ex->run(h->d_gray + px * f0, cols, px, (int)(f1 - f0), (int)f0));
-    }
-  }
-  h->ex->after_select = nullptr;
-  if (depth16) B200_CUDA(cudaStreamWaitEvent(st, h->gather_ev, 0));   // the last chunk's prefetch (the side stream is in order)
-  if (dev_flow)
-    B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, prev_gray ? h->d_prev_gray : nullptr, nframes, rows, cols,
-                        h->d_flow, &h->launches));
-  if (flow || dev_flow) B200_CHECK(h->mask_filter(h->d_flow, thr, depth16 ? h->d_kpd16 : nullptr, nframes));
-  B200_CUDA(cudaMemcpyAsync(h->d_T, Tcw, F * 64, cudaMemcpyHostToDevice, st));
-  B200_CHECK(h->run(depth ? static_cast<const float*>(h->d_depth) : nullptr, depth16 ? h->d_kpd16 : nullptr, factor, h->d_T,
-                    nframes));
-  B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
-  const size_t hc = h->cap;
-  if ((size_t)cap == hc) {
-    B200_CUDA(cudaMemcpyAsync(kps, h->ex->d_kps, sizeof(OrbxKeyPoint) * hc * F, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaMemcpyAsync(desc, h->ex->d_desc, 32 * hc * F, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaMemcpyAsync(cur2last, h->d_c2l, 4 * hc * F, cudaMemcpyDeviceToHost, st));
+  const int depth_bytes = b->device ? -1 : b->depth ? 4 : (d16_alias ? 0 : 2);   // per pixel uploaded
+  B200_CHECK(h->ensure(rows, cols, F, depth_bytes));
+  if (out && out->cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", out->cap, h->cap); return B200ORB_ECAP; }
+  if (masked) B200_CHECK(h->ensure_dyn(b->flow && !b->device, b->device_flow ? &fg : nullptr));
+  // Device batch: every input is read in place from HBM.  Host batch: from the uploaded copies.
+  const float *dd = b->depth, *dflow = b->flow, *dT = b->Tcw;
+  if (b->device) {
+    B200_CHECK(h->ex->run(b->gray, cols, (size_t)rows * cols, F));
   } else {
-    B200_CUDA(cudaMemcpy2DAsync(kps, sizeof(OrbxKeyPoint) * cap, h->ex->d_kps, sizeof(OrbxKeyPoint) * hc,
-                                sizeof(OrbxKeyPoint) * hc, F, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaMemcpy2DAsync(desc, (size_t)32 * cap, h->ex->d_desc, 32 * hc, 32 * hc, F, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaMemcpy2DAsync(cur2last, (size_t)4 * cap, h->d_c2l, 4 * hc, 4 * hc, F, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(upload_and_extract(h, b, d16_alias, depth_bytes));
+    dd = b->depth ? static_cast<const float*>(h->d_depth) : nullptr;
+    dflow = h->d_flow;
+    dT = h->d_T;
   }
-  B200_CUDA(cudaMemcpyAsync(nkp, h->ex->d_n, 4 * F, cudaMemcpyDeviceToHost, st));
-  B200_CUDA(cudaMemcpyAsync(nmatch, h->d_nm, 4 * F, cudaMemcpyDeviceToHost, st));
-  if (wait) B200_CUDA(cudaStreamSynchronize(st));
-  return B200ORB_OK;
-}
-
-int orbs_track_batch(orbs_t* h, const uint8_t* gray, const float* depth, const float* Tcw, int nframes, int rows,
-                     int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch,
-                     int cap) {
-  return track_batch_host(h, gray, depth, nullptr, 0.f, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last, nmatch, cap);
-}
-
-int orbs_track_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                         int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
-                         int32_t* cur2last, int32_t* nmatch, int cap) {
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap);
-}
-
-int orbs_submit_batch_u16(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                          int nframes, int rows, int cols, OrbxKeyPoint* kps, uint8_t* desc, int32_t* nkp,
-                          int32_t* cur2last, int32_t* nmatch, int cap) {
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap, /*wait=*/false);
-}
-
-int orbs_track_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                                const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                                uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
-  if (!flow) { set_error("bad argument"); return B200ORB_EINVAL; }
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap, /*wait=*/true, flow, binary_threshold);
-}
-
-int orbs_submit_batch_u16_masked(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                                 const float* flow, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                                 uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
-  if (!flow) { set_error("bad argument"); return B200ORB_EINVAL; }
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap, /*wait=*/false, flow, binary_threshold);
-}
-
-int orbs_track_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                              const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                              uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap, /*wait=*/true, nullptr, binary_threshold, /*dev_flow=*/true, prev_gray);
-}
-
-int orbs_submit_batch_u16_flow(orbs_t* h, const uint8_t* gray, const uint16_t* depth_u16, float depth_factor, const float* Tcw,
-                               const uint8_t* prev_gray, float binary_threshold, int nframes, int rows, int cols, OrbxKeyPoint* kps,
-                               uint8_t* desc, int32_t* nkp, int32_t* cur2last, int32_t* nmatch, int cap) {
-  return track_batch_host(h, gray, nullptr, depth_u16, depth_factor, Tcw, nframes, rows, cols, kps, desc, nkp, cur2last,
-                          nmatch, cap, /*wait=*/false, nullptr, binary_threshold, /*dev_flow=*/true, prev_gray);
-}
-
-int orbs_track_batch_masked_device(orbs_t* h, const uint8_t* d_gray, const float* d_depth, const float* d_Tcw, const float* d_flow,
-                                   float binary_threshold, int nframes, int rows, int cols) {
-  if (!h || !d_gray || !d_depth || !d_Tcw || !d_flow || nframes <= 0 || rows <= 0 || cols <= 0) {
-    set_error("bad argument");
-    return B200ORB_EINVAL;
-  }
-  B200_CHECK(h->check_masked(rows, cols));
-  DeviceGuard g(h->device);
-  B200_CHECK(h->ensure(rows, cols, nframes, -1));
-  B200_CHECK(h->ensure_dyn(false));
-  B200_CHECK(h->ex->run(d_gray, cols, (size_t)rows * cols, nframes));
-  B200_CHECK(h->mask_filter(d_flow, binary_threshold, nullptr, nframes));
-  return h->run(d_depth, nullptr, 0.f, d_Tcw, nframes);
+  cudaStream_t st = h->ex->stream;
+  if (b->device_flow)
+    B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, b->prev_gray ? h->d_prev_gray : nullptr, F, rows, cols,
+                        h->d_flow, &h->launches));
+  uint16_t* kpd16 = b->depth_u16 ? h->d_kpd16 : nullptr;
+  if (masked) B200_CHECK(h->mask_filter(dflow, b->binary_threshold, kpd16, F));
+  if (!b->device) B200_CUDA(cudaMemcpyAsync(h->d_T, b->Tcw, (size_t)F * 64, cudaMemcpyHostToDevice, st));
+  B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, masked));
+  if (b->device) return B200ORB_OK;
+  B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
+  return download(h, out, F);
 }
 
 // The dynamic mask of frame `frame` of the last batch, if that batch was masked: FrameDrawer's mDynMask
@@ -533,7 +479,7 @@ int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered) {
   return B200ORB_OK;
 }
 
-// frames per upload chunk of the host-buffer entries (default 128; at most MAX_CHUNKS per call): smaller chunks start the
+// frames per upload chunk of host batches (default 128; at most MAX_CHUNKS per call): smaller chunks start the
 // extraction earlier, larger ones keep the launches wider
 int orbs_set_chunk_frames(orbs_t* h, int frames) {
   if (!h || frames <= 0) { set_error("bad argument"); return B200ORB_EINVAL; }
@@ -541,7 +487,7 @@ int orbs_set_chunk_frames(orbs_t* h, int frames) {
   return B200ORB_OK;
 }
 
-// The next host-buffer batch submitted to `h` starts its kernels only when the kernels of `prev`'s last submitted batch
+// The next host batch submitted to `h` starts its kernels only when the kernels of `prev`'s last submitted batch
 // are done, and its uploads only when `prev`'s in-place depth reads are done.  Two handles submitted alternately with this form a 3-stage pipeline:
 // upload of batch k+1 | kernels of batch k | download of batch k-1.
 int orbs_chain_after(orbs_t* h, orbs_t* prev) {

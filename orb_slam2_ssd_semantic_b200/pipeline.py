@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._abi import OrbsParams, OrbxParams, ptr
+from ._abi import OrbsBatch, OrbsParams, OrbsResults, OrbxParams, ptr
 from .extractor import KP_DTYPE
 
 
@@ -48,48 +48,54 @@ class StreamTracker:
             outs.append(t.numpy().view(d).reshape(s))
         return tuple(outs)
 
+    _DTYPES = dict(gray=np.uint8, depth=np.float32, depth_u16=np.uint16, Tcw=np.float32, flow=np.float32, prev_gray=np.uint8)
+
+    def _host_batch(self, form: str, wait: bool, out, depth_factor=0.0, binary_threshold=0.0, **arrays):
+        """One host batch through orbs_submit.  arrays: gray, one depth, Tcw, and flow or prev_gray (the flow computed on
+        the device; None: the sequence starts at gray[0]).  The track_* forms (wait) convert the arrays and end in sync();
+        the submit_* forms take them as they are (no hidden copies) and return after enqueueing."""
+        for k, a in arrays.items():
+            if a is None and k == "prev_gray":
+                continue
+            dt = self._DTYPES[k]
+            if wait:
+                arrays[k] = np.ascontiguousarray(a, dt)
+            elif a.dtype != dt or not a.flags.c_contiguous:
+                raise ValueError("%s takes C-contiguous %s arrays (no hidden copies)" % (form, np.dtype(dt).name))
+        gray, Tcw, flow, prev = arrays["gray"], arrays["Tcw"], arrays.get("flow"), arrays.get("prev_gray")
+        F, rows, cols = gray.shape
+        assert arrays.get("depth", arrays.get("depth_u16")).shape == gray.shape and Tcw.size == F * 16
+        if "flow" in arrays and flow.shape != (F, rows // 2, cols // 2, 2):
+            raise ValueError("flow must be [nframes][rows/2][cols/2][2] float32, got %s" % (flow.shape,))
+        if prev is not None and (prev.dtype != np.uint8 or prev.shape != (rows, cols)):
+            raise ValueError("prev_gray must be a rows x cols uint8 image or None")
+        outs = out if out is not None else self.alloc_outputs(F)
+        b = OrbsBatch(F, rows, cols, 0, ptr(gray), ptr(arrays.get("depth")), ptr(arrays.get("depth_u16")),
+                      float(np.float32(depth_factor)), ptr(Tcw), ptr(flow), int("prev_gray" in arrays), ptr(prev),
+                      float(binary_threshold))
+        _lib.check(self._L.orbs_submit(self._h, C.byref(b), C.byref(OrbsResults(*[ptr(a) for a in outs], self.cap))))
+        if not wait:
+            return out
+        self.sync()
+        return tuple(outs)
+
+    def _device_batch(self, d_gray: int, d_depth: int, d_Tcw: int, d_flow, binary_threshold, nframes: int, rows: int,
+                      cols: int):
+        b = OrbsBatch(nframes, rows, cols, 1, d_gray, d_depth, None, 0.0, d_Tcw, d_flow, 0, None, float(binary_threshold))
+        _lib.check(self._L.orbs_submit(self._h, C.byref(b), None))
+
     def track_batch(self, gray: np.ndarray, depth: np.ndarray, Tcw: np.ndarray, out=None):
         """Host buffers in, host buffers out (the reference-facing call; copies are inside)."""
-        gray = np.ascontiguousarray(gray, np.uint8)
-        depth = np.ascontiguousarray(depth, np.float32)
-        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
-        F, rows, cols = gray.shape
-        assert depth.shape == gray.shape and Tcw.shape[0] == F
-        cap = self.cap
-        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
-        _lib.check(self._L.orbs_track_batch(self._h, ptr(gray), ptr(depth), ptr(Tcw), F, rows, cols, ptr(kps), ptr(desc),
-                                            ptr(nkp), ptr(c2l), ptr(nm), cap))
-        return kps, desc, nkp, c2l, nm
+        return self._host_batch("track_batch", True, out, gray=gray, depth=depth, Tcw=Tcw)
 
     def track_batch_u16(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray, out=None):
         """Like track_batch with the sensor's CV_16U depth; convertTo(CV_32F, depth_factor) runs on the device."""
-        gray = np.ascontiguousarray(gray, np.uint8)
-        depth_u16 = np.ascontiguousarray(depth_u16, np.uint16)
-        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.shape[0] == F
-        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
-        _lib.check(self._L.orbs_track_batch_u16(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)), ptr(Tcw),
-                                                F, rows, cols, ptr(kps), ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
-        return kps, desc, nkp, c2l, nm
+        return self._host_batch("track_batch_u16", True, out, depth_factor, gray=gray, depth_u16=depth_u16, Tcw=Tcw)
 
     def submit_batch_u16(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray, out):
         """Asynchronous track_batch_u16: returns after enqueueing; `out` (alloc_outputs(pinned=True)) is valid after
         sync().  The input arrays must be page-locked, C-contiguous and stay untouched until then."""
-        for a, dt in ((gray, np.uint8), (depth_u16, np.uint16), (Tcw, np.float32)):
-            if a.dtype != dt or not a.flags.c_contiguous:
-                raise ValueError("submit_batch_u16 takes C-contiguous %s arrays (no hidden copies)" % np.dtype(dt).name)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.size == F * 16
-        kps, desc, nkp, c2l, nm = out
-        _lib.check(self._L.orbs_submit_batch_u16(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)), ptr(Tcw),
-                                                 F, rows, cols, ptr(kps), ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
-        return out
-
-    @staticmethod
-    def _check_flow(flow: np.ndarray, F: int, rows: int, cols: int):
-        if flow.shape != (F, rows // 2, cols // 2, 2):
-            raise ValueError("flow must be [nframes][rows/2][cols/2][2] float32, got %s" % (flow.shape,))
+        return self._host_batch("submit_batch_u16", False, out, depth_factor, gray=gray, depth_u16=depth_u16, Tcw=Tcw)
 
     def track_batch_u16_masked(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
                                flow: np.ndarray, binary_threshold: float = 40.0, out=None):
@@ -97,83 +103,37 @@ class StreamTracker:
         mask of each frame computed on the device from its half-resolution optical flow (flow[n][rows/2][cols/2][2],
         calcOpticalFlowFarneback's output; a zero field for a frame without a predecessor) and the keypoints outside the
         mask dropped before tracking.  The outputs describe the filtered frames; dynamic_mask(frame) returns the masks."""
-        gray = np.ascontiguousarray(gray, np.uint8)
-        depth_u16 = np.ascontiguousarray(depth_u16, np.uint16)
-        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
-        flow = np.ascontiguousarray(flow, np.float32)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.shape[0] == F
-        self._check_flow(flow, F, rows, cols)
-        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
-        _lib.check(self._L.orbs_track_batch_u16_masked(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
-                                                       ptr(Tcw), ptr(flow), float(binary_threshold), F, rows, cols, ptr(kps),
-                                                       ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
-        return kps, desc, nkp, c2l, nm
+        return self._host_batch("track_batch_u16_masked", True, out, depth_factor, binary_threshold, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw, flow=flow)
 
     def submit_batch_u16_masked(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
                                 flow: np.ndarray, binary_threshold: float, out):
         """Asynchronous track_batch_u16_masked (as submit_batch_u16): every input, the flow included, must be page-locked,
         C-contiguous and untouched until sync()."""
-        for a, dt in ((gray, np.uint8), (depth_u16, np.uint16), (Tcw, np.float32), (flow, np.float32)):
-            if a.dtype != dt or not a.flags.c_contiguous:
-                raise ValueError("submit_batch_u16_masked takes C-contiguous %s arrays (no hidden copies)" % np.dtype(dt).name)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.size == F * 16
-        self._check_flow(flow, F, rows, cols)
-        kps, desc, nkp, c2l, nm = out
-        _lib.check(self._L.orbs_submit_batch_u16_masked(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
-                                                        ptr(Tcw), ptr(flow), float(binary_threshold), F, rows, cols, ptr(kps),
-                                                        ptr(desc), ptr(nkp), ptr(c2l), ptr(nm), self.cap))
-        return out
-
-    @staticmethod
-    def _check_prev(prev_gray, rows: int, cols: int):
-        if prev_gray is not None and (prev_gray.dtype != np.uint8 or prev_gray.shape != (rows, cols)):
-            raise ValueError("prev_gray must be a rows x cols uint8 image or None")
+        return self._host_batch("submit_batch_u16_masked", False, out, depth_factor, binary_threshold, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw, flow=flow)
 
     def track_batch_u16_flow(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
                              prev_gray=None, binary_threshold: float = 40.0, out=None):
         """track_batch_u16_masked with the optical flow computed on the device from the gray frames (pyrDown +
         calcOpticalFlowFarneback, perfect/src/Flow.cc:26-29): prev_gray is the frame before gray[0], None when the
         sequence starts at gray[0] (its flow is the zero field).  No flow crosses the host link."""
-        gray = np.ascontiguousarray(gray, np.uint8)
-        depth_u16 = np.ascontiguousarray(depth_u16, np.uint16)
-        Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.shape[0] == F
-        if prev_gray is not None:
-            prev_gray = np.ascontiguousarray(prev_gray, np.uint8)
-        self._check_prev(prev_gray, rows, cols)
-        kps, desc, nkp, c2l, nm = out if out is not None else self.alloc_outputs(F)
-        _lib.check(self._L.orbs_track_batch_u16_flow(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
-                                                     ptr(Tcw), None if prev_gray is None else ptr(prev_gray),
-                                                     float(binary_threshold), F, rows, cols, ptr(kps), ptr(desc), ptr(nkp),
-                                                     ptr(c2l), ptr(nm), self.cap))
-        return kps, desc, nkp, c2l, nm
+        return self._host_batch("track_batch_u16_flow", True, out, depth_factor, binary_threshold, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw, prev_gray=prev_gray)
 
     def submit_batch_u16_flow(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
                               prev_gray, binary_threshold: float, out):
         """Asynchronous track_batch_u16_flow (as submit_batch_u16): every input, prev_gray included, must be page-locked,
         C-contiguous and untouched until sync()."""
-        for a, dt in ((gray, np.uint8), (depth_u16, np.uint16), (Tcw, np.float32)) + \
-                (((prev_gray, np.uint8),) if prev_gray is not None else ()):
-            if a.dtype != dt or not a.flags.c_contiguous:
-                raise ValueError("submit_batch_u16_flow takes C-contiguous %s arrays (no hidden copies)" % np.dtype(dt).name)
-        F, rows, cols = gray.shape
-        assert depth_u16.shape == gray.shape and Tcw.size == F * 16
-        self._check_prev(prev_gray, rows, cols)
-        kps, desc, nkp, c2l, nm = out
-        _lib.check(self._L.orbs_submit_batch_u16_flow(self._h, ptr(gray), ptr(depth_u16), float(np.float32(depth_factor)),
-                                                      ptr(Tcw), None if prev_gray is None else ptr(prev_gray),
-                                                      float(binary_threshold), F, rows, cols, ptr(kps), ptr(desc), ptr(nkp),
-                                                      ptr(c2l), ptr(nm), self.cap))
-        return out
+        return self._host_batch("submit_batch_u16_flow", False, out, depth_factor, binary_threshold, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw, prev_gray=prev_gray)
 
     def track_batch_masked_device(self, d_gray: int, d_depth: int, d_Tcw: int, d_flow: int, binary_threshold: float,
                                   nframes: int, rows: int, cols: int):
         """track_batch_device with the dynamic mask; d_flow = [nframes][rows/2][cols/2][2] f32 in HBM. Asynchronous."""
-        _lib.check(self._L.orbs_track_batch_masked_device(self._h, C.c_void_p(d_gray), C.c_void_p(d_depth), C.c_void_p(d_Tcw),
-                                                          C.c_void_p(d_flow), float(binary_threshold), nframes, rows, cols))
+        if not d_flow:   # a NULL flow would make it an unmasked batch
+            raise _lib.B200OrbError(-1, "bad argument")
+        self._device_batch(d_gray, d_depth, d_Tcw, d_flow, binary_threshold, nframes, rows, cols)
 
     def dynamic_mask(self, frame: int):
         """-> (mask rows x cols uint8 0 / 1, filtered) of `frame` of the last batch, which must have been masked:
@@ -199,8 +159,7 @@ class StreamTracker:
 
     def track_batch_device(self, d_gray: int, d_depth: int, d_Tcw: int, nframes: int, rows: int, cols: int):
         """Device pointers (ints) in; results stay in HBM (device_results()). Asynchronous."""
-        _lib.check(self._L.orbs_track_batch_device(self._h, C.c_void_p(d_gray), C.c_void_p(d_depth), C.c_void_p(d_Tcw),
-                                                   nframes, rows, cols))
+        self._device_batch(d_gray, d_depth, d_Tcw, None, 0.0, nframes, rows, cols)
 
     def device_results(self):
         ps = [C.c_void_p() for _ in range(5)]

@@ -1,6 +1,6 @@
 """Deterministic crafted cases for the per-point / per-keypoint Frame members that run on the device: isInFrustum +
 PredictScale (orbm_is_in_frustum), UndistortKeyPoints (orbm_undistort_keypoints), ComputeStereoFromRGBD +
-UnprojectStereo (k_frame_glue, behind orbs_track_batch / orbs_track_batch_u16) and ComputeBoW (orbv_transform + the map
+UnprojectStereo (k_frame_glue, behind track_batch / track_batch_u16) and ComputeBoW (orbv_transform + the map
 assembly of vocabulary.py).  Each case is named after the one edge it makes observable.
 
 isInFrustum: identity or axis-permuted Tcw with integer translation, so PcX / PcY / PcZ are exact and the camera centre

@@ -36,6 +36,9 @@ def test_struct_layouts_match_header():
     assert C.sizeof(_abi.OrbmFrame) == 8 + 7 * 8 + 64 + 10 * 4 + 8 + 8     # n(+pad), 7 ptrs, Tcw, 10 floats, ptr, nlevels(+pad)
     assert C.sizeof(_abi.OrbmLast) == 8 + 6 * 8 + 64
     assert C.sizeof(_abi.OcmParams) == 5 * 8 + 4 * 4 + 8
+    # 4 ints, 3 ptrs, depth_factor(+pad), 2 ptrs, device_flow(+pad), prev_gray, binary_threshold(+pad)
+    assert C.sizeof(_abi.OrbsBatch) == 4 * 4 + 3 * 8 + 8 + 2 * 8 + 8 + 8 + 8
+    assert C.sizeof(_abi.OrbsResults) == 5 * 8 + 8                             # 5 ptrs, cap(+pad)
 
 
 def test_fails_loudly_without_gpu():

@@ -82,7 +82,7 @@ def test_flow_batch_device_across_frame_chunks(dm):
 
 
 def test_flow_batch_then_masked_device_equals_masked_with_oracle_flow(dm):
-    """dynm_flow_batch_device composed with orbs_track_batch_masked_device == the masked path fed the restatement's flow."""
+    """dynm_flow_batch_device composed with track_batch_masked_device == the masked path fed the restatement's flow."""
     import torch
     from tests.test_masked_tracking_gpu import _batch, _device_out, _same as same_out, _tracker
     F = 4
@@ -118,7 +118,7 @@ def _masked_flow_scene(F, seed=1234):
 
 
 def test_track_flow_equals_masked_with_oracle_flow():
-    """orbs_track_batch_u16_flow == orbs_track_batch_u16_masked fed the restatement's flow, 2000 features: every output and
+    """track_batch_u16_flow == track_batch_u16_masked fed the restatement's flow, 2000 features: every output and
     every frame's dynamic mask; then two batches chained by prev_gray == one batch of twice the frames."""
     from tests.test_masked_tracking_gpu import _same as same_out, _tracker
     F = 6
@@ -154,8 +154,8 @@ def test_track_flow_equals_masked_with_oracle_flow():
 
 
 def test_submit_flow_on_chained_handles_equals_track_form():
-    """orbs_submit_batch_u16_flow on two alternating handles chained with orbs_chain_after, each batch carrying the last
-    gray frame of the batch before as prev_gray == orbs_track_batch_u16_flow, batch by batch."""
+    """submit_batch_u16_flow on two alternating handles chained with orbs_chain_after, each batch carrying the last
+    gray frame of the batch before as prev_gray == track_batch_u16_flow, batch by batch."""
     import torch
     from tests.test_masked_tracking_gpu import _same as same_out, _tracker
     F, B = 3, 3

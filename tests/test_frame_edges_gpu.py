@@ -1,6 +1,6 @@
 """Device == oracle, raw bits, on the crafted Frame-member cases of tests/frame_cases.py (the oracles are pinned to the
 reference's own sources, to cv2 and to the DBoW2 stand-in by tests/test_frame_edges_cpu.py): orbm_is_in_frustum on all
-six outputs, orbm_undistort_keypoints, the frame glue of orbs_track_batch / orbs_track_batch_u16 read back with
+six outputs, orbm_undistort_keypoints, the frame glue of track_batch / track_batch_u16 read back with
 orbs_read_frame_glue, and orbv_transform raw and assembled.
 
 One exception to raw bits: a float that is NaN on both sides counts as equal.  A case that reaches NaN (PcZ == +0.0

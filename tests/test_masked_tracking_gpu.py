@@ -184,8 +184,8 @@ def test_host_and_device_paths_equal():
 
 
 def test_two_masked_batches_in_flight_equal_synchronous_calls():
-    """orbs_submit_batch_u16_masked on two alternating handles chained with orbs_chain_after == synchronous
-    orbs_track_batch_u16_masked, batch by batch."""
+    """submit_batch_u16_masked on two alternating handles chained with orbs_chain_after == synchronous
+    track_batch_u16_masked, batch by batch."""
     import torch
     F = 5
     batches = []

@@ -54,7 +54,7 @@ def test_stream_batch_matches_oracle_non_fused(oracle):
 
 
 def test_u16_depth_path_equals_float_path():
-    """orbs_track_batch_u16 (device-side convertTo(CV_32F, 1/5000)) == orbs_track_batch on the float depth the
+    """track_batch_u16 (device-side convertTo(CV_32F, 1/5000)) == track_batch on the float depth the
     reference would have computed (src/Tracking.cc:366-367)."""
     from orb_slam2_ssd_semantic_b200 import StreamTracker
     F = 4
@@ -103,7 +103,7 @@ def test_host_depth_kinds_equal_on_one_handle():
 
 
 def test_u16_pageable_depth_odd_pixel_count():
-    """Pageable CV_16U depth whose batch holds an odd number of pixels (3 x 401 x 533) == orbs_track_batch on the
+    """Pageable CV_16U depth whose batch holds an odd number of pixels (3 x 401 x 533) == track_batch on the
     matching f32 depth."""
     from orb_slam2_ssd_semantic_b200 import StreamTracker
     gray, d16, depth, factor, T = _u16_batch(79, 3, h=401, w=533)
@@ -118,7 +118,7 @@ def test_u16_pageable_depth_odd_pixel_count():
 
 @pytest.mark.gpu
 def test_two_batches_in_flight_equal_synchronous_calls():
-    """orbs_submit_batch_u16 on two alternating handles == orbs_track_batch_u16, batch by batch."""
+    """submit_batch_u16 on two alternating handles == track_batch_u16, batch by batch."""
     import torch
     from orb_slam2_ssd_semantic_b200 import StreamTracker
     ws = synth.WallStream(seed=9)

@@ -1,8 +1,8 @@
 """What the device dense flow costs on the bench's room workload (640 x 480 gray frames, 265-frame batches), one JSON line:
 
   flow_batch_ms     dynm_flow_batch_device alone (pyrDown + Farneback of 265 consecutive pairs, inputs in HBM), CUDA events
-  track_flow_ms     orbs_track_batch_u16_flow (host buffers; the flow computed on the device)
-  track_masked_ms   orbs_track_batch_u16_masked fed the same flow precomputed (uploaded with the batch)
+  track_flow_ms     track_batch_u16_flow (host buffers; orbs_submit with the flow computed on the device)
+  track_masked_ms   track_batch_u16_masked fed the same flow precomputed (orbs_submit uploads it with the batch)
   cv2_ms            cv2.calcOpticalFlowFarneback of the same 265 half-resolution pairs on this machine's CPU (its default
                     dispatch), with cv2's default thread count and with one thread; absent without cv2
 Each: median and p10 - p90 over --reps runs after a warm-up; the two tracker forms are alternated.  The card's name and
