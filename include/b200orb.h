@@ -57,8 +57,13 @@ typedef struct {            /* cv::KeyPoint, 28 bytes, what operator() appends t
 int orbx_create(const OrbxParams* p, int device, orbx_t** out);
 void orbx_destroy(orbx_t* h);
 
-/* Upper bound on keypoints one frame can return: nfeatures + 3*nlevels (SURVEY App. B.13). */
+/* Keypoints one frame can return, summed over the levels: max(N_l + 3, 4*nIni_l), where nIni_l, DistributeOctTree's
+ * number of initial nodes (src/ORBextractor.cc:545), follows from the level's aspect ratio.  orbx_max_keypoints_for gives
+ * the bound of a rows x cols image without allocating anything; it refuses what extraction refuses (rows or cols <= 0:
+ * *n = 0, OK).  orbx_max_keypoints gives that of the handle's current geometry, or, before the first extract, the bound
+ * of images with nIni <= 4 on every level -- wide images (100 x 4000: nIni = 58) need more. */
 int orbx_max_keypoints(const orbx_t* h);
+int orbx_max_keypoints_for(const orbx_t* h, int rows, int cols, int* n);
 
 /* ORBextractor::operator() (src/ORBextractor.cc:1052-1114) on one HOST image (CV_8UC1, row stride in bytes).
  * kps[cap], desc[cap*32] are host buffers; *n_out keypoints are written level-major exactly as the
@@ -99,6 +104,15 @@ int orbx_candidates_per_level(orbx_t* h, int frame, int* counts /*nlevels*/);
  * (vToDistributeKeys, src/ORBextractor.cc:788-843): cell by cell, row-major inside a cell.  xys[3*i..3*i+2] = x, y (level
  * pixels) and score.  *n = the count; cap < *n: B200ORB_ECAP and nothing written. */
 int orbx_get_candidates(orbx_t* h, int frame, int level, int32_t* xys, int cap, int* n);
+/* DistributeOctTree (src/ORBextractor.cc:540-765) alone, run by the extractor's quad-tree kernel on a caller's candidate
+ * list for level `level` of a rows x cols geometry.  xys[3*i..3*i+2] = x, y (level pixels) and score, in
+ * vToDistributeKeys order, n of them; N = the level's target, 0 <= N <= mnFeaturesPerLevel[level].  out[3*j..] = the
+ * selected keypoints in list order, *n_out = their count (cap < *n_out: B200ORB_ECAP, nothing written).  Refused with
+ * nothing launched: a level or N out of range, a coordinate outside the level's distribution region [16, maxBorderX) x
+ * [16, maxBorderY), a score outside 0..255, null pointers, and (B200ORB_ECAP) n above the level's FAST slot capacity.
+ * Synchronous.  Replaces the handle's last results: the read-backs above refuse until the next extract. */
+int orbx_distribute(orbx_t* h, int rows, int cols, int level, int N, const int32_t* xys, int n, int32_t* out, int cap,
+                    int* n_out);
 /* Number of CUDA kernels launched by this handle since creation (bench.py's gpu_launches). */
 long long orbx_launch_count(const orbx_t* h);
 /* Per-stage device time via CUDA events on the handle's stream (bench.py's roofline leg).  Stages:

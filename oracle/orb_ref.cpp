@@ -174,9 +174,11 @@ struct Extractor {
     bool operator<(const SizeSeq& o) const { return size != o.size ? size < o.size : seq < o.seq; }
   };
 
-  // DistributeOctTree :540-765.  Returns -1 if the reference would divide by zero (nIni == 0).
+  // DistributeOctTree :540-765.  Returns -1 if the reference would divide by zero (nIni == 0).  With `trace`, appends
+  // one record of TRACE_INTS ints per round (see orb_ref_distribute); the result does not depend on it.
+  static const int TRACE_INTS = 5;
   int distribute(const std::vector<KeyPoint>& in, int minX, int maxX, int minY, int maxY, int N,
-                 std::vector<KeyPoint>& out) {
+                 std::vector<KeyPoint>& out, std::vector<int>* trace = nullptr) {
     out.clear();
     const int nIni = (int)std::round(static_cast<float>(maxX - minX) / (maxY - minY));
     if (nIni <= 0) return -1;
@@ -205,6 +207,9 @@ struct Extractor {
     }
     bool finish = false;
     std::vector<SizeSeq> vss;
+    auto record = [&](int kind, int before, int count, int splits) {
+      if (trace) trace->insert(trace->end(), {kind, before, (int)nodes.size(), count, splits});
+    };
     auto push_child = [&](Node& n, std::vector<SizeSeq>& v, int* nToExpand) {
       if (n.keys.size() > 0) {
         n.seq = seq_counter++;
@@ -219,7 +224,7 @@ struct Extractor {
     while (!finish) {
       int prevSize = (int)nodes.size();
       auto lit = nodes.begin();
-      int nToExpand = 0;
+      int nToExpand = 0, splits = 0;
       vss.clear();
       while (lit != nodes.end()) {
         if (lit->noMore) { ++lit; continue; }
@@ -230,7 +235,9 @@ struct Extractor {
         push_child(n3, vss, &nToExpand);
         push_child(n4, vss, &nToExpand);
         lit = nodes.erase(lit);
+        ++splits;
       }
+      record(0, prevSize, nToExpand, splits);
       if ((int)nodes.size() >= N || (int)nodes.size() == prevSize) {
         finish = true;
       } else if (((int)nodes.size() + nToExpand * 3) > N) {
@@ -239,6 +246,7 @@ struct Extractor {
           std::vector<SizeSeq> prev = vss;
           vss.clear();
           std::sort(prev.begin(), prev.end());   // :686 (size, address) -> (size, creation seq)
+          int divided = 0;
           for (int j = (int)prev.size() - 1; j >= 0; --j) {
             Node n1, n2, n3, n4;
             divide(*prev[j].node, n1, n2, n3, n4);
@@ -247,8 +255,10 @@ struct Extractor {
             push_child(n3, vss, nullptr);
             push_child(n4, vss, nullptr);
             nodes.erase(prev[j].node->lit);
+            ++divided;
             if ((int)nodes.size() >= N) break;
           }
+          record(1, prevSize, (int)prev.size(), divided);
           if ((int)nodes.size() >= N || (int)nodes.size() == prevSize) finish = true;
         }
       }
@@ -474,14 +484,22 @@ void orb_ref_descriptor(const uint8_t* img, int step, float x, float y, float an
   KeyPoint kp{x, y, 31.f, angle, 0.f, 0, -1};
   Extractor::descriptor(kp, img, step, desc);
 }
-// DistributeOctTree alone: in/out are KeyPoint arrays; returns n_out or <0
+// DistributeOctTree alone: in/out are KeyPoint arrays; returns n_out or <0.  trace (may be null): one record of 5 ints
+// per round -- kind (0: a sweep, :608-667; 1: an iteration of the largest-first loop, :678-739), the list size before
+// and after it, nToExpand (sweep: children holding more than one keypoint) or m (largest-first: the nodes it sorts), and
+// how many nodes it split (a largest-first iteration stops splitting once the list reaches N).  *nrounds = the number
+// of rounds; the first trace_cap / 5 are written.
 int orb_ref_distribute(const void* in, int n_in, int minX, int maxX, int minY, int maxY, int N, void* out,
-                       int cap) {
+                       int cap, int* trace, int trace_cap, int* nrounds) {
   Extractor e(1000, 1.2f, 1, 20, 7);
   std::vector<KeyPoint> vi((const KeyPoint*)in, (const KeyPoint*)in + n_in), vo;
+  std::vector<int> tr;
+  if (nrounds) *nrounds = 0;
   if (n_in == 0) return 0;
-  int rc = e.distribute(vi, minX, maxX, minY, maxY, N, vo);
+  int rc = e.distribute(vi, minX, maxX, minY, maxY, N, vo, &tr);
   if (rc) return rc;
+  if (nrounds) *nrounds = (int)tr.size() / Extractor::TRACE_INTS;
+  if (trace) memcpy(trace, tr.data(), sizeof(int) * std::min((size_t)std::max(trace_cap, 0), tr.size()));
   if ((int)vo.size() > cap) return -2;
   memcpy(out, vo.data(), vo.size() * sizeof(KeyPoint));
   return (int)vo.size();

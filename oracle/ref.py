@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import subprocess
 
@@ -52,13 +53,35 @@ def lib() -> C.CDLL:
         L.orb_ref_descriptor.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p]
         L.orb_ref_distribute.restype = C.c_int
         L.orb_ref_distribute.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                         C.c_void_p, C.c_int]
+                                         C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         _lib = L
     return _lib
 
 
 def _p(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def level_region(rows: int, cols: int, inv_sf: float):
+    """Width and height of a level's distribution region, maxBorder - minBorder (src/ORBextractor.cc:781-786)."""
+    lw = int(np.rint(np.float32(cols) * np.float32(inv_sf)))
+    lh = int(np.rint(np.float32(rows) * np.float32(inv_sf)))
+    return lw - 32, lh - 32
+
+
+def n_ini(width: int, height: int) -> int:
+    """DistributeOctTree's number of initial nodes (:545): std::round of a float quotient."""
+    return int(math.floor(float(np.float32(width) / np.float32(height)) + 0.5))
+
+
+def max_keypoints(features_per_level, inv_scale_factors, rows: int, cols: int) -> int:
+    """Keypoints one rows x cols frame can return: per level max(N_l + 3, 4*nIni_l), DistributeOctTree's first sweep
+    returning four nodes per initial node and a later round stopping within 3 nodes past N_l."""
+    cap = 0
+    for N, inv in zip(features_per_level, inv_scale_factors):
+        w, h = level_region(rows, cols, inv)
+        cap += max(int(N) + 3, 4 * n_ini(w, h) if w > 0 and h > 0 else 0)
+    return cap
 
 
 class RefExtractor:
@@ -87,7 +110,7 @@ class RefExtractor:
         if image is None or image.size == 0:
             return np.zeros(0, KP_DTYPE), np.zeros((0, 32), np.uint8)
         assert image.dtype == np.uint8 and image.ndim == 2
-        cap = self.nfeatures + 3 * self.nlevels + 64
+        cap = max_keypoints(self.mnFeaturesPerLevel, self.mvInvScaleFactor, *image.shape)
         kps = np.zeros(cap, KP_DTYPE)
         desc = np.zeros((cap, 32), np.uint8)
         n = self.L.orb_ref_extract(self.h, _p(image), image.shape[0], image.shape[1], image.strides[0], _p(kps),
@@ -148,13 +171,25 @@ def descriptor(img: np.ndarray, x: float, y: float, angle: float) -> np.ndarray:
     return d
 
 
-def distribute(kps: np.ndarray, minX, maxX, minY, maxY, N) -> np.ndarray:
+TRACE_DTYPE = np.dtype([("kind", "<i4"), ("before", "<i4"), ("after", "<i4"), ("count", "<i4"), ("splits", "<i4")])
+SWEEP, LARGEST_FIRST = 0, 1
+
+
+def distribute(kps: np.ndarray, minX, maxX, minY, maxY, N, trace: bool = False):
+    """DistributeOctTree.  trace=True also returns its rounds (TRACE_DTYPE: kind SWEEP or LARGEST_FIRST, the list size
+    before and after, nToExpand of a sweep or the m nodes a largest-first iteration sorts, and the nodes it split)."""
     kps = np.ascontiguousarray(kps)
     out = np.zeros(max(len(kps), 1), KP_DTYPE)
-    n = lib().orb_ref_distribute(_p(kps), len(kps), minX, maxX, minY, maxY, N, _p(out), len(out))
+    nr = C.c_int(0)
+    n = lib().orb_ref_distribute(_p(kps), len(kps), minX, maxX, minY, maxY, N, _p(out), len(out), None, 0, C.byref(nr))
     if n < 0:
         raise RuntimeError("distribute failed %d" % n)
-    return out[:n]
+    if not trace:
+        return out[:n]
+    tr = np.zeros(max(nr.value, 1), TRACE_DTYPE)
+    lib().orb_ref_distribute(_p(kps), len(kps), minX, maxX, minY, maxY, N, _p(out), len(out), _p(tr), 5 * nr.value,
+                             C.byref(nr))
+    return out[:n], tr[:nr.value]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -453,7 +488,6 @@ class SrcExtractor:
         self.L = reflib()
         self.nlevels = nlevels
         self.h = self.L.refsrc_orb_create(nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST)
-        self.cap = nfeatures + 16 * nlevels + 64
         t = [np.zeros(nlevels, np.float32) for _ in range(4)] + [np.zeros(nlevels, np.int32), np.zeros(16, np.int32)]
         self.L.refsrc_orb_tables(self.h, *[_p(a) for a in t])
         (self.mvScaleFactor, self.mvInvScaleFactor, self.mvLevelSigma2, self.mvInvLevelSigma2,
@@ -469,11 +503,12 @@ class SrcExtractor:
         assert image.dtype == np.uint8 and image.ndim == 2
         if image.strides[1] != 1:
             image = np.ascontiguousarray(image)
-        kps = np.zeros(self.cap, KP_DTYPE)
-        desc = np.zeros((self.cap, 32), np.uint8)
+        cap = max_keypoints(self.mnFeaturesPerLevel, self.mvInvScaleFactor, *image.shape)
+        kps = np.zeros(cap, KP_DTYPE)
+        desc = np.zeros((cap, 32), np.uint8)
         n = C.c_int(0)
         rc = self.L.refsrc_orb_extract(self.h, image.ctypes.data, image.shape[0], image.shape[1], image.strides[0],
-                                       _p(kps), _p(desc), self.cap, C.byref(n))
+                                       _p(kps), _p(desc), cap, C.byref(n))
         assert rc == 0
         return kps[:n.value].copy(), desc[:n.value].copy()
 

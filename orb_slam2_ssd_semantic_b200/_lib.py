@@ -26,6 +26,7 @@ EXPORTS = [
     "orbx_create", "orbx_destroy", "orbx_max_keypoints", "orbx_extract", "orbx_extract_batch",
     "orbx_extract_batch_device", "orbx_device_results", "orbx_sync", "orbx_stream", "orbx_level_dims",
     "orbx_get_level", "orbx_scale_tables", "orbx_candidates_per_level", "orbx_get_candidates", "orbx_launch_count",
+    "orbx_max_keypoints_for", "orbx_distribute",
     "orbx_profile_enable", "orbx_profile_read",
     "orbm_hamming", "orbm_create", "orbm_destroy", "orbm_launch_count", "orbm_search_by_projection_last",
     "orbm_search_by_projection_last_pairs",
@@ -82,6 +83,8 @@ def lib() -> C.CDLL:
     L.orbx_scale_tables.argtypes = [vp, vp, vp, vp, vp, vp]
     L.orbx_candidates_per_level.argtypes = [vp, i, vp]
     L.orbx_get_candidates.argtypes = [vp, i, i, vp, i, C.POINTER(i)]
+    L.orbx_max_keypoints_for.argtypes = [vp, i, i, C.POINTER(i)]
+    L.orbx_distribute.argtypes = [vp, i, i, i, i, vp, i, vp, i, C.POINTER(i)]
     L.orbx_launch_count.argtypes = [vp]
     L.orbx_launch_count.restype = C.c_longlong
     L.orbx_profile_enable.argtypes = [vp, i]

@@ -2,8 +2,11 @@
 // include/ORBextractor.h).  Kernels live in orbx_kernels.cuh.
 #include <cmath>
 #include <cstdlib>
+#include <map>
 #include <memory>
+#include <mutex>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "orbx_kernels.cuh"
@@ -25,6 +28,22 @@ static const signed char kPatternHost[1024] = {
 
 static inline int cv_round_f(float v) { return (int)lrintf(v); }
 static inline int cv_round_d(double v) { return (int)lrint(v); }
+
+// A kernel's dynamic shared-memory limit belongs to the kernel on the current device, not to a handle: raise it to the
+// largest size any handle has needed and never lower it, so that handles of different geometries or quotas, on any
+// thread, can launch after one another.
+static int raise_smem_limit(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limit;
+  int dev = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  size_t& cur = limit[{kernel, dev}];
+  if (bytes <= cur) return B200ORB_OK;
+  B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  cur = bytes;
+  return B200ORB_OK;
+}
 
 }  // namespace b200
 
@@ -85,16 +104,16 @@ int orbx::init(const OrbxParams& p, int dev) {
   return B200ORB_OK;
 }
 
-// (re)build every geometry-dependent table and buffer for F frames of rows x cols
-int orbx::ensure_geometry(int r, int c, int F) {
-  if (r == rows && c == cols && F <= maxF) return B200ORB_OK;
+// Level sizes, FAST cells and the quad-tree's per-level constants of a rows x cols image, with every refusal of
+// extraction; host arithmetic only.  The selection capacity of level l is max(N_l + 3, 4*nIni_l): DistributeOctTree's
+// first sweep may return four nodes per initial node (nIni grows with the aspect ratio: 58 at 4000 x 100), and a later
+// round stops as soon as the list reaches N_l, at most 3 nodes past it.
+int orbx::plan_geometry(int r, int c, GeomPlan& g) const {
   if (r > 4095 || c > 4095) { set_error("image %dx%d exceeds the 4095-px packing limit", c, r); return B200ORB_EINVAL; }
-  const int keepF = (r == rows && c == cols) ? std::max(F, maxF) : F;
-  rows = cols = maxF = 0;   // no geometry until its block exists
-  have_results = false;
   const int nl = prm.nlevels;
+  int* lw = g.lw;
+  int* lh = g.lh;
   // level sizes (:1121-1122)
-  size_t off = 0;
   for (int l = 0; l < nl; ++l) {
     lw[l] = cv_round_f((float)c * invsf[l]);
     lh[l] = cv_round_f((float)r * invsf[l]);
@@ -102,51 +121,11 @@ int orbx::ensure_geometry(int r, int c, int F) {
       set_error("level %d is %dx%d: too small for the 16-px FAST border (reference would crash)", l, lw[l], lh[l]);
       return B200ORB_EGEOM;
     }
-    lpitch[l] = align_up(lw[l], 16);
-    loff[l] = off;
-    off += (size_t)lpitch[l] * lh[l];
-  }
-  frame_bytes = align_up_sz(off, 256);
-  // resize tables (SURVEY App. A.2)
-  std::vector<int2> xt, yt;
-  std::vector<int4> xg;
-  resize_group_ok = true;
-  for (int l = 1; l < nl; ++l) {
-    xt_off[l] = (int)xt.size();
-    yt_off[l] = (int)yt.size();
-    auto fill = [](int dn, int sn, std::vector<int2>& t) {
-      const double scale = 1.0 / ((double)dn / sn);
-      for (int d = 0; d < dn; ++d) {
-        float f = (float)((d + 0.5) * scale - 0.5);
-        int i = (int)std::floor(f);
-        f -= (float)i;
-        if (i < 0) { i = 0; f = 0.f; }
-        if (i >= sn - 1) { i = sn - 1; f = 0.f; }
-        const int a0 = (short)cv_round_f((1.f - f) * 2048.f), a1 = (short)cv_round_f(f * 2048.f);
-        t.push_back(make_int2(i, (a0 & 0xffff) | (a1 << 16)));
-      }
-    };
-    fill(lw[l], lw[l - 1], xt);
-    fill(lh[l], lh[l - 1], yt);
-    // group table of k_resize_g
-    xg_off[l] = (int)xg.size();
-    for (int dx0 = 0; dx0 < lw[l]; dx0 += 4) {
-      const int2* t = xt.data() + xt_off[l];
-      int sx[4], cf[4];
-      for (int i = 0; i < 4; ++i) { const int2 e = t[std::min(dx0 + i, lw[l] - 1)]; sx[i] = e.x; cf[i] = e.y; }
-      for (int i = 1; i < 4; ++i) if (sx[i] < sx[0]) sx[i] = sx[0];   // (replicated tail entries never precede sx[0])
-      int sels = 0;
-      for (int i = 0; i < 4; ++i) {
-        const int dlt = sx[i] - sx[0];
-        if (dlt + 1 > 7) resize_group_ok = false;   // scale > 2: the byte-window path does not apply
-        sels |= (((dlt & 7) | (((dlt + 1) & 7) << 4)) & 0xff) << (8 * i);
-      }
-      xg.push_back(make_int4(sx[0] >> 2, 8 * (sx[0] & 3), sels, 0));
-      xg.push_back(make_int4(cf[0], cf[1], cf[2], cf[3]));
-    }
   }
   // FAST cells (:775-815) and quad-tree constants (:545-547)
-  std::vector<CellDesc> cells;
+  std::vector<CellDesc>& cells = g.cells;
+  cells.clear();
+  LevelTab& ltab = g.ltab;
   int slots = 0, selcap = 0, qcap = 8;
   memset(&ltab, 0, sizeof(ltab));
   ltab.nlevels = nl;
@@ -208,6 +187,70 @@ int orbx::ensure_geometry(int r, int c, int F) {
   ltab.cell_begin[nl] = (int)cells.size();
   ltab.slot_begin[nl] = slots;
   ltab.sel_off[nl] = selcap;
+  g.slots = slots;
+  g.qt_cap = align_up(qcap, 8);
+  if (qt_smem_bytes(g.qt_cap) > 100 * 1024) { set_error("nfeatures too large for the quad-tree kernel's shared memory"); return B200ORB_EINVAL; }
+  return B200ORB_OK;
+}
+
+// (re)build every geometry-dependent table and buffer for F frames of rows x cols
+int orbx::ensure_geometry(int r, int c, int F) {
+  if (r == rows && c == cols && F <= maxF) return B200ORB_OK;
+  GeomPlan g;
+  B200_CHECK(plan_geometry(r, c, g));
+  const int keepF = (r == rows && c == cols) ? std::max(F, maxF) : F;
+  rows = cols = maxF = 0;   // no geometry until its block exists
+  have_results = false;
+  const int nl = prm.nlevels;
+  size_t off = 0;
+  for (int l = 0; l < nl; ++l) {
+    lw[l] = g.lw[l];
+    lh[l] = g.lh[l];
+    lpitch[l] = align_up(lw[l], 16);
+    loff[l] = off;
+    off += (size_t)lpitch[l] * lh[l];
+  }
+  frame_bytes = align_up_sz(off, 256);
+  // resize tables (SURVEY App. A.2)
+  std::vector<int2> xt, yt;
+  std::vector<int4> xg;
+  resize_group_ok = true;
+  for (int l = 1; l < nl; ++l) {
+    xt_off[l] = (int)xt.size();
+    yt_off[l] = (int)yt.size();
+    auto fill = [](int dn, int sn, std::vector<int2>& t) {
+      const double scale = 1.0 / ((double)dn / sn);
+      for (int d = 0; d < dn; ++d) {
+        float f = (float)((d + 0.5) * scale - 0.5);
+        int i = (int)std::floor(f);
+        f -= (float)i;
+        if (i < 0) { i = 0; f = 0.f; }
+        if (i >= sn - 1) { i = sn - 1; f = 0.f; }
+        const int a0 = (short)cv_round_f((1.f - f) * 2048.f), a1 = (short)cv_round_f(f * 2048.f);
+        t.push_back(make_int2(i, (a0 & 0xffff) | (a1 << 16)));
+      }
+    };
+    fill(lw[l], lw[l - 1], xt);
+    fill(lh[l], lh[l - 1], yt);
+    // group table of k_resize_g
+    xg_off[l] = (int)xg.size();
+    for (int dx0 = 0; dx0 < lw[l]; dx0 += 4) {
+      const int2* t = xt.data() + xt_off[l];
+      int sx[4], cf[4];
+      for (int i = 0; i < 4; ++i) { const int2 e = t[std::min(dx0 + i, lw[l] - 1)]; sx[i] = e.x; cf[i] = e.y; }
+      for (int i = 1; i < 4; ++i) if (sx[i] < sx[0]) sx[i] = sx[0];   // (replicated tail entries never precede sx[0])
+      int sels = 0;
+      for (int i = 0; i < 4; ++i) {
+        const int dlt = sx[i] - sx[0];
+        if (dlt + 1 > 7) resize_group_ok = false;   // scale > 2: the byte-window path does not apply
+        sels |= (((dlt & 7) | (((dlt + 1) & 7) << 4)) & 0xff) << (8 * i);
+      }
+      xg.push_back(make_int4(sx[0] >> 2, 8 * (sx[0] & 3), sels, 0));
+      xg.push_back(make_int4(cf[0], cf[1], cf[2], cf[3]));
+    }
+  }
+  const std::vector<CellDesc>& cells = g.cells;
+  ltab = g.ltab;
   ncells = (int)cells.size();
   {
     int rwm = 0, rhm = 0, det = 0;
@@ -220,17 +263,16 @@ int orbx::ensure_geometry(int r, int c, int F) {
     fast_rows_max = rhm;
     fast_smem = (size_t)FAST_WARPS * (2 * rhm * fast_tp + 2 * FAST_QLEN + 2 * fast_clist_cap);
     if (fast_smem > 48 * 1024) {
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
-      B200_CUDA(cudaFuncSetAttribute(k_fast_cells<FAST_TP_SMALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem));
+      B200_CHECK(raise_smem_limit((const void*)k_fast_cells<FAST_TP_BIG>, fast_smem));
+      B200_CHECK(raise_smem_limit((const void*)k_fast_cells<FAST_TP_SMALL>, fast_smem));
     }
   }
-  slots_per_frame = align_up(slots, 4);
-  sel_per_frame = selcap;
-  cap = selcap;
-  qt_cap = align_up(qcap, 8);
+  slots_per_frame = align_up(g.slots, 4);
+  sel_per_frame = ltab.sel_off[nl];
+  cap = sel_per_frame;
+  qt_cap = g.qt_cap;
   qt_smem = qt_smem_bytes(qt_cap);
-  if (qt_smem > 100 * 1024) { set_error("nfeatures too large for the quad-tree kernel's shared memory"); return B200ORB_EINVAL; }
-  B200_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qt_smem));
+  B200_CHECK(raise_smem_limit((const void*)k_quadtree, qt_smem));
 
   std::vector<BlurTile> bt;
   for (int l = 0; l < nl; ++l)
@@ -402,11 +444,21 @@ void orbx_destroy(orbx_t* h) { destroy_handle(h); }
 
 int orbx_max_keypoints(const orbx_t* h) {
   if (!h) return 0;
-  // capacity independent of the geometry: sum over levels of max(N_l + 3, 4*nIni); nIni <= 4 for any image the
-  // reference accepts in practice, so 16 is the floor per level
+  // before the first extract: sum over levels of max(N_l + 3, 16), the bound of images with nIni <= 4 on every level;
+  // wider images need orbx_max_keypoints_for.  After it: the capacity of the current geometry.
   int s = 0;
   for (int l = 0; l < h->prm.nlevels; ++l) s += std::max(h->nfeat[l] + 3, 16);
   return std::max(s, h->cap);
+}
+
+int orbx_max_keypoints_for(const orbx_t* h, int rows, int cols, int* n) {
+  if (!h || !n) { set_error("null argument"); return B200ORB_EINVAL; }
+  *n = 0;
+  if (rows <= 0 || cols <= 0) return B200ORB_OK;   // an empty image returns no keypoints (:1055)
+  GeomPlan g;
+  B200_CHECK(h->plan_geometry(rows, cols, g));
+  *n = g.ltab.sel_off[h->prm.nlevels];
+  return B200ORB_OK;
 }
 
 static int extract_common(orbx* h, const uint8_t* gray, bool on_device, int nframes, int rows, int cols,
@@ -582,6 +634,73 @@ int orbx_get_candidates(orbx_t* h, int frame, int level, int32_t* xys, int cap, 
       xys[3 * k + 1] = (int32_t)((v >> 12) & 0xfff);
       xys[3 * k + 2] = (int32_t)(v >> 24);
     }
+  return B200ORB_OK;
+}
+
+int orbx_distribute(orbx_t* h, int rows, int cols, int level, int N, const int32_t* xys, int n, int32_t* out, int cap,
+                    int* n_out) {
+  if (!h || !n_out || !out || (n > 0 && !xys)) { set_error("null argument"); return B200ORB_EINVAL; }
+  if (rows <= 0 || cols <= 0 || level < 0 || level >= h->prm.nlevels || n < 0) {
+    set_error("bad geometry, level or count");
+    return B200ORB_EINVAL;
+  }
+  if (N < 0 || N > h->nfeat[level]) { set_error("N = %d outside 0..%d", N, h->nfeat[level]); return B200ORB_EINVAL; }
+  DeviceGuard g(h->device);
+  B200_CHECK(h->ensure_geometry(rows, cols, 1));
+  // the distribution region of the level (:783-786): x in [16, maxBorderX), y in [16, maxBorderY)
+  const int maxBX = h->lw[level] - EDGE_THRESHOLD + 3, maxBY = h->lh[level] - EDGE_THRESHOLD + 3;
+  for (int i = 0; i < n; ++i) {
+    const int x = xys[3 * i], y = xys[3 * i + 1], r = xys[3 * i + 2];
+    if (x < FAST_BORDER || x >= maxBX || y < FAST_BORDER || y >= maxBY || r < 0 || r > 255) {
+      set_error("candidate %d (%d, %d, %d) outside [%d, %d) x [%d, %d) x [0, 255]", i, x, y, r, FAST_BORDER, maxBX,
+                FAST_BORDER, maxBY);
+      return B200ORB_EINVAL;
+    }
+  }
+  const LevelTab& lt = h->ltab;
+  const int c0 = lt.cell_begin[level], nc = lt.cell_begin[level + 1] - c0;
+  const int s0 = lt.slot_begin[level], ns = lt.slot_begin[level + 1] - s0;
+  if (n > ns) { set_error("%d candidates > the %d slots of level %d", n, ns, level); return B200ORB_ECAP; }
+  // the list in order through the level's cell segments, each filled up to its slot count: k_quadtree's gather
+  // concatenates exactly the caller's list
+  std::vector<CellDesc> cells(nc);
+  B200_CUDA(cudaMemcpyAsync(cells.data(), h->d_cells + c0, sizeof(CellDesc) * nc, cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  std::vector<unsigned> slots(std::max(ns, 1));
+  std::vector<int> cnt(h->ncells, 0);
+  for (int i = 0; i < n; ++i) slots[i] = (unsigned)xys[3 * i] | ((unsigned)xys[3 * i + 1] << 12) | ((unsigned)xys[3 * i + 2] << 24);
+  for (int c = 0, k = 0; c < nc && k < n; ++c) {
+    const int end = (c + 1 < nc) ? cells[c + 1].slot_off - s0 : ns;
+    cnt[c0 + c] = std::min(n, end) - k;
+    k += cnt[c0 + c];
+  }
+  h->have_results = false;   // the candidates, selections and counts of frame 0 are overwritten
+  if (n > 0)
+    B200_CUDA(cudaMemcpyAsync(h->d_cand + s0, slots.data(), sizeof(unsigned) * n, cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(h->d_cellcnt, cnt.data(), sizeof(int) * h->ncells, cudaMemcpyHostToDevice, h->stream));
+  LevelTab ltab = lt;
+  ltab.nfeat[level] = N;
+  k_quadtree<<<dim3(h->prm.nlevels, 1), QT_THREADS, h->qt_smem, h->stream>>>(
+      ltab, h->d_cells, h->d_cand, h->d_cellcnt, h->ncells, h->slots_per_frame, QtScratchView{h->d_qkp, h->d_qnode},
+      h->qt_cap, h->d_sel, h->d_selcnt, h->d_candcnt, h->sel_per_frame);
+  ++h->launches;
+  B200_CUDA(cudaGetLastError());
+  int m = 0;
+  B200_CUDA(cudaMemcpyAsync(&m, h->d_selcnt + level, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  B200_CUDA(cudaStreamSynchronize(h->stream));
+  *n_out = m;
+  if (cap < m) { set_error("%d keypoints selected > cap %d", m, cap); return B200ORB_ECAP; }
+  std::vector<unsigned> sel(std::max(m, 1));
+  if (m > 0) {
+    B200_CUDA(cudaMemcpyAsync(sel.data(), h->d_sel + lt.sel_off[level], sizeof(unsigned) * m, cudaMemcpyDeviceToHost,
+                              h->stream));
+    B200_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  for (int j = 0; j < m; ++j) {
+    out[3 * j] = (int32_t)(sel[j] & 0xfff);
+    out[3 * j + 1] = (int32_t)((sel[j] >> 12) & 0xfff);
+    out[3 * j + 2] = (int32_t)(sel[j] >> 24);
+  }
   return B200ORB_OK;
 }
 

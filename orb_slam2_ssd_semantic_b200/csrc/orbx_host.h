@@ -46,6 +46,13 @@ struct OrientTab {
   int umax[HALF_PATCH_SIZE + 1];
 };
 
+struct GeomPlan {                // what orbx::plan_geometry derives from rows x cols
+  int lw[MAX_LEVELS], lh[MAX_LEVELS];
+  std::vector<CellDesc> cells;
+  LevelTab ltab;                 // ltab.sel_off[nlevels]: keypoints one frame can return
+  int slots = 0, qt_cap = 0;     // FAST candidate slots per frame; quad-tree list capacity
+};
+
 struct BlurTile { short level, x0, y0, pad; };   // one warp-tile of k_blur7_strip: 128 columns x BLS_ROWS rows of one level
 struct BlurEdge { short level, x0, y0, pad; };   // one border column group of k_blur7_edges
 
@@ -109,6 +116,7 @@ struct orbx {
   std::vector<b200::StageEvents> prof_runs;
 
   int init(const OrbxParams& p, int dev);
+  int plan_geometry(int r, int c, b200::GeomPlan& g) const;
   int ensure_geometry(int r, int c, int F);
   int run(const uint8_t* d_l0, int pitch0, size_t fstride0, int F, int f0 = 0);
   int prof_mark(int boundary);   // record event `boundary` of the current run (no-op unless profiling)

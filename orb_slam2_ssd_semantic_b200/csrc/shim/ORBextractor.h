@@ -63,10 +63,11 @@ class ORBextractor {
     if (_image.empty()) return;                       // :1055
     cv::Mat image = _image.getMat();
     if (image.type() != CV_8UC1) throw std::invalid_argument("ORBextractor: image must be CV_8UC1");   // assert :1059
-    const int cap = orbx_max_keypoints(h_) + 64;
+    int cap = 0, n = 0;
+    if (orbx_max_keypoints_for(h_, image.rows, image.cols, &cap) != B200ORB_OK)
+      throw std::runtime_error(std::string("ORBextractor(B200): ") + b200orb_last_error());
     kps_.resize(cap);
     desc_.resize((size_t)cap * 32);
-    int n = 0;
     if (orbx_extract(h_, image.data, image.rows, image.cols, image.step, kps_.data(), desc_.data(), cap, &n) != B200ORB_OK)
       throw std::runtime_error(std::string("ORBextractor(B200): ") + b200orb_last_error());
     if (n == 0) {

@@ -2,7 +2,9 @@
 // tests use the stand-in of oracle/standin/) and exercises them when a GPU is present.  The matcher shim needs the
 // reference's Frame / KeyFrame / MapPoint classes and is tested through oracle/_ref/libshimsrc.so instead.
 #include <cstdio>
+#include <cstdlib>
 #include <map>
+#include <string>
 
 #include "ORBextractor.h"
 #include "pointcloudmapping.h"
@@ -13,7 +15,34 @@ struct MockKeyFrame {   // what PointCloudMapping reads from a KeyFrame (P varia
   cv::Mat GetPose() { return pose.clone(); }
 };
 
+// `shim_check extract nfeatures nlevels rows cols image.u8 out.bin`: one frame through a FRESH ORBextractor(nfeatures, 1.2,
+// nlevels, 20, 7); writes the keypoint count, the keypoints as OrbxKeyPoint records and the descriptor rows.
+static int extract_to_file(char** a) {
+  const int nf = std::atoi(a[0]), nl = std::atoi(a[1]), rows = std::atoi(a[2]), cols = std::atoi(a[3]);
+  cv::Mat img(rows, cols, CV_8UC1);
+  FILE* f = std::fopen(a[4], "rb");
+  if (!f || std::fread(img.data, 1, (size_t)rows * cols, f) != (size_t)rows * cols) return 5;
+  std::fclose(f);
+  ORB_SLAM2::ORBextractor ex(nf, 1.2f, nl, 20, 7);
+  std::vector<cv::KeyPoint> kps;
+  cv::Mat desc, mask;
+  ex(img, mask, kps, desc);
+  FILE* o = std::fopen(a[5], "wb");
+  if (!o) return 5;
+  const int n = (int)kps.size();
+  std::fwrite(&n, sizeof(int), 1, o);
+  for (const cv::KeyPoint& k : kps) {
+    OrbxKeyPoint r{k.pt.x, k.pt.y, k.size, k.angle, k.response, k.octave, k.class_id};
+    std::fwrite(&r, sizeof(r), 1, o);
+  }
+  for (int i = 0; i < n; ++i) std::fwrite(desc.ptr(i), 1, 32, o);
+  std::fclose(o);
+  std::printf("keypoints %d\n", n);
+  return 0;
+}
+
 int main(int argc, char** argv) {
+  if (argc == 8 && std::string(argv[1]) == "extract") return extract_to_file(argv + 2);
   if (b200orb_device_count() == 0) {
     try {
       ORB_SLAM2::ORBextractor e(1000, 1.2f, 8, 20, 7);

@@ -71,8 +71,14 @@ class ORBextractor:
     def handle(self):
         return self._h
 
-    def max_keypoints(self) -> int:
-        return int(self._L.orbx_max_keypoints(self._h))
+    def max_keypoints(self, rows: int | None = None, cols: int | None = None) -> int:
+        """Keypoints one frame can return: for a rows x cols image (refused like extraction refuses it), or without a
+        geometry orbx_max_keypoints' value for the handle's current one."""
+        if rows is None:
+            return int(self._L.orbx_max_keypoints(self._h))
+        n = C.c_int(0)
+        _lib.check(self._L.orbx_max_keypoints_for(self._h, int(rows), int(cols), C.byref(n)))
+        return n.value
 
     # -- operator() ---------------------------------------------------------------------------------------
     def __call__(self, image: np.ndarray, mask=None):
@@ -83,7 +89,7 @@ class ORBextractor:
             raise ValueError("image must be CV_8UC1 (reference asserts, src/ORBextractor.cc:1059)")
         if image.strides[1] != 1:
             image = np.ascontiguousarray(image)
-        cap = self.max_keypoints() + 64
+        cap = self.max_keypoints(*image.shape)
         kps = np.zeros(cap, KP_DTYPE)
         desc = np.zeros((cap, 32), np.uint8)
         n = C.c_int(0)
@@ -98,7 +104,7 @@ class ORBextractor:
             raise ValueError("images must be [F, rows, cols] uint8")
         images = np.ascontiguousarray(images)
         F, rows, cols = images.shape
-        cap = self.max_keypoints() + 64
+        cap = self.max_keypoints(rows, cols)
         kps = np.zeros((F, cap), KP_DTYPE)
         desc = np.zeros((F, cap, 32), np.uint8)
         n = np.zeros(F, np.int32)
@@ -139,6 +145,19 @@ class ORBextractor:
         out = np.zeros((max(n.value, 1), 3), np.int32)
         _lib.check(self._L.orbx_get_candidates(self._h, frame, level, _p(out), n.value, C.byref(n)))
         return out[:n.value]
+
+    def distribute(self, rows: int, cols: int, level: int, N: int, xys: np.ndarray) -> np.ndarray:
+        """DistributeOctTree alone on the device: the extractor's quad-tree kernel on the candidate list xys ([n, 3] int32
+        x, y, score in level pixels, vToDistributeKeys order) of level `level` of a rows x cols image, with target N.
+        Returns the selected keypoints, [m, 3] int32 in list order.  The pyramid and candidate read-backs refuse until
+        the next extract."""
+        xys = np.ascontiguousarray(xys, np.int32).reshape(-1, 3)
+        n = len(xys)
+        out = np.zeros((max(n, 1), 3), np.int32)   # every selected node holds at least one of the n candidates
+        m = C.c_int(0)
+        _lib.check(self._L.orbx_distribute(self._h, int(rows), int(cols), int(level), int(N), _p(xys), n, _p(out), len(out),
+                                           C.byref(m)))
+        return out[:m.value].copy()
 
     def launch_count(self) -> int:
         return int(self._L.orbx_launch_count(self._h))
