@@ -451,6 +451,17 @@ int dynm_warp_perspective(dynm_t* h, const uint8_t* gray, int rows, int cols, co
  * must not overlap d_gray).  At most 65535 frames per call.  Asynchronous on the handle's stream. */
 int dynm_warp_perspective_batch_device(dynm_t* h, const uint8_t* d_gray, int nframes, int rows, int cols, const double* d_H,
                                        uint8_t* d_dst);
+/* The homography TrackHomo feeds that warp (perfect/src/Tracking.cc:1386): cv::findHomography(points_current,
+ * points_last, RANSAC, 3) with maxIters 2000 and confidence 0.995 -- RANSAC, runKernel on the inliers, the
+ * Levenberg-Marquardt refinement (at most 10 iterations over 9 parameters), H scaled by 1 / H22 and the mask of the
+ * refined H (float reprojection error <= 9) -- in the order of operations of OpenCV 4.13's baseline dispatch
+ * (cv::setUseOptimized(false)), as tests/homography_lm.py restates it: equal to that restatement bit for bit, and to
+ * cv2 bit for bit below 50 inliers (from 100 residual rows a cv2 built with LAPACK sums J^T r in its BLAS's order).  src = points_current, dst = points_last:
+ * float[n][2] host buffers; synchronous.  Exactly 4 pairs: runKernel of all four, unrefined, mask all ones.  No model
+ * (every subset degenerate, or getSubset rejecting 10000 draws in a row before the first hypothesis): *found = 0, H
+ * zeros and mask all zeros, as cv2 returns an empty H and a zero mask.  Otherwise *found = 1 and H is row-major double[9].
+ * n outside [4, 8192] or a NULL pointer returns B200ORB_EINVAL before anything is enqueued. */
+int dynm_find_homography(dynm_t* h, const float* src, const float* dst, int n, double H[9], uint8_t* mask, int* found);
 
 /* ------------------------------------------------------------------------------------------------
  * Stream pipeline (batched many-frame mode of north_star): per frame t of a batch, what

@@ -46,6 +46,7 @@ EXPORTS = [
     "dynm_create", "dynm_destroy", "dynm_launch_count", "dynm_stream", "dynm_sync", "dynm_element", "dynm_mask_from_flow",
     "dynm_mask_from_flow_batch_device", "dynm_filter_keypoints", "dynm_filter_keypoints_batch_device",
     "dynm_farneback", "dynm_flow_batch_device", "dynm_warp_perspective", "dynm_warp_perspective_batch_device",
+    "dynm_find_homography",
 ]
 
 
@@ -144,6 +145,7 @@ def lib() -> C.CDLL:
     L.dynm_flow_batch_device.argtypes = [vp, vp, vp, i, i, i, vp]
     L.dynm_warp_perspective.argtypes = [vp, vp, i, i, vp, vp]
     L.dynm_warp_perspective_batch_device.argtypes = [vp, vp, i, i, i, vp, vp]
+    L.dynm_find_homography.argtypes = [vp, vp, vp, i, vp, vp, vp]
     L.orbs_create.argtypes = [C.POINTER(OrbsParams), i, C.POINTER(vp)]
     L.orbs_destroy.argtypes = [vp]
     L.orbs_destroy.restype = None

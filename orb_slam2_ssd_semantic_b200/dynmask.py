@@ -109,6 +109,21 @@ class DynamicMask:
         _lib.check(self._L.dynm_warp_perspective_batch_device(self._h, C.c_void_p(d_gray), int(nframes), int(rows),
                                                               int(cols), C.c_void_p(d_H), C.c_void_p(d_dst)))
 
+    def find_homography(self, points_current, points_last):
+        """cv::findHomography(points_current, points_last, RANSAC, 3) on the GPU (perfect/src/Tracking.cc:1386), the
+        LM refinement included, in OpenCV 4.13's baseline order of operations -> (H 3x3 float64 or None when no model
+        is found, mask uint8[n]).  4 <= n <= 8192 pairs, float32 [n][2] each."""
+        src = np.ascontiguousarray(points_current, np.float32).reshape(-1, 2)
+        dst = np.ascontiguousarray(points_last, np.float32).reshape(-1, 2)
+        if len(src) != len(dst):
+            raise ValueError("points_current and points_last must have the same length")
+        n = len(src)
+        H = np.zeros(9, np.float64)
+        mask = np.zeros(max(n, 1), np.uint8)
+        found = C.c_int(0)
+        _lib.check(self._L.dynm_find_homography(self._h, _p(src), _p(dst), n, _p(H), _p(mask), C.byref(found)))
+        return (H.reshape(3, 3) if found.value else None), mask[:n]
+
     def stream(self) -> int:
         return int(self._L.dynm_stream(self._h) or 0)
 
