@@ -481,12 +481,14 @@ typedef struct {
 } OrbsParams;
 int orbs_create(const OrbsParams* p, int device, orbs_t** out);
 void orbs_destroy(orbs_t* h);
-/* One batch of orbs_submit: gray[n][rows][cols] u8, Tcw[n][16] f32 row-major, one depth image per frame.  Exactly seven
+/* One batch of orbs_submit: gray[n][rows][cols] u8, Tcw[n][16] f32 row-major, one depth image per frame.  Exactly eight
  * forms are accepted:
- *   host batches (device = 0):    f32 depth | CV_16U depth | CV_16U depth + flow | CV_16U depth + device_flow
+ *   host batches (device = 0):    f32 depth | CV_16U depth | CV_16U depth + flow | CV_16U depth + device_flow |
+ *                                 CV_16U depth + device_flow + homography (prev_gray NULL)
  *   device batches (device = 1):  f32 depth | f32 depth + flow
  * Every other combination -- and a NULL input, a non-positive size, both depths or neither, prev_gray without
- * device_flow -- returns B200ORB_EINVAL before anything is enqueued and before any handle state changes. */
+ * device_flow, homography other than 0 or 1 -- returns B200ORB_EINVAL before anything is enqueued and before any handle
+ * state changes. */
 typedef struct {
   int nframes, rows, cols;
   int device;                   /* 1: every input below is an HBM pointer and the results stay in HBM
@@ -531,6 +533,22 @@ typedef struct {
    * carry one sequence: each batch passes the last gray frame of the batch before. */
   const uint8_t* prev_gray;
   float binary_threshold;       /* masked batches: Flow::ComputeMask's threshold (raised to 40) */
+  /* 1: the masked batch follows the reference's live path in full (perfect/src/Tracking.cc:703-719): before each frame's
+   * ComputeMask, TrackHomo (:1331-1399) searches the UNFILTERED keypoints of frame t against the FILTERED keypoints of
+   * frame t-1 (SearchByProjection(cur, last, th, mono = 0, points_last, points_current) of ORBmatcher(0.9, true), whatever
+   * OrbsParams' nnratio and check_ori), retries at 2 th
+   * below 20 matches, and with at least 20 matches and more than 50 pairs fits H = findHomography(points_current,
+   * points_last, RANSAC, 3) as dynm_find_homography does; a found H makes the frame's mask ComputeMask(GrayImg, H)
+   * (perfect/src/Flow.cc:73-80: the frame warped by H as dynm_warp_perspective does, then Farneback against the previous
+   * half image), every other frame takes ComputeMask(GrayImg).  The previous half image is pyrDown of what the previous
+   * frame's ComputeMask received: its warped image when it took the homography branch.  Frame 0 has no last frame (zero
+   * field) and frame 1 no velocity yet (mVelocity is first set by frame 1's Track), so each batch starts a sequence.
+   * Poses: as the batch's motion-model search, TrackHomo projects frame t-1's points, unprojected from its filtered
+   * keypoints under Tcw[t-1], with Tcw[t].  Everything runs on the device with no host round trip inside the batch;
+   * orbs_read_homography reports each frame's branch.  Only the homography form above; a handle whose keypoint capacity
+   * (orbx_max_keypoints_for) exceeds 8192, findHomography's pair limit, returns B200ORB_EINVAL.  The chain's
+   * launches go to the stream as one CUDA graph, so orbs_submit does not wait here either.  0: none of this. */
+  int homography;
 } OrbsBatch;
 /* Host results: kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1), nmatch[n]; cap below
  * orbx_max_keypoints of the handle's extractor returns B200ORB_ECAP. */
@@ -563,6 +581,16 @@ int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, floa
 /* Frame `frame` of the last batch, which must have been masked: mask[rows][cols] 0 / 1 (the Flow::ComputeMask result,
  * FrameDrawer's mDynMask), *filtered = whether the 65 % rule dropped keypoints of this frame (NULL = skip either). */
 int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered);
+/* What TrackHomo did for frame `frame` of the last batch, which must have been a homography batch (synchronises): *branch
+ * one of ORBS_HOMO_*, *nmatches the count of its final search (0 for frames 0 and 1), *npairs points_current.size() after
+ * it, and H the model findHomography returned, row-major (zeros when there is none).  NULL = skip. */
+#define ORBS_HOMO_NO_LAST 0         /* frame 0 of the batch: no last frame */
+#define ORBS_HOMO_NO_VELOCITY 1     /* frame 1: no velocity yet */
+#define ORBS_HOMO_FEW_MATCHES 2     /* fewer than 20 matches after the retry at 2 th */
+#define ORBS_HOMO_FEW_PAIRS 3       /* at least 20 matches, at most 50 pairs */
+#define ORBS_HOMO_NO_MODEL 4        /* findHomography found no model (empty H) */
+#define ORBS_HOMO_WARPED 5          /* H found: the mask is that of the warped frame */
+int orbs_read_homography(orbs_t* h, int frame, double H[9], int* branch, int* nmatches, int* npairs);
 int orbs_sync(orbs_t* h);
 void* orbs_stream(orbs_t* h);
 long long orbs_launch_count(const orbs_t* h);

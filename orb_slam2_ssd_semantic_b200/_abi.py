@@ -51,7 +51,7 @@ class OrbsParams(C.Structure):
 class OrbsBatch(C.Structure):
     _fields_ = [("nframes", C.c_int), ("rows", C.c_int), ("cols", C.c_int), ("device", C.c_int), ("gray", vp),
                 ("depth", vp), ("depth_u16", vp), ("depth_factor", C.c_float), ("Tcw", vp), ("flow", vp),
-                ("device_flow", C.c_int), ("prev_gray", vp), ("binary_threshold", C.c_float)]
+                ("device_flow", C.c_int), ("prev_gray", vp), ("binary_threshold", C.c_float), ("homography", C.c_int)]
 
 
 class OrbsResults(C.Structure):

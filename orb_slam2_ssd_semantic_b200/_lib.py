@@ -34,7 +34,7 @@ EXPORTS = [
     "orbv_db_create", "orbv_db_destroy", "orbv_db_add", "orbv_db_erase", "orbv_db_clear", "orbv_db_query", "orbv_db_state",
     "orbv_db_launch_count",
     "orbs_create", "orbs_destroy", "orbs_submit", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_device_results",
-    "orbs_read_frame_glue", "orbs_sync", "orbs_read_dynamic_mask",
+    "orbs_read_frame_glue", "orbs_sync", "orbs_read_dynamic_mask", "orbs_read_homography",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
     "gcm_add_keyframe_objects", "gcm_add_keyframe_objects_device",
@@ -155,6 +155,7 @@ def lib() -> C.CDLL:
     L.orbs_device_results.argtypes = [vp] + [C.POINTER(vp)] * 5 + [C.POINTER(i)]
     L.orbs_read_frame_glue.argtypes = [vp, i, vp, vp, vp, vp, i]
     L.orbs_read_dynamic_mask.argtypes = [vp, i, vp, C.POINTER(i)]
+    L.orbs_read_homography.argtypes = [vp, i, vp, C.POINTER(i), C.POINTER(i), C.POINTER(i)]
     L.orbs_sync.argtypes = [vp]
     L.orbs_stream.argtypes = [vp]
     L.orbs_stream.restype = vp

@@ -447,6 +447,12 @@ int fb_pairs(cudaStream_t st, const FbGeom& g, const FbScratch& s, int nimg, flo
   return B200ORB_OK;
 }
 
+void fb_pyrdown(cudaStream_t st, const FbGeom& g, const uint8_t* first, const uint8_t* rest, int nimg, int SH, int SW,
+                uint8_t* dst, long long* launches) {
+  k_fb_pyrdown<<<dim3(fb_blocks((size_t)g.H * g.W, 256), nimg), 256, 0, st>>>(first, rest, SH, SW, dst, g.H, g.W);
+  ++*launches;
+}
+
 int fb_batch(cudaStream_t st, const FbGeom& g, const FbScratch& s, int C, const uint8_t* d_gray, const uint8_t* d_prev,
              int n, int SH, int SW, float* out, long long* launches) {
   const size_t spx = (size_t)SH * SW, fpx = (size_t)g.H * g.W * 2;
@@ -456,9 +462,7 @@ int fb_batch(cudaStream_t st, const FbGeom& g, const FbScratch& s, int C, const 
     if (t0 >= f1) continue;
     const int nimg = f1 - t0 + 1;
     const uint8_t* first = t0 == 0 ? d_prev : d_gray + (size_t)(t0 - 1) * spx;
-    k_fb_pyrdown<<<dim3(fb_blocks((size_t)g.H * g.W, 256), nimg), 256, 0, st>>>(first, d_gray + (size_t)t0 * spx, SH, SW, s.half,
-                                                                                g.H, g.W);
-    ++*launches;
+    fb_pyrdown(st, g, first, d_gray + (size_t)t0 * spx, nimg, SH, SW, s.half, launches);
     B200_CHECK(fb_pairs(st, g, s, nimg, out + (size_t)t0 * fpx, launches));
   }
   return B200ORB_OK;

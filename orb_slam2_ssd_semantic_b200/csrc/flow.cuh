@@ -33,6 +33,10 @@ int fb_geometry(int H, int W, FbGeom* g);
 void fb_take(Carver& t, FbScratch& s, const FbGeom& g, int C);
 // Farneback of the nimg - 1 consecutive pairs of the half-resolution images in s.half -> out [nimg - 1][H][W][2].
 int fb_pairs(cudaStream_t st, const FbGeom& g, const FbScratch& s, int nimg, float* out, long long* launches);
+// pyrDown(Size(SW / 2, SH / 2)) of nimg SH x SW u8 images into dst [nimg][H][W]: image 0 is `first`, image i > 0 is
+// rest + (i - 1) SH SW.
+void fb_pyrdown(cudaStream_t st, const FbGeom& g, const uint8_t* first, const uint8_t* rest, int nimg, int SH, int SW,
+                uint8_t* dst, long long* launches);
 // Flow::ComputeMask's pyrDown + Farneback for n full-resolution frames in HBM (SH x SW each): out[t] is the flow from
 // frame t-1 to frame t, where frame -1 is `d_prev`; without it out[0] is the zero field.  Chunks of at most C frames.
 int fb_batch(cudaStream_t st, const FbGeom& g, const FbScratch& s, int C, const uint8_t* d_gray, const uint8_t* d_prev,

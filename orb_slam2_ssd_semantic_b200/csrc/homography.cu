@@ -25,7 +25,6 @@ namespace b200 {
 
 constexpr int HF_MAX_ITERS = 2000;
 constexpr int HF_MAX_ATTEMPTS = 10000;
-constexpr int HF_MAX_PAIRS = 8192;
 constexpr int HF_LM_ITERS = 10;
 constexpr int HF_HYP_THREADS = 128;
 constexpr int HF_REFINE_THREADS = 512;
@@ -268,10 +267,14 @@ __device__ bool hf_check_subset(const float2* __restrict__ src, const float2* __
   return neg == 0 || neg == 4;
 }
 
-__global__ void __launch_bounds__(32) k_hf_draw(const float2* __restrict__ src, const float2* __restrict__ dst, int n,
-                                                int* __restrict__ subsets, int* __restrict__ nsub) {
+// The fit kernels read the pair count n from device memory; n == 0 (a frame of the batched chain that takes no fit) makes
+// every one of them return at once.
+__global__ void __launch_bounds__(32) k_hf_draw(const float2* __restrict__ src, const float2* __restrict__ dst,
+                                                const int* __restrict__ np, int* __restrict__ subsets,
+                                                int* __restrict__ nsub) {
   __shared__ int cand[32][4];
-  const int lane = threadIdx.x;
+  const int lane = threadIdx.x, n = *np;
+  if (n == 0) return;
   unsigned long long state = ~0ull;
   int accepted = 0, rejected = 0;
   bool done = false;
@@ -310,15 +313,15 @@ __global__ void __launch_bounds__(32) k_hf_draw(const float2* __restrict__ src, 
 }
 
 __global__ void __launch_bounds__(HF_HYP_THREADS) k_hf_hypotheses(const float2* __restrict__ src, const float2* __restrict__ dst,
-                                                                  int n, const int* __restrict__ subsets,
+                                                                  const int* __restrict__ np, const int* __restrict__ subsets,
                                                                   const int* __restrict__ nsub, double* __restrict__ hyp,
                                                                   int* __restrict__ good) {
   __shared__ HfKernel K;
   __shared__ float2 S[4], D[4];
   __shared__ double H[9];
   __shared__ float Hf[9];
-  const int it = blockIdx.x;
-  if (it >= *nsub) return;
+  const int it = blockIdx.x, n = *np;
+  if (n == 0 || it >= *nsub) return;
   if (threadIdx.x < 4) {
     const int i = subsets[it * 4 + threadIdx.x];
     S[threadIdx.x] = src[i];
@@ -486,17 +489,20 @@ __device__ void hf_norm_inf(const double* __restrict__ r, int len, HfRefine& R) 
   __syncthreads();
 }
 
-// out[0..8] H, out[9] found (as a double), mask n bytes.  tab[g] = log(1 - (1 - ep)^4) for g good pairs (NaN where
-// 1 - (1 - ep)^4 < DBL_MIN), tab[n + 1] = log(max(1 - confidence, DBL_MIN)); both from the host's libm.
+// out[0..8] H, out[9] found (as a double), mask n bytes.  tab: hf_tab's rows n0 = tab_n0 and up; row n holds tab[g] =
+// log(1 - (1 - ep)^4) for g good pairs (NaN where 1 - (1 - ep)^4 < DBL_MIN), then log(max(1 - confidence, DBL_MIN)).
 __global__ void __launch_bounds__(HF_REFINE_THREADS) k_hf_refine(const float2* __restrict__ src, const float2* __restrict__ dst,
-                                                                 int n, const int* __restrict__ nsub,
+                                                                 const int* __restrict__ np, const int* __restrict__ nsub,
                                                                  const double* __restrict__ hyp, const int* __restrict__ good,
-                                                                 const double* __restrict__ tab, float2* __restrict__ isrc,
-                                                                 float2* __restrict__ idst, double* __restrict__ J,
-                                                                 double* __restrict__ r, double* __restrict__ rd,
-                                                                 double* __restrict__ out, uint8_t* __restrict__ mask) {
+                                                                 const double* __restrict__ tab, int tab_n0,
+                                                                 float2* __restrict__ isrc, float2* __restrict__ idst,
+                                                                 double* __restrict__ J, double* __restrict__ r,
+                                                                 double* __restrict__ rd, double* __restrict__ out,
+                                                                 uint8_t* __restrict__ mask) {
   __shared__ HfRefine R;
-  const int t = threadIdx.x;
+  const int t = threadIdx.x, n = *np;
+  if (n == 0) return;
+  tab += hf_tab_row(n, tab_n0);
   if (n == 4) {   // runKernel of all four pairs, unrefined, mask all ones
     hf_run_kernel(src, dst, 4, R.K, R.x);
     if (t < 9) out[t] = R.K.ok ? R.x[t] : 0.0;
@@ -656,6 +662,42 @@ __global__ void __launch_bounds__(HF_REFINE_THREADS) k_hf_refine(const float2* _
   for (int i = t; i < n; i += blockDim.x) mask[i] = hf_error(R.Hf, src[i], dst[i]) <= HF_THRESH2;
 }
 
+void hf_tab(int n0, int n1, std::vector<double>& tab) {
+  tab.resize(hf_tab_row(n1 + 1, n0));
+  const double num = std::log(std::max(1. - 0.995, DBL_MIN));
+  for (int n = n0; n <= n1; ++n) {   // RANSACUpdateNumIters(0.995, (n - g) / n, 4, niters)'s log and pow
+    double* row = tab.data() + hf_tab_row(n, n0);
+    for (int g = 0; g <= n; ++g) {
+      double ep = (double)(n - g) / n;
+      ep = std::min(std::max(ep, 0.), 1.);
+      const double denom = 1. - std::pow(1. - ep, 4);
+      row[g] = denom < DBL_MIN ? std::nan("") : std::log(denom);
+    }
+    row[n + 1] = num;
+  }
+}
+
+void hf_take(Carver& t, HfScratch& s, int cap) {
+  s.isrc = t.take<float2>(cap); s.idst = t.take<float2>(cap);
+  s.sub = t.take<int>(4 * HF_MAX_ITERS); s.nsub = t.take<int>(1); s.good = t.take<int>(HF_MAX_ITERS);
+  s.hyp = t.take<double>(9 * HF_MAX_ITERS); s.J = t.take<double>((size_t)18 * cap);
+  s.r = t.take<double>(2 * (size_t)cap); s.rd = t.take<double>(2 * (size_t)cap);
+}
+
+int launch_hf_fit(cudaStream_t st, const float2* src, const float2* dst, const int* d_n, bool ransac, const double* tab,
+                  int tab_n0, const HfScratch& s, double* out, uint8_t* mask, long long* launches) {
+  if (ransac) {
+    k_hf_draw<<<1, 32, 0, st>>>(src, dst, d_n, s.sub, s.nsub);
+    k_hf_hypotheses<<<HF_MAX_ITERS, HF_HYP_THREADS, 0, st>>>(src, dst, d_n, s.sub, s.nsub, s.hyp, s.good);
+    *launches += 2;
+  }
+  k_hf_refine<<<1, HF_REFINE_THREADS, 0, st>>>(src, dst, d_n, s.nsub, s.hyp, s.good, tab, tab_n0, s.isrc, s.idst, s.J, s.r,
+                                               s.rd, out, mask);
+  ++*launches;
+  B200_CUDA(cudaGetLastError());
+  return B200ORB_OK;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -668,38 +710,24 @@ int dynm_find_homography(dynm_t* h, const float* src, const float* dst, int n, d
     set_error("findHomography takes 4 .. %d pairs, not %d", HF_MAX_PAIRS, n);
     return B200ORB_EINVAL;
   }
-  // RANSACUpdateNumIters' log and pow, from the host's libm: tab[g] for g = 0 .. n good pairs, then log(1 - confidence)
-  std::vector<double> tab(n + 2);
-  for (int g = 0; g <= n; ++g) {
-    double ep = (double)(n - g) / n;
-    ep = std::min(std::max(ep, 0.), 1.);
-    const double denom = 1. - std::pow(1. - ep, 4);
-    tab[g] = denom < DBL_MIN ? std::nan("") : std::log(denom);
-  }
-  tab[n + 1] = std::log(std::max(1. - 0.995, DBL_MIN));
+  std::vector<double> tab;
+  hf_tab(n, n, tab);
   DeviceGuard g(h->device);
-  float2 *d_src, *d_dst, *d_isrc, *d_idst;
-  int *d_sub, *d_nsub, *d_good;
-  double *d_hyp, *d_tab, *d_J, *d_r, *d_rd, *d_out;
+  float2 *d_src, *d_dst;
+  int* d_n;
+  double *d_tab, *d_out;
   uint8_t* d_mask;
+  HfScratch s;
   B200_CHECK(h->buf.reserve(h->stream, [&](Carver& t) {
-    d_src = t.take<float2>(n); d_dst = t.take<float2>(n); d_isrc = t.take<float2>(n); d_idst = t.take<float2>(n);
-    d_sub = t.take<int>(4 * HF_MAX_ITERS); d_nsub = t.take<int>(1); d_good = t.take<int>(HF_MAX_ITERS);
-    d_hyp = t.take<double>(9 * HF_MAX_ITERS); d_tab = t.take<double>(n + 2); d_J = t.take<double>((size_t)18 * n);
-    d_r = t.take<double>(2 * n); d_rd = t.take<double>(2 * n); d_out = t.take<double>(10); d_mask = t.take<uint8_t>(n);
+    d_src = t.take<float2>(n); d_dst = t.take<float2>(n); d_n = t.take<int>(1); d_tab = t.take<double>(tab.size());
+    d_out = t.take<double>(10); d_mask = t.take<uint8_t>(n);
+    hf_take(t, s, n);
   }));
   B200_CUDA(cudaMemcpyAsync(d_src, src, n * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(d_dst, dst, n * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
-  B200_CUDA(cudaMemcpyAsync(d_tab, tab.data(), (n + 2) * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  if (n > 4) {
-    k_hf_draw<<<1, 32, 0, h->stream>>>(d_src, d_dst, n, d_sub, d_nsub);
-    k_hf_hypotheses<<<HF_MAX_ITERS, HF_HYP_THREADS, 0, h->stream>>>(d_src, d_dst, n, d_sub, d_nsub, d_hyp, d_good);
-    h->launches += 2;
-  }
-  k_hf_refine<<<1, HF_REFINE_THREADS, 0, h->stream>>>(d_src, d_dst, n, d_nsub, d_hyp, d_good, d_tab, d_isrc, d_idst, d_J,
-                                                      d_r, d_rd, d_out, d_mask);
-  ++h->launches;
-  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaMemcpyAsync(d_n, &n, sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  B200_CUDA(cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  B200_CHECK(launch_hf_fit(h->stream, d_src, d_dst, d_n, n > 4, d_tab, n, s, d_out, d_mask, &h->launches));
   double out[10];
   B200_CUDA(cudaMemcpyAsync(out, d_out, sizeof(out), cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaMemcpyAsync(mask, d_mask, n, cudaMemcpyDeviceToHost, h->stream));

@@ -4,6 +4,7 @@
 #include <memory>
 #include <new>
 
+#include "dynm.cuh"
 #include "dynm_plane.cuh"
 #include "flow.cuh"
 #include "orbm_host.h"
@@ -110,7 +111,99 @@ __global__ void k_fill_i32(int* p, int v, size_t n) {
   if (i < n) p[i] = v;
 }
 
+// ---- TrackHomo (perfect/src/Tracking.cc:1331-1399) of homography batches --------------------------------------------
+// Per frame, what TrackHomo did: HC_WORDS ints, and out[10] doubles (H, found) beside them.
+enum { HC_BRANCH, HC_NMATCH, HC_NPAIRS, HC_NFIT, HC_WARP, HC_WORDS };
+constexpr int HC_MIN_MATCHES = 20;   // `nmatches<20` (perfect/src/Tracking.cc:1366,1374)
+constexpr int HC_MIN_PAIRS = 50;     // `points_current.size() > 50` (:1381)
+constexpr int HC_PAIR_THREADS = 1024;
+
+// `if(nmatches<20)` (perfect/src/Tracking.cc:1366): the search at 2 th takes the last frame's keypoints as its queries;
+// otherwise it takes none, and its kernels return at once.
+__global__ void k_hc_retry(const int* __restrict__ nmatch, const int* __restrict__ nlast, int* __restrict__ retry,
+                           int* __restrict__ nlast2) {
+  *retry = *nmatch < HC_MIN_MATCHES;
+  *nlast2 = *retry ? *nlast : 0;
+}
+
+// After the searches: the pairs of the final search (the second when *retry) in the order the overload pushes them (query i, the last frame's
+// keypoint i, ascending; perfect/src/ORBmatcher.cc:1835-1836) as findHomography(points_current, points_last) takes them
+// (src = the current keypoint, dst = the last one), then the branch: fewer than 20 matches, at most 50 pairs, or the fit
+// with n = the pair count.  out (H, found) starts at zero: the empty H of every branch without a model.
+__global__ void __launch_bounds__(HC_PAIR_THREADS) k_hc_pairs(const int* __restrict__ retry, const int* __restrict__ acc1,
+                                                              const int* __restrict__ nm1, const int* __restrict__ acc2,
+                                                              const int* __restrict__ nm2,
+                                                              const int* __restrict__ nlast, const float* __restrict__ lx,
+                                                              const float* __restrict__ ly, const float* __restrict__ cx,
+                                                              const float* __restrict__ cy, float2* __restrict__ src,
+                                                              float2* __restrict__ dst, int* __restrict__ st,
+                                                              double* __restrict__ out) {
+  __shared__ int ws[HC_PAIR_THREADS / 32];
+  __shared__ int base;
+  const int t = threadIdx.x, nl = *nlast;
+  const int* acc = *retry ? acc2 : acc1;
+  const int* nmatch = *retry ? nm2 : nm1;
+  if (t == 0) base = 0;
+  if (t < 10) out[t] = 0.0;
+  __syncthreads();
+  for (int b0 = 0; b0 < nl; b0 += HC_PAIR_THREADS) {
+    const int i = b0 + t, a = i < nl ? acc[i] : -1;
+    const unsigned bal = __ballot_sync(0xffffffffu, a >= 0);
+    if ((t & 31) == 0) ws[t >> 5] = __popc(bal);
+    __syncthreads();
+    if (t == 0) {
+      int s = base;
+      for (int w = 0; w < HC_PAIR_THREADS / 32; ++w) { const int c = ws[w]; ws[w] = s; s += c; }
+      base = s;
+    }
+    __syncthreads();
+    if (a >= 0) {
+      const int o = ws[t >> 5] + __popc(bal & ((1u << (t & 31)) - 1u));
+      src[o] = make_float2(cx[a], cy[a]);
+      dst[o] = make_float2(lx[i], ly[i]);
+    }
+    __syncthreads();
+  }
+  if (t == 0) {
+    const int m = *nmatch, np = base;
+    const bool fit = m >= HC_MIN_MATCHES && np > HC_MIN_PAIRS;
+    st[HC_BRANCH] = m < HC_MIN_MATCHES ? ORBS_HOMO_FEW_MATCHES : fit ? ORBS_HOMO_NO_MODEL : ORBS_HOMO_FEW_PAIRS;
+    st[HC_NMATCH] = m;
+    st[HC_NPAIRS] = np;
+    st[HC_NFIT] = fit ? np : 0;
+    st[HC_WARP] = 0;
+  }
+}
+
+// `if(flag && !homo.empty())` (perfect/src/Tracking.cc:713): a found model warps the frame
+__global__ void k_hc_found(const double* __restrict__ out, int* __restrict__ st) {
+  if (st[HC_NFIT] && out[9] != 0.0) {
+    st[HC_BRANCH] = ORBS_HOMO_WARPED;
+    st[HC_WARP] = 1;
+  }
+}
+
 }  // namespace b200
+
+// An executable graph, re-targeted in place to each newly captured graph of the same shape (else instantiated anew).
+struct GraphExec {
+  cudaGraphExec_t g = nullptr;
+  GraphExec() = default;
+  GraphExec(const GraphExec&) = delete;
+  GraphExec& operator=(const GraphExec&) = delete;
+  ~GraphExec() { if (g) cudaGraphExecDestroy(g); }
+  int update(cudaGraph_t graph) {
+    if (g) {
+      cudaGraphExecUpdateResultInfo info;
+      if (cudaGraphExecUpdate(g, graph, &info) == cudaSuccess) return B200ORB_OK;
+      cudaGetLastError();
+      cudaGraphExecDestroy(g);
+      g = nullptr;
+    }
+    B200_CUDA(cudaGraphInstantiate(&g, graph, 0));
+    return B200ORB_OK;
+  }
+};
 
 // Host batches are uploaded in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
 static constexpr int MAX_CHUNKS = 7;
@@ -156,6 +249,21 @@ struct orbs {
   FbGeom fbg;                       // and their Farneback geometry and scratch (chunks of min(maxF, FB_CHUNK) frames)
   FbScratch fbs{};
   int mask_F = 0;                // frames of the last batch that carry a dynamic mask (0: it was not masked)
+  // Homography block, reserved by the first homography batch: TrackHomo's per-frame record, its searches' outputs, the
+  // pairs, findHomography's scratch and the warped frame.  The iteration table has a block of its own, filled once per
+  // keypoint capacity.
+  DeviceBlock homo, homo_tab;
+  int* d_hstate = nullptr;       // [maxF][HC_WORDS]
+  double* d_hout = nullptr;      // [maxF][10]
+  int *d_hacc = nullptr, *d_hc2l = nullptr, *d_hnm = nullptr;   // [2][cap], [2][cap], [2]: the searches at th and 2 th
+  int *d_hretry = nullptr, *d_hnl2 = nullptr;
+  float2 *d_hsrc = nullptr, *d_hdst = nullptr;
+  uint8_t *d_hmask = nullptr, *d_dest = nullptr;
+  HfScratch hfs{};
+  double* d_tab = nullptr;
+  int tab_cap = 0;
+  GraphExec chain_exec;          // the last homography batch's launches, replayed with one graph launch
+  int homo_F = 0;                // frames of the last batch that went through TrackHomo (0: it was not a homography batch)
   bool have = false;
   int create_streams() {
     B200_CHECK(copy_stream.create());
@@ -172,6 +280,7 @@ struct orbs {
     if (!(r == rows && c == cols && F <= maxF && ex->cap == cap)) {
       rows = 0;   // no geometry until its block exists
       mask_F = 0;   // the dynamic masks of the last batch belong to the old geometry
+      homo_F = 0;
       in_depth_bytes = -1;   // the host-input block is sized for the old geometry
       const int nF = std::max(F, ex->maxF), ncap = ex->cap;
       const size_t n = (size_t)nF * ncap;
@@ -224,47 +333,153 @@ struct orbs {
     });
   }
   int fb_chunk() const { return std::min(maxF, FB_CHUNK); }
-  // Flow::ComputeMask + the masked Frame constructor's keypoint filter (perfect/src/Flow.cc:24-47, perfect/src/Frame.cc:
-  // 356-377) on the F frames the extractor has just run, in place; kpd16 (the CV_16U depth under the keypoints) moves with
-  // them.  dflow: [F][rows / 2][cols / 2][2] f32.
-  int mask_filter(const float* dflow, float thr, uint16_t* kpd16, int F) {
-    if (thr < 40.0f) thr = 40.0f;   // perfect/src/Flow.cc:24
-    return launch_dynm_plane_filter(F, dflow, rows / 2, cols / 2, thr, rows, cols, d_plane, d_msum, ex->d_kps, ex->d_desc,
-                                    kpd16, ex->d_n, cap, ex->stream, &launches);
+  // Homography batches: TrackHomo's record and scratch, and the iteration table of findHomography for every pair count
+  // the fit can take (51 .. cap), computed once on the host.
+  int ensure_homo() {
+    const size_t px = (size_t)rows * cols;
+    B200_CHECK(homo.reserve(ex->stream, [&](Carver& t) {
+      d_hstate = t.take<int>((size_t)maxF * HC_WORDS); d_hout = t.take<double>((size_t)maxF * 10);
+      d_hacc = t.take<int>(2 * (size_t)cap); d_hc2l = t.take<int>(2 * (size_t)cap); d_hnm = t.take<int>(2);
+      d_hretry = t.take<int>(1); d_hnl2 = t.take<int>(1);
+      d_hsrc = t.take<float2>(cap); d_hdst = t.take<float2>(cap); d_hmask = t.take<uint8_t>(cap);
+      d_dest = t.take<uint8_t>(px);
+      hf_take(t, hfs, cap);
+    }));
+    if (tab_cap == cap) return B200ORB_OK;
+    tab_cap = 0;
+    std::vector<double> tab;
+    if (cap > HC_MIN_PAIRS) hf_tab(HC_MIN_PAIRS + 1, cap, tab);
+    B200_CHECK(homo_tab.carve(ex->stream, [&](Carver& t) { d_tab = t.take<double>(tab.size()); }));
+    // From pageable memory the copy is staged before the call returns (so `tab` may go), and it may wait for the work
+    // already on the stream: once per handle and keypoint capacity, on its first homography batch.
+    B200_CUDA(cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, ex->stream));
+    tab_cap = cap;
+    return B200ORB_OK;
   }
-  // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  Depth is the gathered CV_16U
-  // value under each keypoint times `factor` when kpd16 is given, else the f32 image batch dd.  masked: the frames went
-  // through mask_filter, so orbs_read_dynamic_mask may read their masks.
+  // Flow::ComputeMask + the masked Frame constructor's keypoint filter (perfect/src/Flow.cc:24-47, perfect/src/Frame.cc:
+  // 356-377) on frames [f0, f0 + F) the extractor has just run, in place; kpd16 (the CV_16U depth under the keypoints)
+  // moves with them.  dflow: [F][rows / 2][cols / 2][2] f32 of those frames.
+  int mask_filter(const float* dflow, float thr, uint16_t* kpd16, int f0, int F) {
+    if (thr < 40.0f) thr = 40.0f;   // perfect/src/Flow.cc:24
+    const size_t o = (size_t)f0 * cap;
+    return launch_dynm_plane_filter(F, dflow, rows / 2, cols / 2, thr, rows, cols, d_plane + (size_t)f0 * rows * dynp_words(cols),
+                                    d_msum + f0, ex->d_kps + o, ex->d_desc + o * 32, kpd16 ? kpd16 + o : nullptr, ex->d_n + f0,
+                                    cap, ex->stream, &launches);
+  }
+  // Frame glue of frames [f0, f0 + F) as their keypoints stand.  Depth is the gathered CV_16U value under each keypoint
+  // times `factor` when kpd16 is given, else the f32 image batch dd.
+  void glue(int f0, int F, const float* dd, const uint16_t* kpd16, float factor, const float* dT) {
+    const size_t o = (size_t)f0 * cap;
+    GlueOut go{d_x + o, d_y + o, d_ang + o, d_ur + o, d_dep + o, d_xw + 3 * o, d_oct + o, d_valid + o};
+    k_frame_glue<<<dim3((cap + 255) / 256, F), 256, 0, ex->stream>>>(ex->d_kps + o, ex->d_n + f0, cap,
+                                                                    dd ? dd + (size_t)f0 * rows * cols : nullptr,
+                                                                    kpd16 ? kpd16 + o : nullptr, factor, rows, cols,
+                                                                    dT + 16 * (size_t)f0, prm.fx, prm.fy, prm.cx, prm.cy,
+                                                                    prm.bf, go);
+    ++launches;
+  }
+  // SearchByProjection(frame t + 1, frame t, th, mono = 0) for t = f0 .. f0 + npairs - 1 on the glued frames: acc[t][last
+  // keypoint] (the query's accepted current keypoint before the rotation prune), c2l[t][cur keypoint], nm[t].  nlast: the
+  // last frames' query counts (NULL: their keypoint counts).
+  int search(int f0, int npairs, float th, float nnratio, int check_ori, const int* nlast, const float* dT, int* acc, int* c2l,
+             int* nm) {
+    MatchCam cam;
+    memset(&cam, 0, sizeof(cam));
+    cam.fx = prm.fx; cam.fy = prm.fy; cam.cx = prm.cx; cam.cy = prm.cy; cam.bf = prm.bf;
+    cam.b = prm.bf / prm.fx;                       // mb = mbf/fx, src/Frame.cc:218
+    cam.min_x = 0.f; cam.max_x = (float)cols;      // no distortion: ComputeImageBounds, src/Frame.cc:617-623
+    cam.min_y = 0.f; cam.max_y = (float)rows;
+    for (int l = 0; l < prm.orb.nlevels; ++l) cam.sf[l] = ex->sf[l];
+    cam.th = th; cam.nnratio = nnratio; cam.mono = 0; cam.check_ori = check_ori;
+    cam.nlevels = prm.orb.nlevels;
+    cam.last_obs_default = 1;                      // last-frame points behave like mapped points (Observations()>0)
+    const size_t c = cap, o = (size_t)f0 * c, n = o + c;
+    CurView cv;
+    memset(&cv, 0, sizeof(cv));
+    cv.x = d_x + n; cv.y = d_y + n; cv.ang = d_ang + n; cv.uright = d_ur + n; cv.oct = d_oct + n;
+    cv.desc = ex->d_desc + n * 32; cv.obs = nullptr; cv.n = ex->d_n + f0 + 1; cv.Tcw = dT + 16 * (size_t)(f0 + 1); cv.stride = c;
+    LastView lv{d_xw + 3 * o, d_valid + o, d_oct + o, d_ang + o, ex->d_desc + o * 32, nullptr, nlast ? nlast : ex->d_n + f0,
+                dT + 16 * (size_t)f0, c};
+    return launch_match_last(cv, lv, cam, npairs, d_match_scratch, acc, c2l, nm, ex->stream, &launches);
+  }
+  // The perfect variant's live path frame after frame (perfect/src/Tracking.cc:703-719): TrackHomo against the filtered
+  // frame t-1, ComputeMask of the frame warped by its H (perfect/src/Flow.cc:73-80) or of the frame itself, and the masked
+  // constructor's filter, before frame t+1's TrackHomo reads frame t's filtered keypoints.  Each frame has the same
+  // launches; the branch is decided on the device (HC_* record) and the kernels of a branch not taken return at once.
+  // The launches (about 60 per frame, more than the device's queue of pending launches holds) are captured into a graph
+  // and go to the stream as one graph launch, so that orbs_submit never waits for the device to drain that queue.
+  int homography_chain(const uint16_t* kpd16, float factor, const float* dT, float thr, int F) {
+    cudaStream_t st = ex->stream;
+    B200_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    const int rc = chain_launches(kpd16, factor, dT, thr, F);
+    cudaGraph_t g = nullptr;
+    const cudaError_t ce = cudaStreamEndCapture(st, &g);
+    if (rc != B200ORB_OK || ce != cudaSuccess) {
+      if (g) cudaGraphDestroy(g);
+      if (rc != B200ORB_OK) return rc;
+      B200_CUDA(ce);
+    }
+    const int ur = chain_exec.update(g);
+    cudaGraphDestroy(g);
+    B200_CHECK(ur);
+    B200_CUDA(cudaGraphLaunch(chain_exec.g, st));
+    homo_F = F;
+    return B200ORB_OK;
+  }
+  int chain_launches(const uint16_t* kpd16, float factor, const float* dT, float thr, int F) {
+    cudaStream_t st = ex->stream;
+    const size_t px = (size_t)rows * cols, hpx = (size_t)fbg.H * fbg.W, fpx = hpx * 2, c = cap;
+    B200_CUDA(cudaMemsetAsync(d_hstate, 0, (size_t)F * HC_WORDS * sizeof(int), st));   // frame 0: ORBS_HOMO_NO_LAST
+    B200_CUDA(cudaMemsetAsync(d_hout, 0, (size_t)F * 10 * sizeof(double), st));
+    if (F > 1) {   // frame 1: mVelocity is first set by frame 1's Track
+      k_fill_i32<<<1, 32, 0, st>>>(d_hstate + HC_WORDS + HC_BRANCH, ORBS_HOMO_NO_VELOCITY, 1);
+      ++launches;
+    }
+    // frame 0: no mImGrayLast, the zero field (mask = ones); mImGrayLast = pyrDown(gray_0)
+    fb_pyrdown(st, fbg, d_gray, nullptr, 1, rows, cols, fbs.half, &launches);
+    B200_CUDA(cudaMemsetAsync(d_flow, 0, fpx * sizeof(float), st));
+    B200_CHECK(mask_filter(d_flow, thr, const_cast<uint16_t*>(kpd16), 0, 1));
+    for (int t = 1; t < F; ++t) {
+      const uint8_t* dest = d_gray + (size_t)t * px;
+      if (t >= 2) {
+        int* S = d_hstate + (size_t)t * HC_WORDS;
+        double* O = d_hout + (size_t)t * 10;
+        glue(t - 1, 2, nullptr, kpd16, factor, dT);   // the filtered frame t-1 and the unfiltered frame t
+        // ORBmatcher matcher(0.9, true) (perfect/src/Tracking.cc:1345): nnratio 0.9 and checkOri on
+        B200_CHECK(search(t - 1, 1, prm.th, 0.9f, 1, nullptr, dT, d_hacc, d_hc2l, d_hnm));
+        k_hc_retry<<<1, 1, 0, st>>>(d_hnm, ex->d_n + t - 1, d_hretry, d_hnl2);
+        ++launches;
+        B200_CHECK(search(t - 1, 1, 2 * prm.th, 0.9f, 1, d_hnl2, dT, d_hacc + c, d_hc2l + c, d_hnm + 1));
+        k_hc_pairs<<<1, HC_PAIR_THREADS, 0, st>>>(d_hretry, d_hacc, d_hnm, d_hacc + c, d_hnm + 1, ex->d_n + t - 1,
+                                                  d_x + (t - 1) * c, d_y + (t - 1) * c, d_x + t * c, d_y + t * c, d_hsrc,
+                                                  d_hdst, S, O);
+        ++launches;
+        B200_CHECK(launch_hf_fit(st, d_hsrc, d_hdst, S + HC_NFIT, true, d_tab, HC_MIN_PAIRS + 1, hfs, O, d_hmask, &launches));
+        k_hc_found<<<1, 1, 0, st>>>(O, S);
+        ++launches;
+        B200_CHECK(launch_warp(st, dest, 1, rows, cols, O, S + HC_WARP, d_dest, &launches));
+        dest = d_dest;
+      }
+      // Farneback(mImGrayLast, pyrDown(dest)), then mImGrayLast = pyrDown(dest) (the swap of perfect/src/Flow.cc:50):
+      // the previous frame's WARPED half image whenever that frame took the homography branch
+      fb_pyrdown(st, fbg, dest, nullptr, 1, rows, cols, fbs.half + hpx, &launches);
+      B200_CHECK(fb_pairs(st, fbg, fbs, 2, d_flow + (size_t)t * fpx, &launches));
+      B200_CUDA(cudaMemcpyAsync(fbs.half, fbs.half + hpx, hpx, cudaMemcpyDeviceToDevice, st));
+      B200_CHECK(mask_filter(d_flow + (size_t)t * fpx, thr, const_cast<uint16_t*>(kpd16), t, 1));
+    }
+    return B200ORB_OK;
+  }
+  // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  masked: the frames went through
+  // mask_filter, so orbs_read_dynamic_mask may read their masks.
   int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool masked) {
     cudaStream_t st = ex->stream;
-    GlueOut go{d_x, d_y, d_ang, d_ur, d_dep, d_xw, d_oct, d_valid};
-    k_frame_glue<<<dim3((cap + 255) / 256, F), 256, 0, st>>>(ex->d_kps, ex->d_n, cap, dd, kpd16, factor, rows, cols, dT, prm.fx, prm.fy,
-                                                            prm.cx, prm.cy, prm.bf, go);
-    ++launches;
+    glue(0, F, dd, kpd16, factor, dT);
     B200_CHECK(ex->prof_mark(ST_GLUE + 1));
     // frame 0 of the batch has no predecessor: all -1, 0 matches
     k_fill_i32<<<(cap + 255) / 256, 256, 0, st>>>(d_c2l, -1, (size_t)cap);
     ++launches;
     B200_CUDA(cudaMemsetAsync(d_nm, 0, 4, st));
-    if (F > 1) {
-      MatchCam cam;
-      memset(&cam, 0, sizeof(cam));
-      cam.fx = prm.fx; cam.fy = prm.fy; cam.cx = prm.cx; cam.cy = prm.cy; cam.bf = prm.bf;
-      cam.b = prm.bf / prm.fx;                       // mb = mbf/fx, src/Frame.cc:218
-      cam.min_x = 0.f; cam.max_x = (float)cols;      // no distortion: ComputeImageBounds, src/Frame.cc:617-623
-      cam.min_y = 0.f; cam.max_y = (float)rows;
-      for (int l = 0; l < prm.orb.nlevels; ++l) cam.sf[l] = ex->sf[l];
-      cam.th = prm.th; cam.nnratio = prm.nnratio; cam.mono = 0; cam.check_ori = prm.check_ori;
-      cam.nlevels = prm.orb.nlevels;
-      cam.last_obs_default = 1;                      // last-frame points behave like mapped points (Observations()>0)
-      const size_t c = cap;
-      CurView cv;
-      memset(&cv, 0, sizeof(cv));
-      cv.x = d_x + c; cv.y = d_y + c; cv.ang = d_ang + c; cv.uright = d_ur + c; cv.oct = d_oct + c;
-      cv.desc = ex->d_desc + c * 32; cv.obs = nullptr; cv.n = ex->d_n + 1; cv.Tcw = dT + 16; cv.stride = c;
-      LastView lv{d_xw, d_valid, d_oct, d_ang, ex->d_desc, nullptr, ex->d_n, dT, c};
-      B200_CHECK(launch_match_last(cv, lv, cam, F - 1, d_match_scratch, d_acc, d_c2l + c, d_nm + 1, st, &launches));
-    }
+    if (F > 1) B200_CHECK(search(0, F - 1, prm.th, prm.nnratio, prm.check_ori, nullptr, dT, d_acc, d_c2l + cap, d_nm + 1));
     B200_CHECK(ex->prof_mark(ST_MATCH + 1));
     lastF = F;
     mask_F = masked ? F : 0;
@@ -335,10 +550,11 @@ static int orbs_after_select(void* ctx, int f0, int F) {
   return B200ORB_OK;
 }
 
-// The seven batch forms include/b200orb.h lists under OrbsBatch; every other combination is refused.
+// The eight batch forms include/b200orb.h lists under OrbsBatch; every other combination is refused.
 static bool batch_form_ok(const OrbsBatch* b, const OrbsResults* out) {
   if (!b->gray || !b->Tcw || b->nframes <= 0 || b->rows <= 0 || b->cols <= 0) return false;
   if (!b->depth == !b->depth_u16 || (b->flow && b->device_flow) || (b->prev_gray && !b->device_flow)) return false;
+  if (b->homography != 0 && (b->homography != 1 || b->device || !b->depth_u16 || !b->device_flow || b->prev_gray)) return false;
   if (b->device) return !out && b->depth && !b->device_flow;
   return out && out->kps && out->desc && out->nkp && out->cur2last && out->nmatch &&
          (b->depth_u16 || !(b->flow || b->device_flow));
@@ -415,6 +631,14 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
   if (masked) B200_CHECK(h->check_masked(rows, cols));
   FbGeom fg;
   if (b->device_flow) B200_CHECK(fb_geometry(rows / 2, cols / 2, &fg));
+  if (b->homography) {   // TrackHomo's pairs go to findHomography, which takes at most HF_MAX_PAIRS
+    int kcap = 0;
+    B200_CHECK(orbx_max_keypoints_for(h->ex.get(), rows, cols, &kcap));
+    if (kcap > HF_MAX_PAIRS) {
+      set_error("homography batches take at most %d keypoints per frame (findHomography's pairs), not %d", HF_MAX_PAIRS, kcap);
+      return B200ORB_EINVAL;
+    }
+  }
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
@@ -434,6 +658,8 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
   B200_CHECK(h->ensure(rows, cols, F, depth_bytes));
   if (out && out->cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", out->cap, h->cap); return B200ORB_ECAP; }
   if (masked) B200_CHECK(h->ensure_dyn(b->flow && !b->device, b->device_flow ? &fg : nullptr));
+  if (b->homography) B200_CHECK(h->ensure_homo());
+  h->homo_F = 0;
   // Device batch: every input is read in place from HBM.  Host batch: from the uploaded copies.
   const float *dd = b->depth, *dflow = b->flow, *dT = b->Tcw;
   if (b->device) {
@@ -445,12 +671,16 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
     dT = h->d_T;
   }
   cudaStream_t st = h->ex->stream;
-  if (b->device_flow)
-    B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, b->prev_gray ? h->d_prev_gray : nullptr, F, rows, cols,
-                        h->d_flow, &h->launches));
-  uint16_t* kpd16 = b->depth_u16 ? h->d_kpd16 : nullptr;
-  if (masked) B200_CHECK(h->mask_filter(dflow, b->binary_threshold, kpd16, F));
   if (!b->device) B200_CUDA(cudaMemcpyAsync(h->d_T, b->Tcw, (size_t)F * 64, cudaMemcpyHostToDevice, st));
+  uint16_t* kpd16 = b->depth_u16 ? h->d_kpd16 : nullptr;
+  if (b->homography) {
+    B200_CHECK(h->homography_chain(kpd16, b->depth_factor, dT, b->binary_threshold, F));
+  } else {
+    if (b->device_flow)
+      B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, b->prev_gray ? h->d_prev_gray : nullptr, F, rows,
+                          cols, h->d_flow, &h->launches));
+    if (masked) B200_CHECK(h->mask_filter(dflow, b->binary_threshold, kpd16, 0, F));
+  }
   B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, masked));
   if (b->device) return B200ORB_OK;
   B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
@@ -476,6 +706,27 @@ int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered) {
     for (int y = 0; y < rows; ++y)
       for (int x = 0; x < cols; ++x) mask[(size_t)y * cols + x] = (words[(size_t)y * nw + (x >> 5)] >> (x & 31)) & 1u;
   if (filtered) *filtered = (double)sum > (double)(rows * cols) * 0.65;
+  return B200ORB_OK;
+}
+
+// What TrackHomo did for frame `frame` of the last batch, if that batch was a homography batch.
+int orbs_read_homography(orbs_t* h, int frame, double H[9], int* branch, int* nmatches, int* npairs) {
+  if (!h || frame < 0 || frame >= h->homo_F) {
+    set_error(h && !h->homo_F ? "the last batch was not a homography batch" : "bad argument");
+    return B200ORB_EINVAL;
+  }
+  DeviceGuard g(h->device);
+  int st[HC_WORDS];
+  double out[10];
+  cudaStream_t s = h->ex->stream;
+  B200_CUDA(cudaMemcpyAsync(st, h->d_hstate + (size_t)frame * HC_WORDS, sizeof(st), cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaMemcpyAsync(out, h->d_hout + (size_t)frame * 10, sizeof(out), cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  if (H)
+    for (int i = 0; i < 9; ++i) H[i] = out[i];
+  if (branch) *branch = st[HC_BRANCH];
+  if (nmatches) *nmatches = st[HC_NMATCH];
+  if (npairs) *npairs = st[HC_NPAIRS];
   return B200ORB_OK;
 }
 

@@ -49,16 +49,22 @@ __device__ __forceinline__ int warp_tap(const uint8_t* __restrict__ src, int row
 }
 
 // One thread per destination pixel: blockIdx.y = row, blockIdx.z = frame.  H[f] is the forward map (row-major double[9]);
-// each CTA inverts it once into shared memory.
+// each CTA inverts it once into shared memory.  take (nullable): a frame whose take[f] is 0 is copied, not warped (the
+// batched TrackHomo chain's frames without a model: dest = GrayImg).
 __global__ void __launch_bounds__(WARP_THREADS) k_warp_perspective(const uint8_t* __restrict__ src, int rows, int cols, int bw0,
-                                                                    const double* __restrict__ H, uint8_t* __restrict__ dst) {
+                                                                    const double* __restrict__ H, const int* __restrict__ take,
+                                                                    uint8_t* __restrict__ dst) {
   __shared__ double M[9];
   const size_t plane = (size_t)rows * cols;
   src += blockIdx.z * plane;
   dst += blockIdx.z * plane;
+  const int x = blockIdx.x * WARP_THREADS + threadIdx.x, y = blockIdx.y;
+  if (take && !take[blockIdx.z]) {
+    if (x < cols) dst[(size_t)y * cols + x] = src[(size_t)y * cols + x];
+    return;
+  }
   if (threadIdx.x == 0) warp_invert3(H + 9 * blockIdx.z, M);
   __syncthreads();
-  const int x = blockIdx.x * WARP_THREADS + threadIdx.x, y = blockIdx.y;
   if (x >= cols) return;
   const int x1 = x % bw0, xb = x - x1;
   const double dx1 = x1, dxb = xb, dy = y;
@@ -80,11 +86,11 @@ __global__ void __launch_bounds__(WARP_THREADS) k_warp_perspective(const uint8_t
 }
 
 // d_H: nframes forward maps; d_src / d_dst: nframes rows x cols u8 images back to back
-static int warp_core(cudaStream_t stream, const uint8_t* d_src, int nframes, int rows, int cols, const double* d_H, uint8_t* d_dst,
-                     long long* launches) {
+int launch_warp(cudaStream_t stream, const uint8_t* d_src, int nframes, int rows, int cols, const double* d_H, const int* take,
+                uint8_t* d_dst, long long* launches) {
   const int bh0 = std::min(16, rows), bw0 = std::min(1024 / bh0, cols);
   k_warp_perspective<<<dim3((cols + WARP_THREADS - 1) / WARP_THREADS, rows, nframes), WARP_THREADS, 0, stream>>>(
-      d_src, rows, cols, bw0, d_H, d_dst);
+      d_src, rows, cols, bw0, d_H, take, d_dst);
   ++*launches;
   B200_CUDA(cudaGetLastError());
   return B200ORB_OK;
@@ -117,7 +123,7 @@ int dynm_warp_perspective(dynm_t* h, const uint8_t* gray, int rows, int cols, co
   }));
   B200_CUDA(cudaMemcpyAsync(d_src, gray, px, cudaMemcpyHostToDevice, h->stream));
   B200_CUDA(cudaMemcpyAsync(d_H, H, 9 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  B200_CHECK(warp_core(h->stream, d_src, 1, rows, cols, d_H, d_dst, &h->launches));
+  B200_CHECK(launch_warp(h->stream, d_src, 1, rows, cols, d_H, nullptr, d_dst, &h->launches));
   B200_CUDA(cudaMemcpyAsync(dst, d_dst, px, cudaMemcpyDeviceToHost, h->stream));
   B200_CUDA(cudaStreamSynchronize(h->stream));
   return B200ORB_OK;
@@ -129,7 +135,7 @@ int dynm_warp_perspective_batch_device(dynm_t* h, const uint8_t* d_gray, int nfr
   B200_CHECK(warp_check(nframes, rows, cols));
   if (nframes == 0) return B200ORB_OK;
   DeviceGuard g(h->device);
-  return warp_core(h->stream, d_gray, nframes, rows, cols, d_H, d_dst, &h->launches);
+  return launch_warp(h->stream, d_gray, nframes, rows, cols, d_H, nullptr, d_dst, &h->launches);
 }
 
 }  // extern "C"

@@ -50,7 +50,7 @@ class StreamTracker:
 
     _DTYPES = dict(gray=np.uint8, depth=np.float32, depth_u16=np.uint16, Tcw=np.float32, flow=np.float32, prev_gray=np.uint8)
 
-    def _host_batch(self, form: str, wait: bool, out, depth_factor=0.0, binary_threshold=0.0, **arrays):
+    def _host_batch(self, form: str, wait: bool, out, depth_factor=0.0, binary_threshold=0.0, homography=False, **arrays):
         """One host batch through orbs_submit.  arrays: gray, one depth, Tcw, and flow or prev_gray (the flow computed on
         the device; None: the sequence starts at gray[0]).  The track_* forms (wait) convert the arrays and end in sync();
         the submit_* forms take them as they are (no hidden copies) and return after enqueueing."""
@@ -71,8 +71,8 @@ class StreamTracker:
             raise ValueError("prev_gray must be a rows x cols uint8 image or None")
         outs = out if out is not None else self.alloc_outputs(F)
         b = OrbsBatch(F, rows, cols, 0, ptr(gray), ptr(arrays.get("depth")), ptr(arrays.get("depth_u16")),
-                      float(np.float32(depth_factor)), ptr(Tcw), ptr(flow), int("prev_gray" in arrays), ptr(prev),
-                      float(binary_threshold))
+                      float(np.float32(depth_factor)), ptr(Tcw), ptr(flow), int("prev_gray" in arrays or homography),
+                      ptr(prev), float(binary_threshold), int(homography))
         _lib.check(self._L.orbs_submit(self._h, C.byref(b), C.byref(OrbsResults(*[ptr(a) for a in outs], self.cap))))
         if not wait:
             return out
@@ -127,6 +127,35 @@ class StreamTracker:
         C-contiguous and untouched until sync()."""
         return self._host_batch("submit_batch_u16_flow", False, out, depth_factor, binary_threshold, gray=gray,
                                 depth_u16=depth_u16, Tcw=Tcw, prev_gray=prev_gray)
+
+    def track_batch_u16_homography(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                                   binary_threshold: float = 40.0, out=None):
+        """track_batch_u16_flow along the reference's whole live path (perfect/src/Tracking.cc:703-719): before each
+        frame's ComputeMask, TrackHomo (:1331-1399) searches frame t against the filtered frame t-1 and, with at least 20
+        matches and more than 50 pairs, fits findHomography(points_current, points_last, RANSAC, 3); a found H makes the
+        mask that of the frame warped by H (perfect/src/Flow.cc:73-80).  Everything stays on the device; the batch starts a
+        sequence (frame 0 has no last frame, frame 1 no velocity).  homography(frame) reports each frame's branch."""
+        return self._host_batch("track_batch_u16_homography", True, out, depth_factor, binary_threshold, True, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw)
+
+    def submit_batch_u16_homography(self, gray: np.ndarray, depth_u16: np.ndarray, depth_factor: float, Tcw: np.ndarray,
+                                    binary_threshold: float, out):
+        """Asynchronous track_batch_u16_homography (as submit_batch_u16): every input must be page-locked, C-contiguous
+        and untouched until sync()."""
+        return self._host_batch("submit_batch_u16_homography", False, out, depth_factor, binary_threshold, True, gray=gray,
+                                depth_u16=depth_u16, Tcw=Tcw)
+
+    HOMO_BRANCHES = ("no_last", "no_velocity", "few_matches", "few_pairs", "no_model", "warped")
+
+    def homography(self, frame: int):
+        """-> (branch name, nmatches, npairs, H 3x3 float64 or None) of `frame` of the last batch, which must have been a
+        homography batch: what TrackHomo did for it (HOMO_BRANCHES, include/b200orb.h ORBS_HOMO_*), the count of its final
+        search, points_current.size() and the model findHomography returned."""
+        H = np.zeros(9, np.float64)
+        br, nm, npairs = C.c_int(0), C.c_int(0), C.c_int(0)
+        _lib.check(self._L.orbs_read_homography(self._h, int(frame), ptr(H), C.byref(br), C.byref(nm), C.byref(npairs)))
+        name = self.HOMO_BRANCHES[br.value]
+        return name, nm.value, npairs.value, (H.reshape(3, 3) if name == "warped" else None)
 
     def track_batch_masked_device(self, d_gray: int, d_depth: int, d_Tcw: int, d_flow: int, binary_threshold: float,
                                   nframes: int, rows: int, cols: int):
