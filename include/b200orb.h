@@ -530,7 +530,9 @@ typedef struct {
   int device_flow;
   /* With device_flow: the rows x cols u8 frame before gray[0]; NULL: the sequence starts at gray[0], which takes the zero
    * field.  The predecessor is an argument rather than handle state, so two handles chained with orbs_chain_after can
-   * carry one sequence: each batch passes the last gray frame of the batch before. */
+   * carry one sequence: each batch passes the last gray frame of the batch before.  This repairs frame 0's flow only;
+   * orbs_continue carries the whole last frame (its keypoints for frame 0's search as well as its image), and a
+   * continued batch must leave prev_gray NULL. */
   const uint8_t* prev_gray;
   float binary_threshold;       /* masked batches: Flow::ComputeMask's threshold (raised to 40) */
   /* 1: the masked batch follows the reference's live path in full (perfect/src/Tracking.cc:703-719): before each frame's
@@ -541,8 +543,9 @@ typedef struct {
    * points_last, RANSAC, 3) as dynm_find_homography does; a found H makes the frame's mask ComputeMask(GrayImg, H)
    * (perfect/src/Flow.cc:73-80: the frame warped by H as dynm_warp_perspective does, then Farneback against the previous
    * half image), every other frame takes ComputeMask(GrayImg).  The previous half image is pyrDown of what the previous
-   * frame's ComputeMask received: its warped image when it took the homography branch.  Frame 0 has no last frame (zero
-   * field) and frame 1 no velocity yet (mVelocity is first set by frame 1's Track), so each batch starts a sequence.
+   * frame's ComputeMask received: its warped image when it took the homography branch.  The sequence's frame 0 has no
+   * last frame (zero field) and its frame 1 no velocity yet (mVelocity is first set by frame 1's Track): frames 0 and 1
+   * of a batch that starts a sequence, and the frames of a continued batch (orbs_continue) at those sequence positions.
    * Poses: as the batch's motion-model search, TrackHomo projects frame t-1's points, unprojected from its filtered
    * keypoints under Tcw[t-1], with Tcw[t].  Everything runs on the device with no host round trip inside the batch;
    * orbs_read_homography reports each frame's branch.  Only the homography form above; a handle whose keypoint capacity
@@ -550,7 +553,8 @@ typedef struct {
    * launches go to the stream as one CUDA graph, so orbs_submit does not wait here either.  0: none of this. */
   int homography;
 } OrbsBatch;
-/* Host results: kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1), nmatch[n]; cap below
+/* Host results: kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1 unless the batch continues a
+ * sequence, orbs_continue), nmatch[n]; cap below
  * orbx_max_keypoints of the handle's extractor returns B200ORB_ECAP. */
 typedef struct { OrbxKeyPoint* kps; uint8_t* desc; int32_t* nkp; int32_t* cur2last; int32_t* nmatch; int cap; } OrbsResults;
 /* Tracks one batch; out is non-NULL exactly when !b->device.  Never waits: uploads, kernels and result downloads are
@@ -568,6 +572,28 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out);
  * upload(k+1) | kernels(k) | download(k-1) overlap without two batches' kernels sharing the SMs.  The dependency is
  * consumed by h's next host batch; prev must stay alive until then. */
 int orbs_chain_after(orbs_t* h, orbs_t* prev);
+/* The next batch submitted to h continues the sequence whose last frame is the last frame of the last batch submitted
+ * to prev (prev may be h).  That frame P, exactly as its batch left it (for masked and homography batches: the filtered
+ * keypoints and descriptors, glued under P's own Tcw), becomes frame -1 of h's next batch:
+ *   plain and caller-flow batches: frame 0 runs SearchByProjection(frame 0, P, th, mono = 0) with OrbsParams' nnratio
+ *     and check_ori; cur2last[0] indexes P's keypoints and nmatch[0] is its match count;
+ *   device_flow batches: frame 0's flow is Farneback(pyrDown(P's gray image), pyrDown(gray[0])), then the search above;
+ *   homography batches: a frame at sequence position g (the frames before the batch plus its index in the batch) is
+ *     ORBS_HOMO_NO_LAST only for g = 0 and ORBS_HOMO_NO_VELOCITY only for g = 1; every other frame, frame 0 included,
+ *     takes the full TrackHomo step with P as frame 0's last frame, whose previous half image is pyrDown of what P's
+ *     ComputeMask received (its warped image when P took the homography branch).
+ * The orbs_read_* entries and orbs_device_results describe frame 0 of a continued batch like any other frame.
+ * P's keypoint count, pose, glue, descriptors and (device_flow and homography batches) image are copied into h on prev's
+ * stream, behind prev's last batch and before anything submitted to prev later; the copy first waits for h's batches that
+ * still read an earlier copy, and h's next batch waits for it.  prev may be destroyed once this returns.  A device
+ * batch's Tcw buffer must still hold its poses when its handle is continued.  Exactly one batch consumes the
+ * continuation; the batch after it starts a new sequence unless orbs_continue is called again.
+ * B200ORB_EINVAL, with nothing enqueued and both handles as they were: a NULL handle, a prev that holds no batch, or a
+ * prev on another device.  orbs_submit then refuses with B200ORB_EINVAL, before anything is enqueued and with the
+ * continuation still pending, a batch whose rows / cols, OrbsParams (all but max_frames) or keypoint capacity differ from
+ * P's, a batch of another variant than P's (plain, caller flow, device_flow, homography; the depth kind and host / device
+ * may differ within the forms OrbsBatch lists) and a batch with prev_gray.  Launches one kernel. */
+int orbs_continue(orbs_t* h, orbs_t* prev);
 /* Frames per upload chunk of host batches (default 128, at most 7 chunks per call): the extraction of a chunk
  * starts as soon as it has arrived while the next one is still crossing PCIe.  Gray images and any depth that is
  * uploaded go up chunk by chunk. */

@@ -33,7 +33,8 @@ EXPORTS = [
     "orbm_search_by_projection_points", "orbm_search_by_bow", "orbm_search_by_bow_kf", "orbm_search_projected", "orbm_search_best", "orbm_search_for_initialization", "orbm_search_for_triangulation", "orbm_is_in_frustum", "orbm_undistort_keypoints", "orbv_create", "orbv_destroy", "orbv_num_words", "orbv_launch_count", "orbv_transform",
     "orbv_db_create", "orbv_db_destroy", "orbv_db_add", "orbv_db_erase", "orbv_db_clear", "orbv_db_query", "orbv_db_state",
     "orbv_db_launch_count",
-    "orbs_create", "orbs_destroy", "orbs_submit", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_device_results",
+    "orbs_create", "orbs_destroy", "orbs_submit", "orbs_set_chunk_frames", "orbs_chain_after", "orbs_continue",
+    "orbs_device_results",
     "orbs_read_frame_glue", "orbs_sync", "orbs_read_dynamic_mask", "orbs_read_homography",
     "orbs_stream", "orbs_launch_count", "orbs_extractor",
     "gcm_create", "gcm_destroy", "gcm_add_keyframe", "gcm_add_keyframe_device", "gcm_refilter", "gcm_size", "gcm_export", "gcm_sync", "gcm_launch_count",
@@ -152,6 +153,7 @@ def lib() -> C.CDLL:
     L.orbs_submit.argtypes = [vp, C.POINTER(OrbsBatch), C.POINTER(OrbsResults)]
     L.orbs_set_chunk_frames.argtypes = [vp, i]
     L.orbs_chain_after.argtypes = [vp, vp]
+    L.orbs_continue.argtypes = [vp, vp]
     L.orbs_device_results.argtypes = [vp] + [C.POINTER(vp)] * 5 + [C.POINTER(i)]
     L.orbs_read_frame_glue.argtypes = [vp, i, vp, vp, vp, vp, i]
     L.orbs_read_dynamic_mask.argtypes = [vp, i, vp, C.POINTER(i)]

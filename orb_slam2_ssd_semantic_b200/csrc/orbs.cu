@@ -183,6 +183,49 @@ __global__ void k_hc_found(const double* __restrict__ out, int* __restrict__ st)
   }
 }
 
+// ---- orbs_continue: the last frame of a batch, kept as the next batch's frame -1 --------------------------------------
+struct CarryOut {
+  float *x, *y, *ang, *xw;
+  int* oct;
+  uint8_t *valid, *desc;
+  int* n;
+  float* T;
+  uint8_t* img;   // NULL: no image is carried
+};
+struct CarrySrc {   // one frame of a batch: its glue SoA, descriptors, count and pose
+  const float *x, *y, *ang, *xw;
+  const int* oct;
+  const uint8_t *valid, *desc;
+  const int* n;
+  const float* T;
+};
+
+// Row y = 0: the frame's keypoint count, pose, glue SoA (what LastView and k_hc_pairs read) and descriptors.  Row y = 1:
+// the px-byte image its ComputeMask received -- `warped` when *warp is set (HC_WARP of a homography batch), else `gray`.
+// CARRY_CTAS CTAs per row walk either (a few thousand keypoints, a fraction of a megabyte of image).
+constexpr int CARRY_CTAS = 64;
+__global__ void __launch_bounds__(256) k_carry_gather(CarrySrc s, const uint8_t* __restrict__ gray,
+                                                      const uint8_t* __restrict__ warped, const int* __restrict__ warp,
+                                                      size_t px, CarryOut o) {
+  const int stride = gridDim.x * blockDim.x, i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  if (blockIdx.y == 0) {
+    const int n = *s.n;
+    if (i0 == 0) *o.n = n;
+    if (i0 < 16) o.T[i0] = s.T[i0];
+    for (int i = i0; i < n; i += stride) {
+      o.x[i] = s.x[i]; o.y[i] = s.y[i]; o.ang[i] = s.ang[i]; o.oct[i] = s.oct[i]; o.valid[i] = s.valid[i];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) o.xw[3 * i + r] = s.xw[3 * i + r];
+      const uint4* d = reinterpret_cast<const uint4*>(s.desc) + 2 * i;
+      uint4* e = reinterpret_cast<uint4*>(o.desc) + 2 * i;
+      e[0] = d[0]; e[1] = d[1];
+    }
+    return;
+  }
+  const uint8_t* src = (warp && *warp) ? warped : gray;
+  for (size_t i = i0; i < px; i += stride) o.img[i] = src[i];
+}
+
 }  // namespace b200
 
 // An executable graph, re-targeted in place to each newly captured graph of the same shape (else instantiated anew).
@@ -207,6 +250,17 @@ struct GraphExec {
 
 // Host batches are uploaded in at most MAX_CHUNKS chunks (orbs_set_chunk_frames sets their size).
 static constexpr int MAX_CHUNKS = 7;
+
+// The variants a continued batch must share with the batch it continues (the depth kind and host / device may differ).
+enum BatchVariant { BV_PLAIN, BV_FLOW, BV_DEVICE_FLOW, BV_HOMOGRAPHY };
+static int batch_variant(const OrbsBatch* b) {
+  return b->homography ? BV_HOMOGRAPHY : b->device_flow ? BV_DEVICE_FLOW : b->flow ? BV_FLOW : BV_PLAIN;
+}
+// OrbsParams of two handles whose batches may form one sequence: everything but the batch capacity
+static bool same_params(OrbsParams a, OrbsParams b) {
+  a.max_frames = b.max_frames = 0;
+  return memcmp(&a, &b, sizeof(a)) == 0;
+}
 
 struct orbs {
   OrbsParams prm{};
@@ -265,11 +319,56 @@ struct orbs {
   GraphExec chain_exec;          // the last homography batch's launches, replayed with one graph launch
   int homo_F = 0;                // frames of the last batch that went through TrackHomo (0: it was not a homography batch)
   bool have = false;
+  // The last batch as orbs_continue reads it: its variant, its poses when they are the caller's (device batches; host
+  // batches keep them in d_T) and the sequence position after it, saturated at 2 (TrackHomo only asks whether a frame is
+  // the sequence's first, second or a later one).
+  int last_variant = BV_PLAIN, seq_end = 0;
+  const float* last_dT = nullptr;
+  // Carry block, reserved by orbs_continue: the frame before a continued batch (frame P, the last frame of the last batch
+  // of the handle continued) -- its keypoint count, pose, glue SoA and descriptors, and for device_flow and homography
+  // batches the full-resolution image its ComputeMask received.  Written on P's handle's stream; carry_ev follows the
+  // copy, carry_free_ev the last kernel of this handle that reads it.
+  DeviceBlock carry;
+  CarryOut cy{};
+  Event carry_ev, carry_free_ev;
+  struct {
+    bool pending = false;        // the next batch continues; consumed by that batch
+    int variant = 0, seq = 0, rows = 0, cols = 0, cap = 0;
+    OrbsParams prm{};
+  } cont;
   int create_streams() {
     B200_CHECK(copy_stream.create());
     B200_CHECK(gather_stream.create());
     for (Event& e : chunk_ev) B200_CHECK(e.create());
-    for (Event* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev}) B200_CHECK(e->create());
+    for (Event* e : {&inputs_free_ev, &sel_ev, &gather_ev, &compute_done_ev, &carry_ev, &carry_free_ev}) B200_CHECK(e->create());
+    return B200ORB_OK;
+  }
+  // The carry for frames of r x c pixels and keypoint capacity kc; img: with the image.  Grow-only; a replaced block is
+  // freed by cudaFree, which waits for the device.
+  int ensure_carry(int r, int c, int kc, bool img) {
+    return carry.reserve(ex->stream, [&](Carver& t) {
+      const size_t n = kc;
+      cy.x = t.take<float>(n); cy.y = t.take<float>(n); cy.ang = t.take<float>(n); cy.xw = t.take<float>(3 * n);
+      cy.oct = t.take<int>(n); cy.valid = t.take<uint8_t>(n); cy.desc = t.take<uint8_t>(32 * n); cy.n = t.take<int>(1);
+      cy.T = t.take<float>(16);
+      cy.img = img ? t.take<uint8_t>((size_t)r * c) : nullptr;
+    });
+  }
+  // A continued batch, before it touches any state: the frame it continues has its geometry, parameters, keypoint
+  // capacity and variant, and no prev_gray competes with it.
+  int check_continue(const OrbsBatch* b) const {
+    int kcap = 0;
+    B200_CHECK(orbx_max_keypoints_for(ex.get(), b->rows, b->cols, &kcap));
+    const char* why = b->rows != cont.rows || b->cols != cont.cols ? "its image size"
+                      : !same_params(prm, cont.prm)                ? "its OrbsParams"
+                      : kcap != cont.cap                           ? "its keypoint capacity"
+                      : batch_variant(b) != cont.variant           ? "its variant"
+                      : b->prev_gray                               ? "prev_gray"
+                                                                   : nullptr;
+    if (why) {
+      set_error("a continued batch differs from the frame it continues in %s", why);
+      return B200ORB_EINVAL;
+    }
     return B200ORB_OK;
   }
   // depth_bytes: depth staging per pixel a host batch needs; -1 for a device batch, which needs no host-input
@@ -378,11 +477,21 @@ struct orbs {
                                                                     prm.bf, go);
     ++launches;
   }
-  // SearchByProjection(frame t + 1, frame t, th, mono = 0) for t = f0 .. f0 + npairs - 1 on the glued frames: acc[t][last
-  // keypoint] (the query's accepted current keypoint before the rotation prune), c2l[t][cur keypoint], nm[t].  nlast: the
-  // last frames' query counts (NULL: their keypoint counts).
-  int search(int f0, int npairs, float th, float nnratio, int check_ori, const int* nlast, const float* dT, int* acc, int* c2l,
-             int* nm) {
+  // The glued frame f of the batch as the last frame of a search (instance p: frame f + p).  nlast: its query counts
+  // (NULL: its keypoint counts).
+  LastView frame_last(int f, const int* nlast, const float* dT) const {
+    const size_t o = (size_t)f * cap;
+    return LastView{d_xw + 3 * o, d_valid + o, d_oct + o, d_ang + o, ex->d_desc + o * 32, nullptr,
+                    nlast ? nlast : ex->d_n + f, dT + 16 * (size_t)f, (size_t)cap};
+  }
+  // The carried frame P (orbs_continue) as the last frame of frame 0's search
+  LastView carry_last(const int* nlast) const {
+    return LastView{cy.xw, cy.valid, cy.oct, cy.ang, cy.desc, nullptr, nlast ? nlast : cy.n, cy.T, (size_t)cap};
+  }
+  // SearchByProjection(frame f0 + p, instance p of lv, th, mono = 0) for p = 0 .. npairs - 1 on the glued frames:
+  // acc[p][last keypoint] (the query's accepted current keypoint before the rotation prune), c2l[p][cur keypoint], nm[p].
+  int search(int f0, int npairs, const LastView& lv, float th, float nnratio, int check_ori, const float* dT, int* acc,
+             int* c2l, int* nm) {
     MatchCam cam;
     memset(&cam, 0, sizeof(cam));
     cam.fx = prm.fx; cam.fy = prm.fy; cam.cx = prm.cx; cam.cy = prm.cy; cam.bf = prm.bf;
@@ -393,13 +502,11 @@ struct orbs {
     cam.th = th; cam.nnratio = nnratio; cam.mono = 0; cam.check_ori = check_ori;
     cam.nlevels = prm.orb.nlevels;
     cam.last_obs_default = 1;                      // last-frame points behave like mapped points (Observations()>0)
-    const size_t c = cap, o = (size_t)f0 * c, n = o + c;
+    const size_t c = cap, n = (size_t)f0 * c;
     CurView cv;
     memset(&cv, 0, sizeof(cv));
     cv.x = d_x + n; cv.y = d_y + n; cv.ang = d_ang + n; cv.uright = d_ur + n; cv.oct = d_oct + n;
-    cv.desc = ex->d_desc + n * 32; cv.obs = nullptr; cv.n = ex->d_n + f0 + 1; cv.Tcw = dT + 16 * (size_t)(f0 + 1); cv.stride = c;
-    LastView lv{d_xw + 3 * o, d_valid + o, d_oct + o, d_ang + o, ex->d_desc + o * 32, nullptr, nlast ? nlast : ex->d_n + f0,
-                dT + 16 * (size_t)f0, c};
+    cv.desc = ex->d_desc + n * 32; cv.obs = nullptr; cv.n = ex->d_n + f0; cv.Tcw = dT + 16 * (size_t)f0; cv.stride = c;
     return launch_match_last(cv, lv, cam, npairs, d_match_scratch, acc, c2l, nm, ex->stream, &launches);
   }
   // The perfect variant's live path frame after frame (perfect/src/Tracking.cc:703-719): TrackHomo against the filtered
@@ -408,10 +515,11 @@ struct orbs {
   // launches; the branch is decided on the device (HC_* record) and the kernels of a branch not taken return at once.
   // The launches (about 60 per frame, more than the device's queue of pending launches holds) are captured into a graph
   // and go to the stream as one graph launch, so that orbs_submit never waits for the device to drain that queue.
-  int homography_chain(const uint16_t* kpd16, float factor, const float* dT, float thr, int F) {
+  // s: the frames of the sequence before this batch (saturated at 2); with s > 0 the carried frame P is frame -1.
+  int homography_chain(const uint16_t* kpd16, float factor, const float* dT, float thr, int F, int s) {
     cudaStream_t st = ex->stream;
     B200_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = chain_launches(kpd16, factor, dT, thr, F);
+    const int rc = chain_launches(kpd16, factor, dT, thr, F, s);
     cudaGraph_t g = nullptr;
     const cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc != B200ORB_OK || ce != cudaSuccess) {
@@ -426,33 +534,45 @@ struct orbs {
     homo_F = F;
     return B200ORB_OK;
   }
-  int chain_launches(const uint16_t* kpd16, float factor, const float* dT, float thr, int F) {
+  int chain_launches(const uint16_t* kpd16, float factor, const float* dT, float thr, int F, int s) {
     cudaStream_t st = ex->stream;
     const size_t px = (size_t)rows * cols, hpx = (size_t)fbg.H * fbg.W, fpx = hpx * 2, c = cap;
-    B200_CUDA(cudaMemsetAsync(d_hstate, 0, (size_t)F * HC_WORDS * sizeof(int), st));   // frame 0: ORBS_HOMO_NO_LAST
+    // sequence frame 0: ORBS_HOMO_NO_LAST
+    B200_CUDA(cudaMemsetAsync(d_hstate, 0, (size_t)F * HC_WORDS * sizeof(int), st));
     B200_CUDA(cudaMemsetAsync(d_hout, 0, (size_t)F * 10 * sizeof(double), st));
-    if (F > 1) {   // frame 1: mVelocity is first set by frame 1's Track
-      k_fill_i32<<<1, 32, 0, st>>>(d_hstate + HC_WORDS + HC_BRANCH, ORBS_HOMO_NO_VELOCITY, 1);
+    if (s <= 1 && 1 - s < F) {   // sequence frame 1: mVelocity is first set by frame 1's Track
+      k_fill_i32<<<1, 32, 0, st>>>(d_hstate + (1 - s) * HC_WORDS + HC_BRANCH, ORBS_HOMO_NO_VELOCITY, 1);
       ++launches;
     }
-    // frame 0: no mImGrayLast, the zero field (mask = ones); mImGrayLast = pyrDown(gray_0)
-    fb_pyrdown(st, fbg, d_gray, nullptr, 1, rows, cols, fbs.half, &launches);
-    B200_CUDA(cudaMemsetAsync(d_flow, 0, fpx * sizeof(float), st));
-    B200_CHECK(mask_filter(d_flow, thr, const_cast<uint16_t*>(kpd16), 0, 1));
-    for (int t = 1; t < F; ++t) {
+    int t0 = 0;
+    if (s == 0) {
+      // sequence frame 0: no mImGrayLast, the zero field (mask = ones); mImGrayLast = pyrDown(gray_0)
+      fb_pyrdown(st, fbg, d_gray, nullptr, 1, rows, cols, fbs.half, &launches);
+      B200_CUDA(cudaMemsetAsync(d_flow, 0, fpx * sizeof(float), st));
+      B200_CHECK(mask_filter(d_flow, thr, const_cast<uint16_t*>(kpd16), 0, 1));
+      t0 = 1;
+    } else {
+      // mImGrayLast = pyrDown of what P's ComputeMask received
+      fb_pyrdown(st, fbg, cy.img, nullptr, 1, rows, cols, fbs.half, &launches);
+    }
+    for (int t = t0; t < F; ++t) {
       const uint8_t* dest = d_gray + (size_t)t * px;
-      if (t >= 2) {
+      if (s + t >= 2) {
         int* S = d_hstate + (size_t)t * HC_WORDS;
         double* O = d_hout + (size_t)t * 10;
-        glue(t - 1, 2, nullptr, kpd16, factor, dT);   // the filtered frame t-1 and the unfiltered frame t
+        // the last frame: the filtered frame t-1, or P before frame 0 (glued by its own batch)
+        const int* nl = t ? ex->d_n + t - 1 : cy.n;
+        const float *lx = t ? d_x + (t - 1) * c : cy.x, *ly = t ? d_y + (t - 1) * c : cy.y;
+        glue(t ? t - 1 : 0, t ? 2 : 1, nullptr, kpd16, factor, dT);   // the filtered frame t-1 and the unfiltered frame t
         // ORBmatcher matcher(0.9, true) (perfect/src/Tracking.cc:1345): nnratio 0.9 and checkOri on
-        B200_CHECK(search(t - 1, 1, prm.th, 0.9f, 1, nullptr, dT, d_hacc, d_hc2l, d_hnm));
-        k_hc_retry<<<1, 1, 0, st>>>(d_hnm, ex->d_n + t - 1, d_hretry, d_hnl2);
+        B200_CHECK(search(t, 1, t ? frame_last(t - 1, nullptr, dT) : carry_last(nullptr), prm.th, 0.9f, 1, dT, d_hacc,
+                          d_hc2l, d_hnm));
+        k_hc_retry<<<1, 1, 0, st>>>(d_hnm, nl, d_hretry, d_hnl2);
         ++launches;
-        B200_CHECK(search(t - 1, 1, 2 * prm.th, 0.9f, 1, d_hnl2, dT, d_hacc + c, d_hc2l + c, d_hnm + 1));
-        k_hc_pairs<<<1, HC_PAIR_THREADS, 0, st>>>(d_hretry, d_hacc, d_hnm, d_hacc + c, d_hnm + 1, ex->d_n + t - 1,
-                                                  d_x + (t - 1) * c, d_y + (t - 1) * c, d_x + t * c, d_y + t * c, d_hsrc,
-                                                  d_hdst, S, O);
+        B200_CHECK(search(t, 1, t ? frame_last(t - 1, d_hnl2, dT) : carry_last(d_hnl2), 2 * prm.th, 0.9f, 1, dT,
+                          d_hacc + c, d_hc2l + c, d_hnm + 1));
+        k_hc_pairs<<<1, HC_PAIR_THREADS, 0, st>>>(d_hretry, d_hacc, d_hnm, d_hacc + c, d_hnm + 1, nl, lx, ly, d_x + t * c,
+                                                  d_y + t * c, d_hsrc, d_hdst, S, O);
         ++launches;
         B200_CHECK(launch_hf_fit(st, d_hsrc, d_hdst, S + HC_NFIT, true, d_tab, HC_MIN_PAIRS + 1, hfs, O, d_hmask, &launches));
         k_hc_found<<<1, 1, 0, st>>>(O, S);
@@ -470,16 +590,21 @@ struct orbs {
     return B200ORB_OK;
   }
   // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  masked: the frames went through
-  // mask_filter, so orbs_read_dynamic_mask may read their masks.
-  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool masked) {
+  // mask_filter, so orbs_read_dynamic_mask may read their masks.  cont: frame 0 is searched against the carried frame P.
+  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool masked, bool cont) {
     cudaStream_t st = ex->stream;
     glue(0, F, dd, kpd16, factor, dT);
     B200_CHECK(ex->prof_mark(ST_GLUE + 1));
-    // frame 0 of the batch has no predecessor: all -1, 0 matches
-    k_fill_i32<<<(cap + 255) / 256, 256, 0, st>>>(d_c2l, -1, (size_t)cap);
-    ++launches;
-    B200_CUDA(cudaMemsetAsync(d_nm, 0, 4, st));
-    if (F > 1) B200_CHECK(search(0, F - 1, prm.th, prm.nnratio, prm.check_ori, nullptr, dT, d_acc, d_c2l + cap, d_nm + 1));
+    if (cont) {
+      B200_CHECK(search(0, 1, carry_last(nullptr), prm.th, prm.nnratio, prm.check_ori, dT, d_acc, d_c2l, d_nm));
+    } else {   // frame 0 of the batch has no predecessor: all -1, 0 matches
+      k_fill_i32<<<(cap + 255) / 256, 256, 0, st>>>(d_c2l, -1, (size_t)cap);
+      ++launches;
+      B200_CUDA(cudaMemsetAsync(d_nm, 0, 4, st));
+    }
+    if (F > 1)
+      B200_CHECK(search(1, F - 1, frame_last(0, nullptr, dT), prm.th, prm.nnratio, prm.check_ori, dT, d_acc, d_c2l + cap,
+                        d_nm + 1));
     B200_CHECK(ex->prof_mark(ST_MATCH + 1));
     lastF = F;
     mask_F = masked ? F : 0;
@@ -639,6 +764,8 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
       return B200ORB_EINVAL;
     }
   }
+  const bool cont = h->cont.pending;
+  if (cont) B200_CHECK(h->check_continue(b));
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
@@ -660,6 +787,9 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
   if (masked) B200_CHECK(h->ensure_dyn(b->flow && !b->device, b->device_flow ? &fg : nullptr));
   if (b->homography) B200_CHECK(h->ensure_homo());
   h->homo_F = 0;
+  // The continuation is consumed by this batch; its frames take sequence positions s .. s + F - 1.
+  const int s = cont ? h->cont.seq : 0;
+  h->cont.pending = false;
   // Device batch: every input is read in place from HBM.  Host batch: from the uploaded copies.
   const float *dd = b->depth, *dflow = b->flow, *dT = b->Tcw;
   if (b->device) {
@@ -671,17 +801,24 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
     dT = h->d_T;
   }
   cudaStream_t st = h->ex->stream;
+  if (cont) B200_CUDA(cudaStreamWaitEvent(st, h->carry_ev, 0));   // the carry copy, on the other handle's stream
   if (!b->device) B200_CUDA(cudaMemcpyAsync(h->d_T, b->Tcw, (size_t)F * 64, cudaMemcpyHostToDevice, st));
   uint16_t* kpd16 = b->depth_u16 ? h->d_kpd16 : nullptr;
   if (b->homography) {
-    B200_CHECK(h->homography_chain(kpd16, b->depth_factor, dT, b->binary_threshold, F));
+    B200_CHECK(h->homography_chain(kpd16, b->depth_factor, dT, b->binary_threshold, F, s));
   } else {
+    // frame 0's flow: from prev_gray, from P's image when continued, else the zero field
     if (b->device_flow)
-      B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray, b->prev_gray ? h->d_prev_gray : nullptr, F, rows,
-                          cols, h->d_flow, &h->launches));
+      B200_CHECK(fb_batch(st, h->fbg, h->fbs, h->fb_chunk(), h->d_gray,
+                          b->prev_gray ? h->d_prev_gray : cont ? h->cy.img : nullptr, F, rows, cols, h->d_flow,
+                          &h->launches));
     if (masked) B200_CHECK(h->mask_filter(dflow, b->binary_threshold, kpd16, 0, F));
   }
-  B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, masked));
+  B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, masked, cont));
+  if (cont) B200_CUDA(cudaEventRecord(h->carry_free_ev, st));   // the last read of the carry
+  h->last_variant = batch_variant(b);
+  h->seq_end = std::min(2, s + F);
+  h->last_dT = b->device ? b->Tcw : nullptr;
   if (b->device) return B200ORB_OK;
   B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
   return download(h, out, F);
@@ -744,6 +881,39 @@ int orbs_set_chunk_frames(orbs_t* h, int frames) {
 int orbs_chain_after(orbs_t* h, orbs_t* prev) {
   if (!h || !prev || h == prev || h->device != prev->device) { set_error("bad argument"); return B200ORB_EINVAL; }
   h->chain_prev = prev;
+  return B200ORB_OK;
+}
+
+// h's next batch continues the sequence of prev's last batch: its last frame P is copied into h's carry on prev's
+// stream, behind that batch and before anything submitted to prev later.  The copy waits for h's last batch that read the
+// carry and for a continuation still pending on h; h's next batch waits for the copy.
+int orbs_continue(orbs_t* h, orbs_t* prev) {
+  if (!h || !prev || !prev->have || h->device != prev->device) { set_error("bad argument"); return B200ORB_EINVAL; }
+  DeviceGuard g(h->device);
+  const bool img = prev->last_variant == BV_DEVICE_FLOW || prev->last_variant == BV_HOMOGRAPHY;
+  B200_CHECK(h->ensure_carry(prev->rows, prev->cols, prev->cap, img));
+  cudaStream_t ps = prev->ex->stream;
+  B200_CUDA(cudaStreamWaitEvent(ps, h->carry_free_ev, 0));
+  if (h->cont.pending) B200_CUDA(cudaStreamWaitEvent(ps, h->carry_ev, 0));
+  const int f = prev->lastF - 1;
+  const size_t o = (size_t)f * prev->cap, px = (size_t)prev->rows * prev->cols;
+  const CarrySrc src{prev->d_x + o, prev->d_y + o, prev->d_ang + o, prev->d_xw + 3 * o, prev->d_oct + o, prev->d_valid + o,
+                     prev->ex->d_desc + 32 * o, prev->ex->d_n + f,
+                     prev->last_dT ? prev->last_dT + 16 * (size_t)f : prev->d_T + 16 * (size_t)f};
+  const bool homo = prev->last_variant == BV_HOMOGRAPHY;
+  k_carry_gather<<<dim3(CARRY_CTAS, img ? 2 : 1), 256, 0, ps>>>(
+      src, img ? prev->d_gray + f * px : nullptr, homo ? prev->d_dest : nullptr,
+      homo ? prev->d_hstate + f * HC_WORDS + HC_WARP : nullptr, px, h->cy);
+  ++h->launches;
+  B200_CUDA(cudaGetLastError());
+  B200_CUDA(cudaEventRecord(h->carry_ev, ps));
+  h->cont.pending = true;
+  h->cont.variant = prev->last_variant;
+  h->cont.seq = prev->seq_end;
+  h->cont.rows = prev->rows;
+  h->cont.cols = prev->cols;
+  h->cont.cap = prev->cap;
+  h->cont.prm = prev->prm;
   return B200ORB_OK;
 }
 

@@ -134,7 +134,7 @@ class StreamTracker:
         frame's ComputeMask, TrackHomo (:1331-1399) searches frame t against the filtered frame t-1 and, with at least 20
         matches and more than 50 pairs, fits findHomography(points_current, points_last, RANSAC, 3); a found H makes the
         mask that of the frame warped by H (perfect/src/Flow.cc:73-80).  Everything stays on the device; the batch starts a
-        sequence (frame 0 has no last frame, frame 1 no velocity).  homography(frame) reports each frame's branch."""
+        sequence (frame 0 has no last frame, frame 1 no velocity) unless continue_after() carries one into it.  homography(frame) reports each frame's branch."""
         return self._host_batch("track_batch_u16_homography", True, out, depth_factor, binary_threshold, True, gray=gray,
                                 depth_u16=depth_u16, Tcw=Tcw)
 
@@ -185,6 +185,13 @@ class StreamTracker:
     def chain_after(self, prev: "StreamTracker"):
         """The next submitted batch starts its kernels when `prev`'s kernels are done (uploads are not held back)."""
         _lib.check(self._L.orbs_chain_after(self._h, prev._h))
+
+    def continue_after(self, prev: "StreamTracker"):
+        """The next submitted batch continues the sequence of `prev`'s last batch (prev may be self): its frame 0 is
+        tracked against that batch's last frame, a device_flow batch takes that frame's image as frame 0's predecessor,
+        and a homography batch's TrackHomo chain carries on.  Consumed by the next batch; `prev` may go once this
+        returns."""
+        _lib.check(self._L.orbs_continue(self._h, prev._h))
 
     def track_batch_device(self, d_gray: int, d_depth: int, d_Tcw: int, nframes: int, rows: int, cols: int):
         """Device pointers (ints) in; results stay in HBM (device_results()). Asynchronous."""
