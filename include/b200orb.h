@@ -554,8 +554,8 @@ typedef struct {
   int homography;
 } OrbsBatch;
 /* Host results: kps[n][cap], desc[n][cap][32], nkp[n], cur2last[n][cap] (frame 0: all -1 unless the batch continues a
- * sequence, orbs_continue), nmatch[n]; cap below
- * orbx_max_keypoints of the handle's extractor returns B200ORB_ECAP. */
+ * sequence, orbs_continue), nmatch[n]; cap below the keypoint capacity of the batch's image size
+ * (orbx_max_keypoints_for) returns B200ORB_ECAP. */
 typedef struct { OrbxKeyPoint* kps; uint8_t* desc; int32_t* nkp; int32_t* cur2last; int32_t* nmatch; int cap; } OrbsResults;
 /* Tracks one batch; out is non-NULL exactly when !b->device.  Never waits: uploads, kernels and result downloads are
  * enqueued on the handle's streams (orbs_stream for the kernels) and the results are valid after orbs_sync(h); the
@@ -565,7 +565,11 @@ typedef struct { OrbxKeyPoint* kps; uint8_t* desc; int32_t* nkp; int32_t* cur2la
  * Examples/RGB-D/rgbd_tum.cc:88-109, done here for whole batches).
  * Only host batches take part in orbs_chain_after: a host batch consumes the dependency set on h and records the end
  * of its kernels for a handle chained after h.  A device batch neither waits for the dependency (it stays set for h's
- * next host batch) nor records. */
+ * next host batch) nor records.
+ * Every refusal -- B200ORB_EINVAL for the forms, sizes and continuations described here and B200ORB_ECAP -- returns
+ * before anything is enqueued and before any handle state changes; the last batch stays readable.  A submit that fails
+ * after that point (an allocation, a launch) leaves h with no batch: orbs_device_results, the orbs_read_* entries and
+ * orbs_continue(., h) return B200ORB_EINVAL until a batch succeeds. */
 int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out);
 /* Pipelining aid for two handles used alternately: the next host batch submitted to h starts its kernels only when the
  * kernels of prev's last host batch are done; h's uploads and prev's downloads proceed meanwhile, so the stages
@@ -600,9 +604,9 @@ int orbs_continue(orbs_t* h, orbs_t* prev);
 int orbs_set_chunk_frames(orbs_t* h, int frames);
 int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d_desc, const int32_t** d_nkp,
                         const int32_t** d_cur2last, const int32_t** d_nmatch, int* cap);
-/* Frame glue of frame `frame` of the last batch: mvuRight / mvDepth (Frame::ComputeStereoFromRGBD, src/Frame.cc:850-871), the
- * world point Frame::UnprojectStereo gives per keypoint under that frame's pose (:879-899) and whether the keypoint has
- * depth; host arrays of at least the handle's keypoint capacity (NULL = skip). */
+/* Frame glue of frame `frame`, in [0, nframes) of the last batch: mvuRight / mvDepth (Frame::ComputeStereoFromRGBD,
+ * src/Frame.cc:850-871), the world point Frame::UnprojectStereo gives per keypoint under that frame's pose (:879-899) and
+ * whether the keypoint has depth; host arrays of at least the handle's keypoint capacity (NULL = skip). */
 int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, float* xw, uint8_t* valid, int cap);
 /* Frame `frame` of the last batch, which must have been masked: mask[rows][cols] 0 / 1 (the Flow::ComputeMask result,
  * FrameDrawer's mDynMask), *filtered = whether the 65 % rule dropped keypoints of this frame (NULL = skip either). */

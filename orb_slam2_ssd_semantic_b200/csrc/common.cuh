@@ -94,7 +94,9 @@ struct Block {
       release();
     }
     void* q = nullptr;
-    B200_CUDA(PINNED ? cudaHostAlloc(&q, n, cudaHostAllocDefault) : cudaMalloc(&q, n));
+    const cudaError_t e = PINNED ? cudaHostAlloc(&q, n, cudaHostAllocDefault) : cudaMalloc(&q, n);
+    if (e != cudaSuccess) cudaGetLastError();   // consume the refusal, so that the next launch check does not report it
+    B200_CUDA(e);
     p = q;
     bytes = n;
     return cut(take_all);

@@ -262,12 +262,21 @@ static bool same_params(OrbsParams a, OrbsParams b) {
   return memcmp(&a, &b, sizeof(a)) == 0;
 }
 
+// One enqueued batch, as the readers and orbs_continue see it.  F = 0: no batch.
+struct BatchRecord {
+  int F = 0, rows = 0, cols = 0, cap = 0;
+  int variant = BV_PLAIN;     // flow, device_flow and homography batches are masked; only homography batches ran TrackHomo
+  int seq_end = 0;            // the sequence position after it, saturated at 2 (TrackHomo asks: first, second or later)
+  const float* dT = nullptr;  // a device batch's poses, the caller's buffer; NULL: a host batch, whose poses are in d_T
+  OrbsParams prm{};
+};
+
 struct orbs {
   OrbsParams prm{};
   int device = 0;
   std::unique_ptr<orbx> ex;
   long long launches = 0;
-  int rows = 0, cols = 0, maxF = 0, cap = 0, lastF = 0;
+  int rows = 0, cols = 0, maxF = 0, cap = 0;
   // Geometry block, carved for (rows, cols, maxF, cap): the glue's SoA, the match results and the scratch of the
   // non-fused LAST search.
   DeviceBlock geom;
@@ -302,7 +311,6 @@ struct orbs {
   uint8_t* d_prev_gray = nullptr;   // prev_gray of batches with device_flow
   FbGeom fbg;                       // and their Farneback geometry and scratch (chunks of min(maxF, FB_CHUNK) frames)
   FbScratch fbs{};
-  int mask_F = 0;                // frames of the last batch that carry a dynamic mask (0: it was not masked)
   // Homography block, reserved by the first homography batch: TrackHomo's per-frame record, its searches' outputs, the
   // pairs, findHomography's scratch and the warped frame.  The iteration table has a block of its own, filled once per
   // keypoint capacity.
@@ -317,13 +325,8 @@ struct orbs {
   double* d_tab = nullptr;
   int tab_cap = 0;
   GraphExec chain_exec;          // the last homography batch's launches, replayed with one graph launch
-  int homo_F = 0;                // frames of the last batch that went through TrackHomo (0: it was not a homography batch)
-  bool have = false;
-  // The last batch as orbs_continue reads it: its variant, its poses when they are the caller's (device batches; host
-  // batches keep them in d_T) and the sequence position after it, saturated at 2 (TrackHomo only asks whether a frame is
-  // the sequence's first, second or a later one).
-  int last_variant = BV_PLAIN, seq_end = 0;
-  const float* last_dT = nullptr;
+  // The last batch: cleared before orbs_submit changes any state, written once a batch is wholly enqueued.
+  BatchRecord last;
   // Carry block, reserved by orbs_continue: the frame before a continued batch (frame P, the last frame of the last batch
   // of the handle continued) -- its keypoint count, pose, glue SoA and descriptors, and for device_flow and homography
   // batches the full-resolution image its ComputeMask received.  Written on P's handle's stream; carry_ev follows the
@@ -333,8 +336,7 @@ struct orbs {
   Event carry_ev, carry_free_ev;
   struct {
     bool pending = false;        // the next batch continues; consumed by that batch
-    int variant = 0, seq = 0, rows = 0, cols = 0, cap = 0;
-    OrbsParams prm{};
+    BatchRecord from;            // the batch whose last frame the carry holds
   } cont;
   int create_streams() {
     B200_CHECK(copy_stream.create());
@@ -354,17 +356,16 @@ struct orbs {
       cy.img = img ? t.take<uint8_t>((size_t)r * c) : nullptr;
     });
   }
-  // A continued batch, before it touches any state: the frame it continues has its geometry, parameters, keypoint
-  // capacity and variant, and no prev_gray competes with it.
-  int check_continue(const OrbsBatch* b) const {
-    int kcap = 0;
-    B200_CHECK(orbx_max_keypoints_for(ex.get(), b->rows, b->cols, &kcap));
-    const char* why = b->rows != cont.rows || b->cols != cont.cols ? "its image size"
-                      : !same_params(prm, cont.prm)                ? "its OrbsParams"
-                      : kcap != cont.cap                           ? "its keypoint capacity"
-                      : batch_variant(b) != cont.variant           ? "its variant"
-                      : b->prev_gray                               ? "prev_gray"
-                                                                   : nullptr;
+  // A continued batch of keypoint capacity kcap, before it touches any state: the frame it continues has its geometry,
+  // parameters, keypoint capacity and variant, and no prev_gray competes with it.
+  int check_continue(const OrbsBatch* b, int kcap) const {
+    const BatchRecord& p = cont.from;
+    const char* why = b->rows != p.rows || b->cols != p.cols ? "its image size"
+                      : !same_params(prm, p.prm)            ? "its OrbsParams"
+                      : kcap != p.cap                       ? "its keypoint capacity"
+                      : batch_variant(b) != p.variant       ? "its variant"
+                      : b->prev_gray                        ? "prev_gray"
+                                                            : nullptr;
     if (why) {
       set_error("a continued batch differs from the frame it continues in %s", why);
       return B200ORB_EINVAL;
@@ -378,8 +379,6 @@ struct orbs {
     B200_CHECK(ex->ensure_geometry(r, c, F));
     if (!(r == rows && c == cols && F <= maxF && ex->cap == cap)) {
       rows = 0;   // no geometry until its block exists
-      mask_F = 0;   // the dynamic masks of the last batch belong to the old geometry
-      homo_F = 0;
       in_depth_bytes = -1;   // the host-input block is sized for the old geometry
       const int nF = std::max(F, ex->maxF), ncap = ex->cap;
       const size_t n = (size_t)nF * ncap;
@@ -531,7 +530,6 @@ struct orbs {
     cudaGraphDestroy(g);
     B200_CHECK(ur);
     B200_CUDA(cudaGraphLaunch(chain_exec.g, st));
-    homo_F = F;
     return B200ORB_OK;
   }
   int chain_launches(const uint16_t* kpd16, float factor, const float* dT, float thr, int F, int s) {
@@ -589,9 +587,9 @@ struct orbs {
     }
     return B200ORB_OK;
   }
-  // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  masked: the frames went through
-  // mask_filter, so orbs_read_dynamic_mask may read their masks.  cont: frame 0 is searched against the carried frame P.
-  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool masked, bool cont) {
+  // Frame glue and SearchByProjection(t, t-1) of the F frames the extractor has just run.  cont: frame 0 is searched
+  // against the carried frame P.
+  int run(const float* dd, const uint16_t* kpd16, float factor, const float* dT, int F, bool cont) {
     cudaStream_t st = ex->stream;
     glue(0, F, dd, kpd16, factor, dT);
     B200_CHECK(ex->prof_mark(ST_GLUE + 1));
@@ -605,13 +603,23 @@ struct orbs {
     if (F > 1)
       B200_CHECK(search(1, F - 1, frame_last(0, nullptr, dT), prm.th, prm.nnratio, prm.check_ori, dT, d_acc, d_c2l + cap,
                         d_nm + 1));
-    B200_CHECK(ex->prof_mark(ST_MATCH + 1));
-    lastF = F;
-    mask_F = masked ? F : 0;
-    have = true;
-    return B200ORB_OK;
+    return ex->prof_mark(ST_MATCH + 1);
   }
 };
+
+// The one check of every reader of the last batch and of orbs_continue: h holds a batch, `frame` is one of its frames and
+// the batch is of the kind the reader needs.
+enum LastNeed { ANY_BATCH, MASKED_BATCH, HOMO_BATCH };
+static int check_last(const orbs* h, int frame, LastNeed need) {
+  const char* why = !h                                                       ? "bad argument"
+                    : !h->last.F                                             ? "no results"
+                    : need == MASKED_BATCH && h->last.variant == BV_PLAIN    ? "the last batch was not masked"
+                    : need == HOMO_BATCH && h->last.variant != BV_HOMOGRAPHY ? "the last batch was not a homography batch"
+                    : frame < 0 || frame >= h->last.F                        ? "frame outside the last batch"
+                                                                             : nullptr;
+  if (why) set_error("%s", why);
+  return why ? B200ORB_EINVAL : B200ORB_OK;
+}
 
 extern "C" {
 
@@ -634,22 +642,23 @@ void orbs_destroy(orbs_t* h) { destroy_handle(h); }
 
 int orbs_device_results(orbs_t* h, const OrbxKeyPoint** d_kps, const uint8_t** d_desc, const int32_t** d_nkp,
                         const int32_t** d_cur2last, const int32_t** d_nmatch, int* cap) {
-  if (!h || !h->have) { set_error("no results"); return B200ORB_EINVAL; }
+  B200_CHECK(check_last(h, 0, ANY_BATCH));
   if (d_kps) *d_kps = h->ex->d_kps;
   if (d_desc) *d_desc = h->ex->d_desc;
   if (d_nkp) *d_nkp = h->ex->d_n;
   if (d_cur2last) *d_cur2last = h->d_c2l;
   if (d_nmatch) *d_nmatch = h->d_nm;
-  if (cap) *cap = h->cap;
+  if (cap) *cap = h->last.cap;
   return B200ORB_OK;
 }
 
 // Frame-glue outputs of frame `frame` of the last batch (Frame::ComputeStereoFromRGBD + UnprojectStereo per keypoint):
 // mvuRight, mvDepth, the world point of the keypoint under the frame's pose, and whether it has depth.
 int orbs_read_frame_glue(orbs_t* h, int frame, float* uright, float* depth, float* xw, uint8_t* valid, int cap) {
-  if (!h || !h->have || frame < 0 || cap < h->cap) { set_error("bad argument"); return B200ORB_EINVAL; }
+  B200_CHECK(check_last(h, frame, ANY_BATCH));
+  if (cap < h->last.cap) { set_error("cap %d < the last batch's keypoint capacity %d", cap, h->last.cap); return B200ORB_EINVAL; }
   DeviceGuard g(h->device);
-  const size_t o = (size_t)frame * h->cap, n = (size_t)h->cap;
+  const size_t o = (size_t)frame * h->last.cap, n = (size_t)h->last.cap;
   cudaStream_t st = h->ex->stream;
   if (uright) B200_CUDA(cudaMemcpyAsync(uright, h->d_ur + o, 4 * n, cudaMemcpyDeviceToHost, st));
   if (depth) B200_CUDA(cudaMemcpyAsync(depth, h->d_dep + o, 4 * n, cudaMemcpyDeviceToHost, st));
@@ -751,21 +760,21 @@ static int download(orbs_t* h, const OrbsResults* out, size_t F) {
 
 int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
   if (!h || !b || !batch_form_ok(b, out)) { set_error("bad argument"); return B200ORB_EINVAL; }
+  // Every refusal comes before the first state change.
   const int F = b->nframes, rows = b->rows, cols = b->cols;
   const bool masked = b->flow || b->device_flow;
   if (masked) B200_CHECK(h->check_masked(rows, cols));
   FbGeom fg;
   if (b->device_flow) B200_CHECK(fb_geometry(rows / 2, cols / 2, &fg));
-  if (b->homography) {   // TrackHomo's pairs go to findHomography, which takes at most HF_MAX_PAIRS
-    int kcap = 0;
-    B200_CHECK(orbx_max_keypoints_for(h->ex.get(), rows, cols, &kcap));
-    if (kcap > HF_MAX_PAIRS) {
-      set_error("homography batches take at most %d keypoints per frame (findHomography's pairs), not %d", HF_MAX_PAIRS, kcap);
-      return B200ORB_EINVAL;
-    }
+  int kcap = 0;   // the keypoint capacity ensure() gives the handle for this image size
+  B200_CHECK(orbx_max_keypoints_for(h->ex.get(), rows, cols, &kcap));
+  if (b->homography && kcap > HF_MAX_PAIRS) {   // TrackHomo's pairs go to findHomography, which takes at most HF_MAX_PAIRS
+    set_error("homography batches take at most %d keypoints per frame (findHomography's pairs), not %d", HF_MAX_PAIRS, kcap);
+    return B200ORB_EINVAL;
   }
   const bool cont = h->cont.pending;
-  if (cont) B200_CHECK(h->check_continue(b));
+  if (cont) B200_CHECK(h->check_continue(b, kcap));
+  if (out && out->cap < kcap) { set_error("cap %d < required %d (orbx_max_keypoints)", out->cap, kcap); return B200ORB_ECAP; }
   DeviceGuard g(h->device);
   // The only CV_16U depth pixels the tracking path ever reads are the ones under the keypoints
   // (Frame::ComputeStereoFromRGBD); k_depth_prefetch fetches them as soon as a chunk's keypoints are selected.
@@ -782,13 +791,13 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
       cudaGetLastError();
   }
   const int depth_bytes = b->device ? -1 : b->depth ? 4 : (d16_alias ? 0 : 2);   // per pixel uploaded
+  // From here on a failure leaves the handle with no batch: its buffers may have been replaced or partly written.
+  h->last = BatchRecord{};
   B200_CHECK(h->ensure(rows, cols, F, depth_bytes));
-  if (out && out->cap < h->cap) { set_error("cap %d < required %d (orbx_max_keypoints)", out->cap, h->cap); return B200ORB_ECAP; }
   if (masked) B200_CHECK(h->ensure_dyn(b->flow && !b->device, b->device_flow ? &fg : nullptr));
   if (b->homography) B200_CHECK(h->ensure_homo());
-  h->homo_F = 0;
   // The continuation is consumed by this batch; its frames take sequence positions s .. s + F - 1.
-  const int s = cont ? h->cont.seq : 0;
+  const int s = cont ? h->cont.from.seq_end : 0;
   h->cont.pending = false;
   // Device batch: every input is read in place from HBM.  Host batch: from the uploaded copies.
   const float *dd = b->depth, *dflow = b->flow, *dT = b->Tcw;
@@ -814,25 +823,22 @@ int orbs_submit(orbs_t* h, const OrbsBatch* b, const OrbsResults* out) {
                           &h->launches));
     if (masked) B200_CHECK(h->mask_filter(dflow, b->binary_threshold, kpd16, 0, F));
   }
-  B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, masked, cont));
+  B200_CHECK(h->run(dd, kpd16, b->depth_factor, dT, F, cont));
   if (cont) B200_CUDA(cudaEventRecord(h->carry_free_ev, st));   // the last read of the carry
-  h->last_variant = batch_variant(b);
-  h->seq_end = std::min(2, s + F);
-  h->last_dT = b->device ? b->Tcw : nullptr;
-  if (b->device) return B200ORB_OK;
-  B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
-  return download(h, out, F);
+  if (!b->device) {
+    B200_CUDA(cudaEventRecord(h->compute_done_ev, st));
+    B200_CHECK(download(h, out, F));
+  }
+  h->last = BatchRecord{F, rows, cols, kcap, batch_variant(b), std::min(2, s + F), b->device ? b->Tcw : nullptr, h->prm};
+  return B200ORB_OK;
 }
 
 // The dynamic mask of frame `frame` of the last batch, if that batch was masked: FrameDrawer's mDynMask
 // (perfect/src/FrameDrawer.cc:262), unpacked to one byte per pixel, and whether the 65 % rule filtered the frame.
 int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered) {
-  if (!h || frame < 0 || frame >= h->mask_F) {
-    set_error(h && !h->mask_F ? "the last batch was not masked" : "bad argument");
-    return B200ORB_EINVAL;
-  }
+  B200_CHECK(check_last(h, frame, MASKED_BATCH));
   DeviceGuard g(h->device);
-  const int rows = h->rows, cols = h->cols, nw = dynp_words(cols);
+  const int rows = h->last.rows, cols = h->last.cols, nw = dynp_words(cols);
   std::vector<uint32_t> words((size_t)rows * nw);
   unsigned sum = 0;
   cudaStream_t st = h->ex->stream;
@@ -848,10 +854,7 @@ int orbs_read_dynamic_mask(orbs_t* h, int frame, uint8_t* mask, int* filtered) {
 
 // What TrackHomo did for frame `frame` of the last batch, if that batch was a homography batch.
 int orbs_read_homography(orbs_t* h, int frame, double H[9], int* branch, int* nmatches, int* npairs) {
-  if (!h || frame < 0 || frame >= h->homo_F) {
-    set_error(h && !h->homo_F ? "the last batch was not a homography batch" : "bad argument");
-    return B200ORB_EINVAL;
-  }
+  B200_CHECK(check_last(h, frame, HOMO_BATCH));
   DeviceGuard g(h->device);
   int st[HC_WORDS];
   double out[10];
@@ -888,19 +891,20 @@ int orbs_chain_after(orbs_t* h, orbs_t* prev) {
 // stream, behind that batch and before anything submitted to prev later.  The copy waits for h's last batch that read the
 // carry and for a continuation still pending on h; h's next batch waits for the copy.
 int orbs_continue(orbs_t* h, orbs_t* prev) {
-  if (!h || !prev || !prev->have || h->device != prev->device) { set_error("bad argument"); return B200ORB_EINVAL; }
+  if (!h || !prev || h->device != prev->device) { set_error("bad argument"); return B200ORB_EINVAL; }
+  B200_CHECK(check_last(prev, 0, ANY_BATCH));
   DeviceGuard g(h->device);
-  const bool img = prev->last_variant == BV_DEVICE_FLOW || prev->last_variant == BV_HOMOGRAPHY;
-  B200_CHECK(h->ensure_carry(prev->rows, prev->cols, prev->cap, img));
+  const BatchRecord& p = prev->last;
+  const bool img = p.variant == BV_DEVICE_FLOW || p.variant == BV_HOMOGRAPHY;
+  B200_CHECK(h->ensure_carry(p.rows, p.cols, p.cap, img));
   cudaStream_t ps = prev->ex->stream;
   B200_CUDA(cudaStreamWaitEvent(ps, h->carry_free_ev, 0));
   if (h->cont.pending) B200_CUDA(cudaStreamWaitEvent(ps, h->carry_ev, 0));
-  const int f = prev->lastF - 1;
-  const size_t o = (size_t)f * prev->cap, px = (size_t)prev->rows * prev->cols;
+  const int f = p.F - 1;
+  const size_t o = (size_t)f * p.cap, px = (size_t)p.rows * p.cols;
   const CarrySrc src{prev->d_x + o, prev->d_y + o, prev->d_ang + o, prev->d_xw + 3 * o, prev->d_oct + o, prev->d_valid + o,
-                     prev->ex->d_desc + 32 * o, prev->ex->d_n + f,
-                     prev->last_dT ? prev->last_dT + 16 * (size_t)f : prev->d_T + 16 * (size_t)f};
-  const bool homo = prev->last_variant == BV_HOMOGRAPHY;
+                     prev->ex->d_desc + 32 * o, prev->ex->d_n + f, (p.dT ? p.dT : prev->d_T) + 16 * (size_t)f};
+  const bool homo = p.variant == BV_HOMOGRAPHY;
   k_carry_gather<<<dim3(CARRY_CTAS, img ? 2 : 1), 256, 0, ps>>>(
       src, img ? prev->d_gray + f * px : nullptr, homo ? prev->d_dest : nullptr,
       homo ? prev->d_hstate + f * HC_WORDS + HC_WARP : nullptr, px, h->cy);
@@ -908,12 +912,7 @@ int orbs_continue(orbs_t* h, orbs_t* prev) {
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaEventRecord(h->carry_ev, ps));
   h->cont.pending = true;
-  h->cont.variant = prev->last_variant;
-  h->cont.seq = prev->seq_end;
-  h->cont.rows = prev->rows;
-  h->cont.cols = prev->cols;
-  h->cont.cap = prev->cap;
-  h->cont.prm = prev->prm;
+  h->cont.from = p;
   return B200ORB_OK;
 }
 
