@@ -262,12 +262,15 @@ class CvRNG:
 
 
 def _collinear(P) -> bool:
-    """haveCollinearPoints: the last point against every pair of the earlier ones (and near-coincident points)."""
+    """haveCollinearPoints: the last point against every pair of the earlier ones (and near-coincident points).  Each
+    difference is taken in float, as OpenCV's Point2f subtraction does, and widened to double; the products, the sums
+    and the comparison are double."""
+    P = np.asarray(P, np.float32)
     i = len(P) - 1
     for j in range(i):
-        dx1, dy1 = float(P[j][0]) - float(P[i][0]), float(P[j][1]) - float(P[i][1])
+        dx1, dy1 = float(P[j][0] - P[i][0]), float(P[j][1] - P[i][1])
         for k in range(j):
-            dx2, dy2 = float(P[k][0]) - float(P[i][0]), float(P[k][1]) - float(P[i][1])
+            dx2, dy2 = float(P[k][0] - P[i][0]), float(P[k][1] - P[i][1])
             if abs(dx2 * dy1 - dy2 * dx1) <= FLT_EPS * (abs(dx1) + abs(dy1) + abs(dx2) + abs(dy2)):
                 return True
     return False

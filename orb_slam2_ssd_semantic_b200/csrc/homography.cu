@@ -238,12 +238,14 @@ __device__ __forceinline__ float hf_error(const float* Hf, float2 M, float2 m) {
 
 // ---- RANSAC ------------------------------------------------------------------------------------------------------------
 
+// haveCollinearPoints of the last point: each difference is a float subtraction (Point2f - Point2f) widened to double,
+// the products, sums and the comparison are double
 __device__ bool hf_collinear(const float2* P) {
   const int i = 3;
   for (int j = 0; j < i; ++j) {
-    const double dx1 = (double)P[j].x - (double)P[i].x, dy1 = (double)P[j].y - (double)P[i].y;
+    const double dx1 = (double)(P[j].x - P[i].x), dy1 = (double)(P[j].y - P[i].y);
     for (int k = 0; k < j; ++k) {
-      const double dx2 = (double)P[k].x - (double)P[i].x, dy2 = (double)P[k].y - (double)P[i].y;
+      const double dx2 = (double)(P[k].x - P[i].x), dy2 = (double)(P[k].y - P[i].y);
       if (fabs(dx2 * dy1 - dy2 * dx1) <= HF_FLT_EPS * (fabs(dx1) + fabs(dy1) + fabs(dx2) + fabs(dy2))) return true;
     }
   }
@@ -426,13 +428,12 @@ __device__ void hf_normal_equations(const double* __restrict__ J, const double* 
   }
 }
 
-// Mat::dot of two 9-vectors (dotProd_64f)
+// Mat::dot of two 9-vectors (dotProd_64f at baseline: dotProd_'s loop unrolled by 4, then the tail in order)
 __device__ double hf_dot9(const double* a, const double* b) {
-  double l0 = 0.0, l1 = 0.0;
-  for (int i = 0; i < 8; i += 2) { l0 += a[i] * b[i]; l1 += a[i + 1] * b[i + 1]; }
-  double tail = 0.0;
-  tail += a[8] * b[8];
-  return (0.0 + (l0 + l1)) + tail;
+  double r = 0.0;
+  for (int i = 0; i < 8; i += 4) r += ((a[i] * b[i] + a[i + 1] * b[i + 1]) + a[i + 2] * b[i + 2]) + a[i + 3] * b[i + 3];
+  r += a[8] * b[8];
+  return r;
 }
 
 // SVBkSb's basis of the symmetric R.K.jac.A: Jacobi, then the threshold 2 DBL_EPSILON times the sequential sum of W

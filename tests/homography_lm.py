@@ -20,8 +20,8 @@ code, which still runs SSE2 universal intrinsics (tests/test_homography_lm_cpu.p
   norm_l2sqr(r)         NormL2_SIMD<double>: four v_float64x2 accumulators over blocks of 8, each reduced across the
                         accumulators then the lanes, the tail added in order
   norm_inf(r)           the largest magnitude (no rounding)
-  dot(a, b)             dotProd_64f: one v_float64x2 accumulator over blocks of 4, reduced across its lanes, then the
-                        remaining elements in order
+  dot(a, b)             dotProd_64f: a running sum, each block of 4 products summed left to right and added to it,
+                        then the remaining products in order
   solve_eig(A, b)       solve(A, b, x, DECOMP_EIG) and invert(A, X, DECOMP_EIG): the Jacobi eigen-decomposition of
   invert_eig(A)           oracle/homography_py.eigen_sym, then SVBkSb: eigenvalues at most 2 DBL_EPSILON times their
                         (signed, sequential) sum are dropped, every kept eigenpair adds into x (or X) in order
@@ -109,14 +109,18 @@ def norm_inf(r) -> float:
 
 
 def dot(a, b) -> float:
-    """Mat::dot of two double vectors (dotProd_64f): lanes l0 over a[4j] b[4j], a[4j+2] b[4j+2] and l1 over the odd
-    ones, r = 0 + (l0 + l1), then the remaining elements summed in order from 0 and added to r."""
+    """Mat::dot of two double vectors (dotProd_64f at baseline dispatch, dotProd_ unrolled by 4): r = 0, then
+    r += ((p0 + p1) + p2) + p3 per block of four products, then the remaining products added to r in order."""
     a = np.asarray(a, np.float64).ravel()
     b = np.asarray(b, np.float64).ravel()
     n4 = len(a) // 4 * 4
     p = a * b
-    lanes = (_seq(p[0:n4:2]), _seq(p[1:n4:2]))
-    return (0.0 + (lanes[0] + lanes[1])) + _seq(p[n4:])
+    r = 0.0
+    for i in range(0, n4, 4):
+        r += ((p[i] + p[i + 1]) + p[i + 2]) + p[i + 3]
+    for i in range(n4, len(p)):
+        r += p[i]
+    return float(r)
 
 
 def _svbksb_basis(A):
