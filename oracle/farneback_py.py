@@ -354,8 +354,10 @@ def vertical_sums(M: np.ndarray, winsize: int = WINSIZE) -> np.ndarray:
     return out.reshape(H, W, 5)
 
 
-def horizontal_solve(V: np.ndarray, winsize: int = WINSIZE) -> np.ndarray:
-    """Running row sums over the column sums (replicated borders, sequential in x) and the 2x2 solve per pixel."""
+def horizontal_solve(V: np.ndarray, winsize: int = WINSIZE, counts: dict | None = None) -> np.ndarray:
+    """Running row sums over the column sums (replicated borders, sequential in x) and the 2x2 solve per pixel.
+    `counts` (a dict) accumulates how many solves had det = g11*g22 - g12^2 below 1e-3 with h != 0 ("det_small") and
+    exactly 0 ("det_zero")."""
     H, W = V.shape[:2]
     m = winsize // 2
     scale = 1.0 / (winsize * winsize)
@@ -368,6 +370,10 @@ def horizontal_solve(V: np.ndarray, winsize: int = WINSIZE) -> np.ndarray:
     for x in range(W):
         acc = acc + (Vp[:, x + 2 * m + 1] - Vp[:, x])
         g11, g12, g22, h1, h2 = (acc[:, c] * scale for c in range(5))
+        if counts is not None:
+            det = g11 * g22 - g12 * g12
+            counts["det_small"] = counts.get("det_small", 0) + int(((det < 1e-3) & ((h1 != 0) | (h2 != 0))).sum())
+            counts["det_zero"] = counts.get("det_zero", 0) + int((det == 0).sum())
         idet = 1.0 / (g11 * g22 - g12 * g12 + 1e-3)
         flow[:, x, 0] = ((g11 * h2 - g12 * h1) * idet).astype(F32)
         flow[:, x, 1] = ((g22 * h1 - g12 * h2) * idet).astype(F32)
